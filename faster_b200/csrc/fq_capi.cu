@@ -50,30 +50,37 @@ void fq_fill_plan_args(const FqPlanDev& pd, FqKernelArgs* a)
   a->TZ = pd.TZ; a->T0 = pd.T0; a->FT = pd.FT;
 }
 
-namespace
+const char* fq_scan_corridors(int n_prob, const int* poly_ofs, const int* face_ofs, FqCorridorSizes* sizes)
 {
-inline int fail(fq_ctx* c, int code, const std::string& msg) { return fq_fail(c, code, msg); }
-inline size_t align16(size_t x) { return fq_align16(x); }
-inline bool all_finite(const double* p, size_t n) { return fq_scan_all_finite(p, n); }
-inline bool all_positive_finite(const double* p, size_t n) { return fq_scan_all_positive_finite(p, n); }
-typedef FqPlanDev PlanDev;
-inline int get_plan(fq_ctx* ctx, int N, int force_final, PlanDev** out) { return fq_get_plan(ctx, N, force_final, out); }
-inline void fill_plan_args(const PlanDev& pd, FqKernelArgs* a) { fq_fill_plan_args(pd, a); }
-const int kCounterSlots = kFqCounterSlots;
-}  // namespace
+  *sizes = FqCorridorSizes();
+  for (int j = 0; j < n_prob; j++)
+  {
+    const int P = poly_ofs[j + 1] - poly_ofs[j];
+    if (P < 0 || P > FQ_MAX_POLY) return "polytope count out of range (0..FQ_MAX_POLY)";
+    for (int p = poly_ofs[j]; p < poly_ofs[j + 1]; p++)
+    {
+      if (face_ofs[p + 1] < face_ofs[p]) return "face_ofs not monotone";
+      sizes->max_poly_faces = std::max(sizes->max_poly_faces, face_ofs[p + 1] - face_ofs[p]);
+    }
+    sizes->max_faces = std::max(sizes->max_faces, face_ofs[poly_ofs[j + 1]] - face_ofs[poly_ofs[j]]);
+  }
+  sizes->n_poly = poly_ofs[n_prob];
+  sizes->n_face = face_ofs[sizes->n_poly];
+  return nullptr;
+}
 
 extern "C" int fq_create(fq_ctx** out, int device)
 {
-  if (!out) return fail(nullptr, FQ_E_ARG, "out is NULL");
+  if (!out) return fq_fail(nullptr, FQ_E_ARG, "out is NULL");
   *out = nullptr;
   int n = 0;
   cudaError_t e = cudaGetDeviceCount(&n);
   if (e != cudaSuccess || n <= 0)
-    return fail(nullptr, FQ_E_NOGPU, std::string("no CUDA device: ") + (e != cudaSuccess ? cudaGetErrorString(e) : "count 0") +
-                                         " (faster_b200 has no CPU fallback)");
-  if (device < 0 || device >= n) return fail(nullptr, FQ_E_ARG, "device index out of range");
+    return fq_fail(nullptr, FQ_E_NOGPU, std::string("no CUDA device: ") + (e != cudaSuccess ? cudaGetErrorString(e) : "count 0") +
+                                            " (faster_b200 has no CPU fallback)");
+  if (device < 0 || device >= n) return fq_fail(nullptr, FQ_E_ARG, "device index out of range");
   fq_ctx* ctx = new (std::nothrow) fq_ctx();
-  if (!ctx) return fail(nullptr, FQ_E_NOMEM, "out of host memory");
+  if (!ctx) return fq_fail(nullptr, FQ_E_NOMEM, "out of host memory");
   ctx->device = device;
   e = cudaSetDevice(device);
   if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking);
@@ -81,12 +88,12 @@ extern "C" int fq_create(fq_ctx** out, int device)
   if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->ev_head, cudaEventDisableTiming);
   if (e == cudaSuccess) e = cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device);
   ctx->counters_cap = 4096;
-  if (e == cudaSuccess) e = cudaMalloc(&ctx->d_counters, sizeof(int) * (size_t)kCounterSlots * ctx->counters_cap);
+  if (e == cudaSuccess) e = cudaMalloc(&ctx->d_counters, sizeof(int) * (size_t)kFqCounterSlots * ctx->counters_cap);
   if (e != cudaSuccess)
   {
     std::string msg = std::string("cuda init: ") + cudaGetErrorString(e);
     delete ctx;
-    return fail(nullptr, FQ_E_CUDA, msg);
+    return fq_fail(nullptr, FQ_E_CUDA, msg);
   }
   *out = ctx;
   return 0;
@@ -123,11 +130,11 @@ extern "C" int fq_set_option(fq_ctx* ctx, const char* key, int value)
   if (std::string(key) == "sweep_early_exit") { ctx->early_exit = value != 0; return 0; }
   if (std::string(key) == "row_tol_1e9")
   { // row tolerance in units of 1e-9 (10 = the default 1e-8, 1000 = Gurobi's default FeasibilityTol 1e-6); >= 0
-    if (value < 0 || value > 1000000) return fail(ctx, FQ_E_ARG, "row_tol_1e9 out of range (0..1000000)");
+    if (value < 0 || value > 1000000) return fq_fail(ctx, FQ_E_ARG, "row_tol_1e9 out of range (0..1000000)");
     ctx->row_tol = 1e-9 * (double)value;
     return 0;
   }
-  return fail(ctx, FQ_E_ARG, std::string("unknown option ") + key);
+  return fq_fail(ctx, FQ_E_ARG, std::string("unknown option ") + key);
 }
 
 extern "C" int fq_has_feature(const char* name)
@@ -141,25 +148,18 @@ extern "C" int fq_has_feature(const char* name)
 
 extern "C" const char* fq_last_error(const fq_ctx* ctx) { return ctx ? ctx->err.c_str() : g_create_error.c_str(); }
 
-// common launch: every pointer is a device pointer
-int fq_launch_solve_ctx(fq_ctx* ctx, int N, int force_final, int n_prob, const double* d_x0, const double* d_xf,
-                 const double* d_lim, const int* d_poly_ofs, const int* d_face_ofs, const double* d_Ab,
-                 const int* d_cand_ofs, int max_cand, int max_faces, int max_poly_faces, const double* d_dt,
-                 const uint8_t* d_sigma, uint8_t* d_feasible, double* d_cost, double* d_coeffs, int32_t* d_iters,
-                 cudaStream_t stream)
+int fq_launch_solve_ctx(fq_ctx* ctx, FqKernelArgs a, int max_cand, int max_poly_faces, cudaStream_t stream, bool* tail)
 {
-  PlanDev* pd = nullptr;
-  int rc = get_plan(ctx, N, force_final, &pd);
-  if (rc) return rc;
-  FqKernelArgs a;
-  fill_plan_args(*pd, &a);
-  a.n_prob = n_prob; a.x0 = d_x0; a.xf = d_xf; a.lim = d_lim; a.poly_ofs = d_poly_ofs; a.face_ofs = d_face_ofs;
-  a.Ab = d_Ab; a.max_faces = max_faces > 0 ? max_faces : 1;
-  a.item_cap = N * (max_poly_faces > 0 && max_poly_faces <= a.max_faces ? max_poly_faces : a.max_faces); a.cand_ofs = d_cand_ofs; a.dt = d_dt; a.sigma = d_sigma;
-  a.feasible = d_feasible; a.cost = d_cost; a.coeffs = d_coeffs; a.iters = d_iters; a.row_tol = ctx->row_tol;
+  if (tail) *tail = false;
+  FqPlanDev* pd = nullptr;
+  if (int rc = fq_get_plan(ctx, a.N, a.force_final, &pd)) return rc;
+  fq_fill_plan_args(*pd, &a);
+  if (a.max_faces <= 0) a.max_faces = 1;
+  a.item_cap = a.N * (max_poly_faces > 0 && max_poly_faces <= a.max_faces ? max_poly_faces : a.max_faces);
+  a.row_tol = ctx->row_tol;
   if (fq_solve_smem_bytes(a) > 227 * 1024)
-    return fail(ctx, FQ_E_ARG, "problem too large for shared memory (N / faces per problem)");
-  static const bool env_generic = std::getenv("FQ_KERNEL") && std::string(std::getenv("FQ_KERNEL")) == "generic";
+    return fq_fail(ctx, FQ_E_ARG, "problem too large for shared memory (N / faces per problem)");
+  const int n_prob = a.n_prob;
   if (n_prob > ctx->counters_cap)
   { // rare: grow the counter ring (needs the device idle because earlier launches may still use the old one)
     FQ_CUDA(cudaDeviceSynchronize());
@@ -167,16 +167,13 @@ int fq_launch_solve_ctx(fq_ctx* ctx, int N, int force_final, int n_prob, const d
     ctx->d_counters = nullptr;
     if (ctx->d_first) { cudaFree(ctx->d_first); ctx->d_first = nullptr; }
     ctx->counters_cap = n_prob + n_prob / 2;
-    FQ_CUDA(cudaMalloc(&ctx->d_counters, sizeof(int) * (size_t)kCounterSlots * ctx->counters_cap));
+    FQ_CUDA(cudaMalloc(&ctx->d_counters, sizeof(int) * (size_t)kFqCounterSlots * ctx->counters_cap));
   }
-  const unsigned slot = ctx->counters_pos++ % kCounterSlots;
+  const unsigned slot = ctx->counters_pos++ % kFqCounterSlots;
   int* counters = ctx->d_counters + (size_t)slot * ctx->counters_cap;
-  a.memo = nullptr; a.memo_salt = 0; a.cert = ctx->cert_out; a.cert_stride = ctx->cert_stride;
-  a.first_feasible = nullptr; a.sorted_dt = ctx->launch_sorted_dt ? 1 : 0; a.ee_width = ctx->launch_ee_width;
-  ctx->launch_sorted_dt = false; ctx->launch_ee_width = 0;
   if (ctx->early_exit && max_cand > 1)
   {
-    if (!ctx->d_first) FQ_CUDA(cudaMalloc(&ctx->d_first, sizeof(unsigned long long) * (size_t)kCounterSlots * ctx->counters_cap));
+    if (!ctx->d_first) FQ_CUDA(cudaMalloc(&ctx->d_first, sizeof(unsigned long long) * (size_t)kFqCounterSlots * ctx->counters_cap));
     a.first_feasible = ctx->d_first + (size_t)slot * ctx->counters_cap;
     FQ_CUDA(cudaMemsetAsync(a.first_feasible, 0xff, sizeof(unsigned long long) * (size_t)n_prob, stream));
   }
@@ -187,44 +184,28 @@ int fq_launch_solve_ctx(fq_ctx* ctx, int N, int force_final, int n_prob, const d
     const size_t per_slot = (size_t)kFqMemoProbs * FQ_MEMO_NB * FQ_MEMO_BE;
     if (!ctx->d_memo)
     {
-      FQ_CUDA(cudaMalloc(&ctx->d_memo, sizeof(FqMemoEntry) * per_slot * kCounterSlots));
-      FQ_CUDA(cudaMemset(ctx->d_memo, 0, sizeof(FqMemoEntry) * per_slot * kCounterSlots));
+      FQ_CUDA(cudaMalloc(&ctx->d_memo, sizeof(FqMemoEntry) * per_slot * kFqCounterSlots));
+      FQ_CUDA(cudaMemset(ctx->d_memo, 0, sizeof(FqMemoEntry) * per_slot * kFqCounterSlots));
     }
     if (++ctx->memo_salt == 0)
     { // 2^32 launches later: start over with a clean table
       FQ_CUDA(cudaDeviceSynchronize());
-      FQ_CUDA(cudaMemset(ctx->d_memo, 0, sizeof(FqMemoEntry) * per_slot * kCounterSlots));
+      FQ_CUDA(cudaMemset(ctx->d_memo, 0, sizeof(FqMemoEntry) * per_slot * kFqCounterSlots));
       ctx->memo_salt = 1;
     }
     a.memo = ctx->d_memo + per_slot * slot;
     a.memo_salt = ctx->memo_salt;
   }
 #endif
-  a.sweep_done = nullptr; a.sweep_n_sigma = 0; a.sweep_idx = nullptr; a.sweep_win = nullptr;
-  const bool generic = env_generic || ctx->force_generic || a.cert != nullptr;
-  if (ctx->launch_sweep_n_sigma > 0 && n_prob == 1 && d_coeffs && !generic)
-  {
-    a.sweep_done = counters + n_prob; a.sweep_n_sigma = ctx->launch_sweep_n_sigma;
-    a.sweep_idx = ctx->launch_sweep_idx; a.sweep_win = ctx->launch_sweep_win;
-  }
-  ctx->launch_sweep_n_sigma = 0;
+  const bool generic = ctx->force_generic || a.cert != nullptr;
+  // the selection in the tail needs the specialised kernel, one problem and the coefficients of every candidate
+  a.sweep_done = a.sweep_n_sigma > 0 && n_prob == 1 && a.coeffs && !generic ? counters + n_prob : nullptr;
+  if (!a.sweep_done) { a.sweep_n_sigma = 0; a.sweep_idx = nullptr; a.sweep_win = nullptr; }
   bool spec = false;
   FQ_CUDA(fq_launch_solve(a, max_cand, stream, counters, ctx->sm_count, generic, &spec));
-  ctx->last_launch_tail = spec && a.sweep_done != nullptr;
+  if (tail) *tail = spec && a.sweep_done != nullptr;
   return 0;
 }
-namespace
-{
-inline int launch_solve(fq_ctx* ctx, int N, int force_final, int n_prob, const double* d_x0, const double* d_xf,
-                        const double* d_lim, const int* d_poly_ofs, const int* d_face_ofs, const double* d_Ab,
-                        const int* d_cand_ofs, int max_cand, int max_faces, int max_poly_faces, const double* d_dt,
-                        const uint8_t* d_sigma, uint8_t* d_feasible, double* d_cost, double* d_coeffs, int32_t* d_iters,
-                        cudaStream_t stream)
-{
-  return fq_launch_solve_ctx(ctx, N, force_final, n_prob, d_x0, d_xf, d_lim, d_poly_ofs, d_face_ofs, d_Ab, d_cand_ofs, max_cand,
-                             max_faces, max_poly_faces, d_dt, d_sigma, d_feasible, d_cost, d_coeffs, d_iters, stream);
-}
-}  // namespace
 
 extern "C" int fq_solve_multi_dev(fq_ctx* ctx, int N, int force_final, int n_prob, const double* d_x0,
                                   const double* d_xf, const double* d_lim, const int* d_poly_ofs,
@@ -234,13 +215,16 @@ extern "C" int fq_solve_multi_dev(fq_ctx* ctx, int N, int force_final, int n_pro
                                   int32_t* d_iters, void* stream)
 {
   if (!ctx) return FQ_E_ARG;
-  if (n_prob < 0 || max_cand_per_prob < 0) return fail(ctx, FQ_E_ARG, "negative count");
+  if (n_prob < 0 || max_cand_per_prob < 0) return fq_fail(ctx, FQ_E_ARG, "negative count");
   if (n_prob == 0 || max_cand_per_prob == 0) return 0;
-  if (((uintptr_t)d_Ab & 15) != 0) return fail(ctx, FQ_E_ARG, "Ab must be 16-byte aligned");
+  if (((uintptr_t)d_Ab & 15) != 0) return fq_fail(ctx, FQ_E_ARG, "Ab must be 16-byte aligned");
   FQ_CUDA(cudaSetDevice(ctx->device));
-  return launch_solve(ctx, N, force_final, n_prob, d_x0, d_xf, d_lim, d_poly_ofs, d_face_ofs, d_Ab, d_cand_ofs,
-                      max_cand_per_prob, max_faces_per_prob, ctx->max_poly_faces_hint, d_dt, d_sigma, d_feasible, d_cost,
-                      d_coeffs, d_iters, stream ? (cudaStream_t)stream : ctx->stream);
+  FqKernelArgs a{};
+  a.N = N; a.force_final = force_final; a.n_prob = n_prob; a.x0 = d_x0; a.xf = d_xf; a.lim = d_lim;
+  a.poly_ofs = d_poly_ofs; a.face_ofs = d_face_ofs; a.Ab = d_Ab; a.max_faces = max_faces_per_prob;
+  a.cand_ofs = d_cand_ofs; a.dt = d_dt; a.sigma = d_sigma;
+  a.feasible = d_feasible; a.cost = d_cost; a.coeffs = d_coeffs; a.iters = d_iters;
+  return fq_launch_solve_ctx(ctx, a, max_cand_per_prob, ctx->max_poly_faces_hint, stream ? (cudaStream_t)stream : ctx->stream);
 }
 
 int fq_settle(fq_ctx* ctx)
@@ -254,10 +238,6 @@ int fq_settle(fq_ctx* ctx)
   FQ_CUDA(cudaStreamSynchronize(ctx->stream));
   return 0;
 }
-namespace
-{
-inline int settle(fq_ctx* ctx) { return fq_settle(ctx); }
-}  // namespace
 
 namespace
 {
@@ -270,45 +250,37 @@ struct HostLayout
 // validates the host description and computes sizes
 int describe(fq_ctx* ctx, int N, int force_final, int n_prob, const int* poly_ofs, const int* face_ofs,
              const int* cand_ofs, const uint8_t* sigma, bool want_coeffs, bool want_iters, HostLayout* L,
-             int* n_cand, int* n_poly, int* n_face, int* max_cand, int* max_faces, int* max_poly_faces)
+             FqCorridorSizes* cs, int* n_cand, int* max_cand)
 {
   const int ne = force_final ? 3 : 2;
-  if (N < ne || N > FQ_MAX_N) return fail(ctx, FQ_E_ARG, "N out of range");
-  if (n_prob <= 0) return fail(ctx, FQ_E_ARG, "n_prob <= 0");
-  if (poly_ofs[0] != 0 || cand_ofs[0] != 0 || face_ofs[0] != 0) return fail(ctx, FQ_E_ARG, "offset arrays must start at 0");
-  *max_cand = 0; *max_faces = 0; *max_poly_faces = 0;
+  if (N < ne || N > FQ_MAX_N) return fq_fail(ctx, FQ_E_ARG, "N out of range");
+  if (n_prob <= 0) return fq_fail(ctx, FQ_E_ARG, "n_prob <= 0");
+  if (poly_ofs[0] != 0 || cand_ofs[0] != 0 || face_ofs[0] != 0) return fq_fail(ctx, FQ_E_ARG, "offset arrays must start at 0");
+  if (const char* why = fq_scan_corridors(n_prob, poly_ofs, face_ofs, cs)) return fq_fail(ctx, FQ_E_ARG, why);
+  *max_cand = 0;
   for (int j = 0; j < n_prob; j++)
   {
     const int P = poly_ofs[j + 1] - poly_ofs[j], nc = cand_ofs[j + 1] - cand_ofs[j];
-    if (P < 0 || P > FQ_MAX_POLY) return fail(ctx, FQ_E_ARG, "polytope count out of range (0..FQ_MAX_POLY)");
-    if (nc < 0) return fail(ctx, FQ_E_ARG, "cand_ofs not monotone");
-    const int nf = face_ofs[poly_ofs[j + 1]] - face_ofs[poly_ofs[j]];
-    if (nf < 0) return fail(ctx, FQ_E_ARG, "face_ofs not monotone");
-    for (int p = poly_ofs[j]; p < poly_ofs[j + 1]; p++)
-    {
-      if (face_ofs[p + 1] < face_ofs[p]) return fail(ctx, FQ_E_ARG, "face_ofs not monotone");
-      if (face_ofs[p + 1] - face_ofs[p] > *max_poly_faces) *max_poly_faces = face_ofs[p + 1] - face_ofs[p];
-    }
+    if (nc < 0) return fq_fail(ctx, FQ_E_ARG, "cand_ofs not monotone");
     if (P > 0 && sigma)
     { // branch-free max over the bytes (vectorises); one compare per problem
       if (fq_scan_max_u8(sigma + (size_t)cand_ofs[j] * N, (size_t)nc * N) >= P)
-        return fail(ctx, FQ_E_ARG, "sigma entry >= number of polytopes");
+        return fq_fail(ctx, FQ_E_ARG, "sigma entry >= number of polytopes");
     }
     if (nc > *max_cand) *max_cand = nc;
-    if (nf > *max_faces) *max_faces = nf;
   }
-  *n_cand = cand_ofs[n_prob]; *n_poly = poly_ofs[n_prob]; *n_face = face_ofs[*n_poly];
+  *n_cand = cand_ofs[n_prob];
   size_t o = 0;
-  L->Ab = o;        o = align16(o + sizeof(double) * 4 * (size_t)(*n_face > 0 ? *n_face : 1));
+  L->Ab = o;        o = fq_align16(o + sizeof(double) * 4 * (size_t)(cs->n_face > 0 ? cs->n_face : 1));
   L->x0 = o;        o += sizeof(double) * 9 * (size_t)n_prob;
   L->xf = o;        o += sizeof(double) * 9 * (size_t)n_prob;
   L->lim = o;       o += sizeof(double) * 3 * (size_t)n_prob;
   L->poly_ofs = o;  o += sizeof(int) * (size_t)(n_prob + 1);
-  L->face_ofs = o;  o += sizeof(int) * (size_t)(*n_poly + 1);
-  L->cand_ofs = o;  o = align16(o + sizeof(int) * (size_t)(n_prob + 1));
+  L->face_ofs = o;  o += sizeof(int) * (size_t)(cs->n_poly + 1);
+  L->cand_ofs = o;  o = fq_align16(o + sizeof(int) * (size_t)(n_prob + 1));
   L->dt = o;        o += sizeof(double) * (size_t)*n_cand;      // per-candidate arrays last: [0, dt) is the
   L->sigma = o;     o += (size_t)*n_cand * N;                   // per-problem description
-  L->in_bytes = align16(o);
+  L->in_bytes = fq_align16(o);
   o = 0;
   L->cost = o;      o += sizeof(double) * (size_t)*n_cand;
   L->win_cost = o;  o += sizeof(double) * (size_t)n_prob;       // per-problem winners (fq_solve_multi_sharded)
@@ -318,15 +290,12 @@ int describe(fq_ctx* ctx, int N, int force_final, int n_prob, const int* poly_of
   L->win_idx = o;   o += sizeof(int) * (size_t)n_prob;
   L->win_ofs = o;   o += sizeof(int) * (size_t)(n_prob + 1);
   L->feasible = o;  o += (size_t)*n_cand;
-  L->out_bytes = align16(o);
+  L->out_bytes = fq_align16(o);
   return 0;
 }
 
 constexpr size_t kPackThreshold = 512 * 1024;   // below this, inputs are packed into one pinned staging copy
-}  // namespace
 
-namespace
-{
 struct Trace
 { // FQ_TRACE=1: host-side phase times of fq_solve_multi on stderr
   bool on;
@@ -340,52 +309,62 @@ struct Trace
     t0 = t1;
   }
 };
-}  // namespace
 
-namespace
-{
-// deferred: return once everything is enqueued (large batches only; small ones complete before returning either way)
+// deferred: return once everything is enqueued (large batches only; small ones complete before returning either way).
+// cert (device, cert_stride doubles per candidate): fq_solve_batch_cert's certificate buffer, or nullptr
 int solve_multi_impl(fq_ctx* ctx, int N, int force_final, int n_prob, const double* x0, const double* xf,
                      const double* lim, const int* poly_ofs, const int* face_ofs, const double* Ab,
                      const int* cand_ofs, const double* dt, const uint8_t* sigma, uint8_t* feasible,
-                     double* cost, double* coeffs, int32_t* iters, bool deferred, HostLayout* L_out = nullptr)
+                     double* cost, double* coeffs, int32_t* iters, bool deferred, HostLayout* L_out = nullptr,
+                     double* cert = nullptr, int cert_stride = 0)
 {
   if (!ctx) return FQ_E_ARG;
-  if (int src = settle(ctx)) return src;
+  if (int src = fq_settle(ctx)) return src;
   Trace tr;
   if (!x0 || !xf || !lim || !poly_ofs || !face_ofs || !cand_ofs || !dt || !feasible || !cost)
-    return fail(ctx, FQ_E_ARG, "NULL argument");
+    return fq_fail(ctx, FQ_E_ARG, "NULL argument");
   HostLayout L;
-  int n_cand, n_poly, n_face, max_cand, max_faces, max_poly_faces;
+  FqCorridorSizes cs;
+  int n_cand, max_cand;
   int rc = describe(ctx, N, force_final, n_prob, poly_ofs, face_ofs, cand_ofs, sigma, coeffs != nullptr,
-                    iters != nullptr, &L, &n_cand, &n_poly, &n_face, &max_cand, &max_faces, &max_poly_faces);
+                    iters != nullptr, &L, &cs, &n_cand, &max_cand);
   if (rc) return rc;
   if (L_out) *L_out = L;
   tr.mark("describe");
   if (n_cand == 0) return 0;
-  if (n_poly > 0 && (!Ab || !sigma)) return fail(ctx, FQ_E_ARG, "polytopes given but Ab or sigma is NULL");
+  const int n_poly = cs.n_poly;
+  if (n_poly > 0 && (!Ab || !sigma)) return fq_fail(ctx, FQ_E_ARG, "polytopes given but Ab or sigma is NULL");
   // value checks (the kernels also refuse non-finite data, but an argument error is the better answer).  Small batches:
   // before anything is enqueued.  Large batches: while the GPU already works on the data (see the throughput path).
   auto values_ok = [&]() -> const char* {
-    if (!all_finite(x0, 9 * (size_t)n_prob) || !all_finite(xf, 9 * (size_t)n_prob) || !all_finite(Ab, 4 * (size_t)n_face))
+    if (!fq_scan_all_finite(x0, 9 * (size_t)n_prob) || !fq_scan_all_finite(xf, 9 * (size_t)n_prob) ||
+        !fq_scan_all_finite(Ab, 4 * (size_t)cs.n_face))
       return "non-finite value in x0/xf/Ab";
-    if (!all_positive_finite(dt, (size_t)n_cand)) return "dt must be finite and > 0";
-    if (!all_positive_finite(lim, 3 * (size_t)n_prob)) return "limits must be finite and > 0";
+    if (!fq_scan_all_positive_finite(dt, (size_t)n_cand)) return "dt must be finite and > 0";
+    if (!fq_scan_all_positive_finite(lim, 3 * (size_t)n_prob)) return "limits must be finite and > 0";
     return nullptr;
   };
   const bool big = L.in_bytes > kPackThreshold;
   if (!big)
-    if (const char* why = values_ok()) return fail(ctx, FQ_E_ARG, why);
+    if (const char* why = values_ok()) return fq_fail(ctx, FQ_E_ARG, why);
   FQ_CUDA(cudaSetDevice(ctx->device));
   FQ_CUDA(ctx->d_in.reserve(L.in_bytes));
   FQ_CUDA(ctx->d_out.reserve(L.out_bytes));
   char* din = (char*)ctx->d_in.p;
   char* dout = (char*)ctx->d_out.p;
+  FqKernelArgs a{};      // the whole batch; a slice of it offsets the per-problem pointers
+  a.N = N; a.force_final = force_final; a.n_prob = n_prob;
+  a.x0 = (const double*)(din + L.x0); a.xf = (const double*)(din + L.xf); a.lim = (const double*)(din + L.lim);
+  a.poly_ofs = (const int*)(din + L.poly_ofs); a.face_ofs = (const int*)(din + L.face_ofs); a.Ab = (const double*)(din + L.Ab);
+  a.max_faces = cs.max_faces; a.cand_ofs = (const int*)(din + L.cand_ofs); a.dt = (const double*)(din + L.dt);
+  a.sigma = (const uint8_t*)(din + L.sigma); a.feasible = (uint8_t*)(dout + L.feasible); a.cost = (double*)(dout + L.cost);
+  a.coeffs = coeffs ? (double*)(dout + L.coeffs) : nullptr; a.iters = iters ? (int32_t*)(dout + L.iters) : nullptr;
+  a.cert = cert; a.cert_stride = cert_stride;
   cudaStream_t st = ctx->stream;
   const size_t sig_bytes = (size_t)n_cand * N;
   struct Piece { size_t off; const void* src; size_t bytes; };
   const Piece pieces[] = {
-    { L.Ab, Ab, sizeof(double) * 4 * (size_t)n_face }, { L.x0, x0, sizeof(double) * 9 * (size_t)n_prob },
+    { L.Ab, Ab, sizeof(double) * 4 * (size_t)cs.n_face }, { L.x0, x0, sizeof(double) * 9 * (size_t)n_prob },
     { L.xf, xf, sizeof(double) * 9 * (size_t)n_prob }, { L.lim, lim, sizeof(double) * 3 * (size_t)n_prob },
     { L.dt, dt, sizeof(double) * (size_t)n_cand },     { L.poly_ofs, poly_ofs, sizeof(int) * (size_t)(n_prob + 1) },
     { L.face_ofs, face_ofs, sizeof(int) * (size_t)(n_poly + 1) },
@@ -438,12 +417,10 @@ int solve_multi_impl(fq_ctx* ctx, int N, int force_final, int n_prob, const doub
           FQ_CUDA(cudaMemcpyAsync(din + L.sigma + c_lo * N, sigma + c_lo * N, c_n * N, cudaMemcpyHostToDevice, s2));
         else
           FQ_CUDA(cudaMemsetAsync(din + L.sigma + c_lo * N, 0, c_n * N, s2));
-        rc = launch_solve(ctx, N, force_final, p_hi - p_lo, (const double*)(din + L.x0) + 9 * (size_t)p_lo,
-                          (const double*)(din + L.xf) + 9 * (size_t)p_lo, (const double*)(din + L.lim) + 3 * (size_t)p_lo,
-                          (const int*)(din + L.poly_ofs) + p_lo, (const int*)(din + L.face_ofs), (const double*)(din + L.Ab),
-                          (const int*)(din + L.cand_ofs) + p_lo, mc, max_faces, max_poly_faces, (const double*)(din + L.dt),
-                          (const uint8_t*)(din + L.sigma), (uint8_t*)(dout + L.feasible), (double*)(dout + L.cost),
-                          coeffs ? (double*)(dout + L.coeffs) : nullptr, iters ? (int32_t*)(dout + L.iters) : nullptr, s2);
+        FqKernelArgs slice = a;
+        slice.n_prob = p_hi - p_lo; slice.x0 += 9 * (size_t)p_lo; slice.xf += 9 * (size_t)p_lo; slice.lim += 3 * (size_t)p_lo;
+        slice.poly_ofs += p_lo; slice.cand_ofs += p_lo;
+        rc = fq_launch_solve_ctx(ctx, slice, mc, cs.max_poly_faces, s2);
         if (rc) { cudaStreamSynchronize(st); cudaStreamSynchronize(ctx->stream2); return rc; }
         FQ_CUDA(cudaMemcpyAsync(cost + c_lo, dout + L.cost + sizeof(double) * c_lo, sizeof(double) * c_n, cudaMemcpyDeviceToHost, s2));
         FQ_CUDA(cudaMemcpyAsync(feasible + c_lo, dout + L.feasible + c_lo, c_n, cudaMemcpyDeviceToHost, s2));
@@ -462,16 +439,11 @@ int solve_multi_impl(fq_ctx* ctx, int N, int force_final, int n_prob, const doub
     FQ_CUDA(cudaStreamSynchronize(ctx->stream2));
     FQ_CUDA(cudaStreamSynchronize(st));
     tr.mark("wait");
-    if (why) return fail(ctx, FQ_E_ARG, why);      // outputs were written but are not to be trusted
+    if (why) return fq_fail(ctx, FQ_E_ARG, why);      // outputs were written but are not to be trusted
     return 0;
   }
   if (n_poly == 0) FQ_CUDA(cudaMemsetAsync(din + L.sigma, 0, sig_bytes, st));
-  rc = launch_solve(ctx, N, force_final, n_prob, (const double*)(din + L.x0), (const double*)(din + L.xf),
-                    (const double*)(din + L.lim), (const int*)(din + L.poly_ofs), (const int*)(din + L.face_ofs),
-                    (const double*)(din + L.Ab), (const int*)(din + L.cand_ofs), max_cand, max_faces, max_poly_faces,
-                    (const double*)(din + L.dt), (const uint8_t*)(din + L.sigma), (uint8_t*)(dout + L.feasible),
-                    (double*)(dout + L.cost), coeffs ? (double*)(dout + L.coeffs) : nullptr,
-                    iters ? (int32_t*)(dout + L.iters) : nullptr, st);
+  rc = fq_launch_solve_ctx(ctx, a, max_cand, cs.max_poly_faces, st);
   if (rc) return rc;
   if (L.out_bytes <= kPackThreshold)
   {
@@ -496,6 +468,17 @@ int solve_multi_impl(fq_ctx* ctx, int N, int force_final, int n_prob, const doub
   }
   return 0;
 }
+
+// fq_solve_batch's one problem as a multi-problem description (cert as in solve_multi_impl)
+int solve_batch_impl(fq_ctx* ctx, int N, int force_final, const double* x0, const double* xf, const double* lim, int P,
+                     const int* face_ofs, const double* Ab, int n_cand, const double* dt, const uint8_t* sigma,
+                     uint8_t* feasible, double* cost, double* coeffs, int32_t* iters, double* cert, int cert_stride)
+{
+  if (P < 0 || n_cand < 0) return fq_fail(ctx, FQ_E_ARG, "negative count");
+  const int poly_ofs[2] = { 0, P }, cand_ofs[2] = { 0, n_cand }, zero_face[1] = { 0 };
+  return solve_multi_impl(ctx, N, force_final, 1, x0, xf, lim, poly_ofs, P > 0 ? face_ofs : zero_face, Ab, cand_ofs, dt, sigma,
+                          feasible, cost, coeffs, iters, false, nullptr, cert, cert_stride);
+}
 }  // namespace
 
 extern "C" int fq_solve_multi(fq_ctx* ctx, int N, int force_final, int n_prob, const double* x0, const double* xf,
@@ -516,8 +499,6 @@ extern "C" int fq_solve_multi_async(fq_ctx* ctx, int N, int force_final, int n_p
                           coeffs, iters, true);
 }
 
-// fq_solve_multi_async + the genNewTraj winner of every problem, selected on the device (the arrays stay in the context's
-// output arena until the next call): what the multi-GPU path all-gathers (fq_multi.cu)
 int fq_solve_multi_host_ex(fq_ctx* ctx, int N, int force_final, int n_prob, const double* x0, const double* xf, const double* lim,
                            const int* poly_ofs, const int* face_ofs, const double* Ab, const int* cand_ofs, const double* dt,
                            const uint8_t* sigma, uint8_t* feasible, double* cost, double* coeffs, int32_t* iters, bool deferred,
@@ -527,7 +508,7 @@ int fq_solve_multi_host_ex(fq_ctx* ctx, int N, int force_final, int n_prob, cons
   int rc = solve_multi_impl(ctx, N, force_final, n_prob, x0, xf, lim, poly_ofs, face_ofs, Ab, cand_ofs, dt, sigma, feasible, cost,
                             coeffs, iters, true, &L);
   if (rc) return rc;
-  if (cand_ofs[n_prob] == 0) return fail(ctx, FQ_E_ARG, "no candidates");
+  if (cand_ofs[n_prob] == 0) return fq_fail(ctx, FQ_E_ARG, "no candidates");
   FQ_CUDA(cudaSetDevice(ctx->device));
   // slices of a large batch alternate between the two streams: join before selecting
   FQ_CUDA(cudaEventRecord(ctx->ev_head, ctx->stream2));
@@ -543,7 +524,7 @@ int fq_solve_multi_host_ex(fq_ctx* ctx, int N, int force_final, int n_prob, cons
   if (d_win_idx) *d_win_idx = sa.win_idx;
   if (d_win_cost) *d_win_cost = sa.win_cost;
   ctx->pending = true;
-  if (!deferred) return settle(ctx);
+  if (!deferred) return fq_settle(ctx);
   return 0;
 }
 
@@ -552,7 +533,7 @@ extern "C" int fq_wait(fq_ctx* ctx)
   if (!ctx) return FQ_E_ARG;
   ctx->pending = true;          // also drains device-pointer launches made on the context's own stream
   for (fq_ctx* p : ctx->peers) p->pending = true;
-  return settle(ctx);
+  return fq_settle(ctx);
 }
 
 // fq_solve_batch through the size-generic kernel, which also exports, for every candidate it finds infeasible, the Farkas
@@ -568,9 +549,8 @@ extern "C" int fq_solve_batch_cert(fq_ctx* ctx, int N, int force_final, const do
   FqArena arena;
   FQ_CUDA(arena.reserve(sizeof(double) * (size_t)cert_stride * n_cand));
   FQ_CUDA(cudaMemset(arena.p, 0, sizeof(double) * (size_t)cert_stride * n_cand));
-  ctx->cert_out = (double*)arena.p; ctx->cert_stride = cert_stride;
-  const int rc = fq_solve_batch(ctx, N, force_final, x0, xf, lim, P, face_ofs, Ab, n_cand, dt, sigma, feasible, cost, nullptr, nullptr);
-  ctx->cert_out = nullptr; ctx->cert_stride = 0;
+  const int rc = solve_batch_impl(ctx, N, force_final, x0, xf, lim, P, face_ofs, Ab, n_cand, dt, sigma, feasible, cost, nullptr,
+                                  nullptr, (double*)arena.p, cert_stride);
   cudaError_t e = cudaMemcpy(cert, arena.p, sizeof(double) * (size_t)cert_stride * n_cand, cudaMemcpyDeviceToHost);
   arena.release();
   if (rc) return rc;
@@ -584,10 +564,8 @@ extern "C" int fq_solve_batch(fq_ctx* ctx, int N, int force_final, const double*
                               double* coeffs, int32_t* iters)
 {
   if (!ctx) return FQ_E_ARG;
-  if (P < 0 || n_cand < 0) return fail(ctx, FQ_E_ARG, "negative count");
-  const int poly_ofs[2] = { 0, P }, cand_ofs[2] = { 0, n_cand }, zero_face[1] = { 0 };
-  return fq_solve_multi(ctx, N, force_final, 1, x0, xf, lim, poly_ofs, P > 0 ? face_ofs : zero_face, Ab, cand_ofs, dt,
-                        sigma, feasible, cost, coeffs, iters);
+  return solve_batch_impl(ctx, N, force_final, x0, xf, lim, P, face_ofs, Ab, n_cand, dt, sigma, feasible, cost, coeffs, iters,
+                          nullptr, 0);
 }
 
 namespace
@@ -598,31 +576,30 @@ int gen_new_traj_impl(fq_ctx* ctx, int N, int force_final, const double* x0, con
                       int max_samples, double* samples, int* n_samples)
 {
   if (!ctx) return FQ_E_ARG;
-  if (int src = settle(ctx)) return src;
+  if (int src = fq_settle(ctx)) return src;
   Trace tr;
-  if (!x0 || !xf || !lim || !dts) return fail(ctx, FQ_E_ARG, "NULL argument");
-  if (P < 0 || P > FQ_MAX_POLY || n_dt <= 0) return fail(ctx, FQ_E_ARG, "bad P or n_dt");
+  if (!x0 || !xf || !lim || !dts) return fq_fail(ctx, FQ_E_ARG, "NULL argument");
+  if (P < 0 || P > FQ_MAX_POLY || n_dt <= 0) return fq_fail(ctx, FQ_E_ARG, "bad P or n_dt");
   if (P == 0) n_sigma = 1;
-  if (n_sigma <= 0 || (P > 0 && (!sigmas || !face_ofs || !Ab))) return fail(ctx, FQ_E_ARG, "bad sigma list / polytopes");
-  if (n_sigma > (1 << 20)) return fail(ctx, FQ_E_ARG, "n_sigma > 2^20");
+  if (n_sigma <= 0 || (P > 0 && (!sigmas || !face_ofs || !Ab))) return fq_fail(ctx, FQ_E_ARG, "bad sigma list / polytopes");
+  if (n_sigma > (1 << 20)) return fq_fail(ctx, FQ_E_ARG, "n_sigma > 2^20");
   const int ne = force_final ? 3 : 2;
-  if (N < ne || N > FQ_MAX_N) return fail(ctx, FQ_E_ARG, "N out of range");
-  if (!all_finite(x0, 9) || !all_finite(xf, 9) || !all_positive_finite(lim, 3) || !all_positive_finite(dts, (size_t)n_dt) ||
-      (P > 0 && !all_finite(Ab, 4 * (size_t)face_ofs[P])))
-    return fail(ctx, FQ_E_ARG, "non-finite input, dt <= 0 or limit <= 0");
+  if (N < ne || N > FQ_MAX_N) return fq_fail(ctx, FQ_E_ARG, "N out of range");
+  const int poly_ofs[2] = { 0, P }, zero_face[1] = { 0 };
+  FqCorridorSizes cs;
+  if (const char* why = fq_scan_corridors(1, poly_ofs, P > 0 ? face_ofs : zero_face, &cs)) return fq_fail(ctx, FQ_E_ARG, why);
+  const int n_face = cs.n_face;
+  if (!fq_scan_all_finite(x0, 9) || !fq_scan_all_finite(xf, 9) || !fq_scan_all_positive_finite(lim, 3) ||
+      !fq_scan_all_positive_finite(dts, (size_t)n_dt) || (P > 0 && !fq_scan_all_finite(Ab, 4 * (size_t)n_face)))
+    return fq_fail(ctx, FQ_E_ARG, "non-finite input, dt <= 0 or limit <= 0");
   const long long n_cand_ll = (long long)n_dt * n_sigma;
-  if (n_cand_ll > (1LL << 30)) return fail(ctx, FQ_E_ARG, "too many candidates");
+  if (n_cand_ll > (1LL << 30)) return fq_fail(ctx, FQ_E_ARG, "too many candidates");
   const int n_cand = (int)n_cand_ll;
-  const int n_face = P > 0 ? face_ofs[P] : 0;
-  int max_pf = 0;
-  for (int p = 0; p < P; p++) max_pf = std::max(max_pf, face_ofs[p + 1] - face_ofs[p]);
-  if (P > 0)
-    for (size_t i = 0; i < (size_t)n_sigma * N; i++)
-      if (sigmas[i] >= P) return fail(ctx, FQ_E_ARG, "sigma entry >= number of polytopes");
+  if (P > 0 && fq_scan_max_u8(sigmas, (size_t)n_sigma * N) >= P) return fq_fail(ctx, FQ_E_ARG, "sigma entry >= number of polytopes");
   FQ_CUDA(cudaSetDevice(ctx->device));
   // ---- pack the (small) problem description; the dt x sigma grid is expanded on the host side of the copy
   size_t o = 0;
-  const size_t oAb = o;   o = align16(o + sizeof(double) * 4 * (size_t)(n_face > 0 ? n_face : 1));
+  const size_t oAb = o;   o = fq_align16(o + sizeof(double) * 4 * (size_t)(n_face > 0 ? n_face : 1));
   const size_t ox0 = o;   o += sizeof(double) * 9;
   const size_t oxf = o;   o += sizeof(double) * 9;
   const size_t olim = o;  o += sizeof(double) * 3;
@@ -630,9 +607,9 @@ int gen_new_traj_impl(fq_ctx* ctx, int N, int force_final, const double* x0, con
   const size_t opo = o;   o += sizeof(int) * 2;
   const size_t ofo = o;   o += sizeof(int) * (size_t)(P + 1);
   const size_t oco = o;   o += sizeof(int) * 2;
-  const size_t osig = o;  o = align16(o + (size_t)n_cand * N);
+  const size_t osig = o;  o = fq_align16(o + (size_t)n_cand * N);
   const size_t odts = o;  o += sizeof(double) * (size_t)n_dt;      // the n_dt distinct time allocations (for fillX)
-  const size_t in_bytes = align16(o);
+  const size_t in_bytes = fq_align16(o);
   o = 0;
   const size_t ocost = o;   o += sizeof(double) * (size_t)n_cand;
   const size_t ocoef = o;   o += sizeof(double) * 12 * (size_t)N * n_cand;
@@ -641,7 +618,7 @@ int gen_new_traj_impl(fq_ctx* ctx, int N, int force_final, const double* x0, con
   const size_t onsamp = o;  o += sizeof(int) * 2;
   const size_t osamp = o;   o += samples ? sizeof(double) * 12 * (size_t)max_samples : 0;
   const size_t ofeas = o;   o += (size_t)n_cand;
-  const size_t out_bytes = align16(o);
+  const size_t out_bytes = fq_align16(o);
   FQ_CUDA(ctx->d_in.reserve(in_bytes));
   FQ_CUDA(ctx->d_out.reserve(out_bytes));
   FQ_CUDA(ctx->h_in.reserve(in_bytes));
@@ -677,11 +654,16 @@ int gen_new_traj_impl(fq_ctx* ctx, int N, int force_final, const double* x0, con
   if (tr.on) cudaEventRecord(tev[0], st);
   FQ_CUDA(cudaMemcpyAsync(din, hi, in_bytes, cudaMemcpyHostToDevice, st));
   if (tr.on) cudaEventRecord(tev[1], st);
-  {
-    bool asc = true;
-    for (int d = 1; d < n_dt; d++) asc = asc && dts[d] >= dts[d - 1];
-    ctx->launch_sorted_dt = asc; ctx->launch_ee_width = asc ? n_sigma : 0;
-  }
+  FqKernelArgs a{};
+  a.N = N; a.force_final = force_final; a.n_prob = 1;
+  a.x0 = (const double*)(din + ox0); a.xf = (const double*)(din + oxf); a.lim = (const double*)(din + olim);
+  a.poly_ofs = (const int*)(din + opo); a.face_ofs = (const int*)(din + ofo); a.Ab = (const double*)(din + oAb);
+  a.max_faces = n_face; a.cand_ofs = (const int*)(din + oco); a.dt = (const double*)(din + odt);
+  a.sigma = (const uint8_t*)(din + osig); a.feasible = (uint8_t*)(dout + ofeas); a.cost = (double*)(dout + ocost);
+  a.coeffs = (double*)(dout + ocoef);
+  a.sorted_dt = 1;
+  for (int d = 1; d < n_dt; d++) a.sorted_dt = a.sorted_dt && dts[d] >= dts[d - 1];
+  a.ee_width = a.sorted_dt ? n_sigma : 0;
   char* ho = (char*)ctx->h_out.p;
   const size_t win_bytes = sizeof(double) * (1 + 12 * (size_t)N);
   if (!samples)
@@ -690,19 +672,15 @@ int gen_new_traj_impl(fq_ctx* ctx, int N, int force_final, const double* x0, con
     void *dwin = nullptr;
     if (cudaHostGetDevicePointer(&dwin, ho, 0) == cudaSuccess)
     {
-      ctx->launch_sweep_n_sigma = n_sigma;
-      ctx->launch_sweep_win = (double*)dwin;
-      ctx->launch_sweep_idx = (int*)((char*)dwin + win_bytes);
+      a.sweep_n_sigma = n_sigma;
+      a.sweep_win = (double*)dwin;
+      a.sweep_idx = (int*)((char*)dwin + win_bytes);
       ((int*)(ho + win_bytes))[0] = -2;               // overwritten by the kernel
     }
   }
-  int rc = launch_solve(ctx, N, force_final, 1, (const double*)(din + ox0), (const double*)(din + oxf),
-                        (const double*)(din + olim), (const int*)(din + opo), (const int*)(din + ofo),
-                        (const double*)(din + oAb), (const int*)(din + oco), n_cand, n_face, max_pf,
-                        (const double*)(din + odt), (const uint8_t*)(din + osig), (uint8_t*)(dout + ofeas),
-                        (double*)(dout + ocost), (double*)(dout + ocoef), nullptr, st);
+  bool tail = false;
+  int rc = fq_launch_solve_ctx(ctx, a, n_cand, cs.max_poly_faces, st, &tail);
   if (rc) return rc;
-  const bool tail = ctx->last_launch_tail;
   if (tr.on) cudaEventRecord(tev[2], st);
   FqSelectArgs sa;
   sa.n_dt = n_dt; sa.n_sigma = n_sigma; sa.N = N;
@@ -738,7 +716,7 @@ int gen_new_traj_impl(fq_ctx* ctx, int N, int force_final, const double* x0, con
   static_assert(sizeof(double) == 8, "layout");
   const int* idx = (const int*)(ho + win_bytes);
   const double* win = (const double*)ho;
-  if (tail && idx[0] == -2) return fail(ctx, FQ_E_CUDA, "internal: the sweep finished without its selection");
+  if (tail && idx[0] == -2) return fq_fail(ctx, FQ_E_CUDA, "internal: the sweep finished without its selection");
   if (dt_index) *dt_index = idx[0];
   if (sigma_index) *sigma_index = idx[1];
   if (n_samples) *n_samples = 0;
@@ -771,7 +749,7 @@ extern "C" int fq_gen_new_traj_sampled(fq_ctx* ctx, int N, int force_final, cons
                                        double* coeffs, double* samples, int* n_samples)
 {
   if (!ctx) return FQ_E_ARG;
-  if (!samples || max_samples < 2 || !(DC > 0)) return fail(ctx, FQ_E_ARG, "samples buffer, max_samples >= 2 and DC > 0 required");
+  if (!samples || max_samples < 2 || !(DC > 0)) return fq_fail(ctx, FQ_E_ARG, "samples buffer, max_samples >= 2 and DC > 0 required");
   return gen_new_traj_impl(ctx, N, force_final, x0, xf, lim, P, face_ofs, Ab, n_dt, dts, n_sigma, sigmas, dt_index,
                            sigma_index, cost, coeffs, DC, max_samples, samples, n_samples);
 }
@@ -788,20 +766,21 @@ extern "C" int fq_gen_new_traj_exact(fq_ctx* ctx, int N, int force_final, const 
                                      long* nodes_out, int* exact_out)
 {
   if (!ctx) return FQ_E_ARG;
-  if (int src = settle(ctx)) return src;
-  if (!x0 || !xf || !lim || !dts || n_dt <= 0) return fail(ctx, FQ_E_ARG, "NULL argument or n_dt <= 0");
-  if (P < 0 || P > FQ_MAX_POLY) return fail(ctx, FQ_E_ARG, "bad P");
-  if (N < (force_final ? 3 : 2) || N > FQ_MAX_N) return fail(ctx, FQ_E_ARG, "N out of range");
+  if (int src = fq_settle(ctx)) return src;
+  if (!x0 || !xf || !lim || !dts || n_dt <= 0) return fq_fail(ctx, FQ_E_ARG, "NULL argument or n_dt <= 0");
+  if (P < 0 || P > FQ_MAX_POLY) return fq_fail(ctx, FQ_E_ARG, "bad P");
+  if (N < (force_final ? 3 : 2) || N > FQ_MAX_N) return fq_fail(ctx, FQ_E_ARG, "N out of range");
   if (nodes_out) *nodes_out = 0;
   if (exact_out) *exact_out = 1;
   if (sigma_out) std::memset(sigma_out, 0, (size_t)N);
   if (P == 0)
     return gen_new_traj_impl(ctx, N, force_final, x0, xf, lim, 0, face_ofs, Ab, n_dt, dts, 1, nullptr, dt_index, nullptr, cost,
                              coeffs, 0.0, 0, nullptr, nullptr);
-  if (!face_ofs || !Ab) return fail(ctx, FQ_E_ARG, "polytopes missing");
-  const int n_face = face_ofs[P];
-  int max_pf = 0;
-  for (int p = 0; p < P; p++) max_pf = std::max(max_pf, face_ofs[p + 1] - face_ofs[p]);
+  if (!face_ofs || !Ab) return fq_fail(ctx, FQ_E_ARG, "polytopes missing");
+  const int poly_ofs[2] = { 0, P };
+  FqCorridorSizes cs;
+  if (const char* why = fq_scan_corridors(1, poly_ofs, face_ofs, &cs)) return fq_fail(ctx, FQ_E_ARG, why);
+  const int n_face = cs.n_face;
   const size_t nb = fq_bnb_node_bytes(N, force_final);
   // ---- 1. non-decreasing assignments for every time allocation: the ordinary sweep (one launch + selection).  Its winner
   //         is the first monotone-feasible time allocation `fstar` with that allocation's best monotone cost; earlier
@@ -810,7 +789,7 @@ extern "C" int fq_gen_new_traj_exact(fq_ctx* ctx, int N, int force_final, const 
   long n_mono = 1;
   for (int i = 1; i <= N && n_mono <= (1L << 40); i++) n_mono = n_mono * (P - 1 + i) / i;
   if (n_mono <= 0 || n_mono > (1L << 20) || (long long)n_mono * n_dt > (1LL << 24))
-    return fail(ctx, FQ_E_ARG, "assignment list too long for the monotone pre-sweep (N, P, n_dt too large)");
+    return fq_fail(ctx, FQ_E_ARG, "assignment list too long for the monotone pre-sweep (N, P, n_dt too large)");
   std::vector<uint8_t> mono((size_t)n_mono * N);
   fq_monotone_sigmas(N, P, mono.data(), n_mono);
   int m_dt = -1, m_sig = -1;
@@ -832,7 +811,7 @@ extern "C" int fq_gen_new_traj_exact(fq_ctx* ctx, int N, int force_final, const 
     // ---- 2. device buffers
     const int cap = 65536, leaf_cap = 4096;
     size_t o = 0;
-    const size_t oAb = o;    o = align16(o + sizeof(double) * 4 * (size_t)n_face);
+    const size_t oAb = o;    o = fq_align16(o + sizeof(double) * 4 * (size_t)n_face);
     const size_t ox0 = o;    o += sizeof(double) * 9;
     const size_t oxf = o;    o += sizeof(double) * 9;
     const size_t olim = o;   o += sizeof(double) * 3;
@@ -841,11 +820,11 @@ extern "C" int fq_gen_new_traj_exact(fq_ctx* ctx, int N, int force_final, const 
     const size_t opo = o;    o += sizeof(int) * 2;
     const size_t ofo = o;    o += sizeof(int) * (size_t)(P + 1);
     const size_t oroot = o;  o += sizeof(int) * (size_t)n_dt;
-    const size_t ocnt = o;   o = align16(o + sizeof(int) * 8);   // [0] n_children [1] n_leaves [2..3] flags
+    const size_t ocnt = o;   o = fq_align16(o + sizeof(int) * 8);   // [0] n_children [1] n_leaves [2..3] flags
     const size_t head = o;
-    const size_t oleaf = o;  o = align16(o + 32 * (size_t)leaf_cap);
-    const size_t opoolA = o; o = align16(o + nb * (size_t)cap);
-    const size_t opoolB = o; o = align16(o + nb * (size_t)cap);
+    const size_t oleaf = o;  o = fq_align16(o + 32 * (size_t)leaf_cap);
+    const size_t opoolA = o; o = fq_align16(o + nb * (size_t)cap);
+    const size_t opoolB = o; o = fq_align16(o + nb * (size_t)cap);
     FQ_CUDA(cudaSetDevice(ctx->device));
     FQ_CUDA(ctx->d_bnb.reserve(o));
     FQ_CUDA(ctx->h_in.reserve(head));
@@ -904,16 +883,14 @@ extern "C" int fq_gen_new_traj_exact(fq_ctx* ctx, int N, int force_final, const 
     for (int p = 0; p <= P; p++) ((int*)(hi + ofo))[p] = face_ofs[p];
     cudaStream_t st = ctx->stream;
     FQ_CUDA(cudaMemcpyAsync(db, hi, head, cudaMemcpyHostToDevice, st));
-    PlanDev* pd = nullptr;
-    rc = get_plan(ctx, N, force_final, &pd);
+    FqPlanDev* pd = nullptr;
+    rc = fq_get_plan(ctx, N, force_final, &pd);
     if (rc) return rc;
-    FqBnbLevel L;
-    fill_plan_args(*pd, &L.k);
+    FqBnbLevel L{};
+    fq_fill_plan_args(*pd, &L.k);
     L.k.n_prob = 1; L.k.x0 = (const double*)(db + ox0); L.k.xf = (const double*)(db + oxf); L.k.lim = (const double*)(db + olim);
     L.k.poly_ofs = (const int*)(db + opo); L.k.face_ofs = (const int*)(db + ofo); L.k.Ab = (const double*)(db + oAb);
-    L.k.max_faces = n_face; L.k.item_cap = N * max_pf; L.k.cand_ofs = nullptr; L.k.dt = nullptr; L.k.sigma = nullptr;
-    L.k.feasible = nullptr; L.k.cost = nullptr; L.k.coeffs = nullptr; L.k.iters = nullptr; L.k.row_tol = ctx->row_tol;
-    L.k.memo = nullptr; L.k.memo_salt = 0; L.k.cert = nullptr; L.k.cert_stride = 0; L.k.first_feasible = nullptr; L.k.sorted_dt = 0; L.k.ee_width = 0; L.k.sweep_done = nullptr; L.k.sweep_n_sigma = 0; L.k.sweep_idx = nullptr; L.k.sweep_win = nullptr;
+    L.k.max_faces = n_face; L.k.item_cap = N * cs.max_poly_faces; L.k.row_tol = ctx->row_tol;
     L.n_dt = n_dt; L.P = P; L.dts = (const double*)(db + odts); L.roots = (const int*)(db + oroot);
     L.incumbent = (unsigned long long*)(db + oinc); L.leaves = db + oleaf; L.n_leaves = (int*)(db + ocnt) + 1;
     L.leaf_cap = leaf_cap; L.flags = (int*)(db + ocnt) + 2; L.n_children = (int*)(db + ocnt); L.cap = cap;
@@ -981,7 +958,7 @@ extern "C" int fq_gen_new_traj_exact(fq_ctx* ctx, int N, int force_final, const 
   std::vector<double> co((size_t)12 * N);
   rc = fq_solve_batch(ctx, N, force_final, x0, xf, lim, P, face_ofs, Ab, 1, &dts[win_dt], win_sigma.data(), &f1, &c1, co.data(), nullptr);
   if (rc) return rc;
-  if (!f1) return fail(ctx, FQ_E_CUDA, "internal: the winning assignment did not re-solve");
+  if (!f1) return fq_fail(ctx, FQ_E_CUDA, "internal: the winning assignment did not re-solve");
   if (cost) *cost = c1;
   if (coeffs) std::memcpy(coeffs, co.data(), sizeof(double) * 12 * (size_t)N);
   return 1;

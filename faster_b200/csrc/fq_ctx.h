@@ -73,16 +73,7 @@ struct fq_ctx
   unsigned memo_salt = 0;         // launch counter stamped into the memo entries (stale entries carry another value)
   bool cert_memo = true;          // option "cert_memo"
   bool early_exit = false;        // option "sweep_early_exit": candidates that cannot win genNewTraj's selection are skipped
-  bool launch_sorted_dt = false;  // set by the chained replan for its next launch: candidate lists are in ascending dt order
-  int launch_ee_width = 0;        // ... and hold this many candidates per time allocation
-  // single-problem sweep with the selection in the solve kernel's tail (consumed by the next launch):
-  int launch_sweep_n_sigma = 0;   // > 0: requested
-  int* launch_sweep_idx = nullptr;       // device-visible (host-mapped) outputs
-  double* launch_sweep_win = nullptr;
-  bool last_launch_tail = false;  // the last launch did run the tail selection (specialised kernel)
   unsigned long long* d_first = nullptr;   // ring (as d_counters) of per-problem "smallest feasible dt so far"
-  double* cert_out = nullptr;     // fq_solve_batch_cert: device buffer the generic kernel writes certificates into
-  int cert_stride = 0;
   // ---- multi-GPU (fq_multi.cu)
   FqComm* comm = nullptr;         // communicator this context belongs to (one process per GPU), or nullptr
   int rank = 0, world = 1;
@@ -104,12 +95,33 @@ int fq_get_plan(fq_ctx* ctx, int N, int force_final, FqPlanDev** out);
 void fq_fill_plan_args(const FqPlanDev& pd, FqKernelArgs* a);
 // a deferred call owns the context's arenas until it has drained: every entry point that reuses them settles first
 int fq_settle(fq_ctx* ctx);
-// common launch of the batch solve: every pointer is a device pointer
-int fq_launch_solve_ctx(fq_ctx* ctx, int N, int force_final, int n_prob, const double* d_x0, const double* d_xf,
-                        const double* d_lim, const int* d_poly_ofs, const int* d_face_ofs, const double* d_Ab,
-                        const int* d_cand_ofs, int max_cand, int max_faces, int max_poly_faces, const double* d_dt,
-                        const uint8_t* d_sigma, uint8_t* d_feasible, double* d_cost, double* d_coeffs, int32_t* d_iters,
-                        cudaStream_t stream);
+// common launch of the batch solve.  `a` comes value-initialised with N, force_final, the problems and outputs (device
+// pointers), max_faces and this launch's options (sorted_dt, ee_width, sweep_*, cert); the launch adds the plan tables,
+// row_tol, item_cap (max_poly_faces <= 0: unknown) and the context's state.  *tail: the selection ran in the kernel's tail.
+int fq_launch_solve_ctx(fq_ctx* ctx, FqKernelArgs a, int max_cand, int max_poly_faces, cudaStream_t stream, bool* tail = nullptr);
 inline size_t fq_align16(size_t x) { return (x + 15) & ~(size_t)15; }
+// corridors of n_prob problems (problem j: polytopes poly_ofs[j] .. poly_ofs[j+1]-1; polytope p: rows face_ofs[p] ..
+// face_ofs[p+1]-1 of Ab).  fq_scan_corridors checks that every polytope count is in 0..FQ_MAX_POLY and that face_ofs is
+// monotone, and returns why it refuses the description, or nullptr.  Entries that stage the arrays as given also
+// require both offset arrays to start at 0; the single-problem sweeps do not (they stage rows 0 .. face_ofs[P]-1).
+struct FqCorridorSizes
+{
+  int max_faces = 0, max_poly_faces = 0;    // largest total faces of one problem / faces of one polytope
+  int n_poly = 0, n_face = 0;               // poly_ofs[n_prob], face_ofs[n_poly]
+};
+const char* fq_scan_corridors(int n_prob, const int* poly_ofs, const int* face_ofs, FqCorridorSizes* sizes);
+// fq_solve_multi_async + the genNewTraj winner of every problem, selected on the device (the arrays stay in the context's
+// output arena until the next call): what the multi-GPU path all-gathers
+int fq_solve_multi_host_ex(fq_ctx* ctx, int N, int force_final, int n_prob, const double* x0, const double* xf, const double* lim,
+                           const int* poly_ofs, const int* face_ofs, const double* Ab, const int* cand_ofs, const double* dt,
+                           const uint8_t* sigma, uint8_t* feasible, double* cost, double* coeffs, int32_t* iters, bool deferred,
+                           int** d_win_idx, double** d_win_cost);
+// fq_pair_capi.cu.  d_results (may be NULL): receives the device address of the result records; copy_results = false
+// leaves the caller's `results` array untouched (the multi-GPU path reads the all-gathered table instead)
+int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results);
 // fq_multi.cu
 void fq_comm_release(fq_ctx* ctx);
+// all-gather on one context's communicator (one process per GPU): `bytes` from every rank, rank order
+int fq_comm_allgather(fq_ctx* ctx, const void* d_send, void* d_recv, size_t bytes, cudaStream_t stream);
+// fq_replan_pairs on a multi-GPU context (a group or a rank of a communicator)
+int fq_replan_pairs_sharded(fq_ctx* g, const fq_pair_args* a, bool deferred);

@@ -15,12 +15,6 @@
 #include <mutex>
 #include <nccl.h>
 
-int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results);
-int fq_solve_multi_host_ex(fq_ctx* ctx, int N, int force_final, int n_prob, const double* x0, const double* xf, const double* lim,
-                           const int* poly_ofs, const int* face_ofs, const double* Ab, const int* cand_ofs, const double* dt,
-                           const uint8_t* sigma, uint8_t* feasible, double* cost, double* coeffs, int32_t* iters, bool deferred,
-                           int** d_win_idx, double** d_win_cost);
-
 namespace
 {
 struct NcclApi
@@ -177,7 +171,6 @@ extern "C" int fq_create_multi(fq_ctx** out, int n_gpus, const int* devices)
   return 0;
 }
 
-// all-gather on one context's communicator (one process per GPU): `bytes` from every rank, rank order
 int fq_comm_allgather(fq_ctx* ctx, const void* d_send, void* d_recv, size_t bytes, cudaStream_t stream)
 {
   if (!ctx->comm) return fq_fail(ctx, FQ_E_ARG, "no communicator attached (fq_comm_init / fq_create_multi)");
@@ -237,10 +230,17 @@ struct SubCorridors
   }
 };
 
-// all-gather over the members of a single-process group: member i sends `bytes` from send[i] into recv[i] (world x bytes)
-int group_allgather(fq_ctx* g, const std::vector<const void*>& send, const std::vector<void*>& recv, size_t bytes)
+// the one exchange of a sharded call: local member i (one for a rank context) sends `count` records from send[i] and
+// receives every rank's, in rank order, into recv[i].  Over the members of a single-process group, over a rank's
+// communicator, or a copy for a world of one.
+template <class T>
+int exchange(fq_ctx* g, const std::vector<T*>& send, const std::vector<T*>& recv, size_t count)
 {
   fq_ctx* ctx = g;
+  const size_t bytes = sizeof(T) * count;
+  if (!g->is_group && g->comm) return fq_comm_allgather(g, send[0], recv[0], bytes, g->stream);
+  // a context that is neither a group nor a communicator's rank keeps world == 1 (only fq_comm_init and fq_create_multi
+  // set it), so past this point world > 1 means a group with world - 1 peers
   if (g->world == 1)
   {
     FQ_CUDA(cudaSetDevice(g->device));
@@ -322,20 +322,7 @@ int fq_replan_pairs_sharded(fq_ctx* g, const fq_pair_args* a, bool deferred)
     e = cudaMemcpyAsync(d_res[i], dr, sizeof(fq_pair_result) * (size_t)n, cudaMemcpyDeviceToDevice, c->stream);
     if (e != cudaSuccess) return fq_cuda_fail(g, e, "gather staging");
   }
-  // ---- the one exchange
-  if (group)
-  {
-    std::vector<const void*> send(world);
-    std::vector<void*> recv(world);
-    for (int i = 0; i < world; i++) { send[i] = d_res[i]; recv[i] = d_all[i]; }
-    if (int rc = group_allgather(g, send, recv, sizeof(fq_pair_result) * (size_t)pad)) return rc;
-  }
-  else if (g->comm)
-  {
-    if (int rc = fq_comm_allgather(g, d_res[0], d_all[0], sizeof(fq_pair_result) * (size_t)pad, g->stream)) return rc;
-  }
-  else
-    FQ_CUDA(cudaMemcpyAsync(d_all[0], d_res[0], sizeof(fq_pair_result) * (size_t)pad, cudaMemcpyDeviceToDevice, g->stream));
+  if (int rc = exchange(g, d_res, d_all, (size_t)pad)) return rc;
   // ---- the gathered table, shard by shard, into the caller's results (from member 0 / this rank)
   FQ_CUDA(cudaSetDevice(g->device));
   for (int r = 0; r < world; r++)
@@ -402,19 +389,7 @@ extern "C" int fq_solve_multi_sharded(fq_ctx* g, int N, int force_final, int n_p
       e = cudaMemcpy2DAsync(&d_res[i][0].idx, sizeof(Rec), dwi, sizeof(int), sizeof(int), n, cudaMemcpyDeviceToDevice, c->stream);
     if (e != cudaSuccess) return fq_cuda_fail(g, e, "winner records");
   }
-  if (group)
-  {
-    std::vector<const void*> send(world);
-    std::vector<void*> recv(world);
-    for (int i = 0; i < world; i++) { send[i] = d_res[i]; recv[i] = d_all[i]; }
-    if (int rc = group_allgather(g, send, recv, sizeof(Rec) * (size_t)pad)) return rc;
-  }
-  else if (g->comm)
-  {
-    if (int rc = fq_comm_allgather(g, d_res[0], d_all[0], sizeof(Rec) * (size_t)pad, g->stream)) return rc;
-  }
-  else
-    FQ_CUDA(cudaMemcpyAsync(d_all[0], d_res[0], sizeof(Rec) * (size_t)pad, cudaMemcpyDeviceToDevice, g->stream));
+  if (int rc = exchange(g, d_res, d_all, (size_t)pad)) return rc;
   FQ_CUDA(cudaSetDevice(g->device));
   std::vector<Rec> all((size_t)pad * world);
   FQ_CUDA(cudaMemcpyAsync(all.data(), d_all[0], sizeof(Rec) * all.size(), cudaMemcpyDeviceToHost, g->stream));

@@ -7,8 +7,6 @@
 #include <cmath>
 #include <cstring>
 
-int fq_comm_allgather(fq_ctx* ctx, const void* d_send, void* d_recv, size_t bytes, cudaStream_t stream);   // fq_multi.cu
-
 namespace
 {
 struct Scratch
@@ -89,15 +87,21 @@ extern "C" int fq_replan_pairs_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_r
     double* coeffs_w = a->coeffs_whole ? a->coeffs_whole : s.coeffs_w;
     double* coeffs_s = a->coeffs_safe ? a->coeffs_safe : s.coeffs_s;
     const int mcw = a->n_fac_whole * a->n_sig_whole, mcs = a->n_fac_safe * a->n_sig_safe;
+    // the corridors of the two sweeps; each launch adds its candidates and outputs
+    FqKernelArgs whole{}, safe{};
+    whole.N = Nw; whole.force_final = 1; whole.n_prob = P; whole.x0 = a->x0; whole.xf = a->xf_whole; whole.lim = a->lim;
+    whole.poly_ofs = a->poly_ofs_whole; whole.face_ofs = a->face_ofs_whole; whole.Ab = a->Ab_whole; whole.max_faces = a->max_faces_whole;
+    safe.N = Ns; safe.force_final = 0; safe.n_prob = P; safe.x0 = s.x0_safe; safe.xf = a->xf_safe; safe.lim = a->lim;
+    safe.poly_ofs = a->poly_ofs_safe; safe.face_ofs = a->face_ofs_safe; safe.Ab = a->Ab_safe; safe.max_faces = a->max_faces_safe;
 
     // ---- whole sweep (faster.cpp:406-418)
     FQ_CUDA(fq_launch_dtbase(P, Nw, a->DC, a->x0, a->xf_whole, a->lim, s.dt_base_w, st));
     FQ_CUDA(fq_launch_expand_grid(P, Nw, a->n_fac_whole, a->n_sig_whole, a->factors_whole, a->sigmas_whole, s.dt_base_w, s.dt_w,
                                   s.sig_w, s.cand_ofs_w, st));
-    ctx->launch_sorted_dt = true; ctx->launch_ee_width = a->n_sig_whole;   // factor-major grid, ascending factors
-    int rc = fq_launch_solve_ctx(ctx, Nw, 1, P, a->x0, a->xf_whole, a->lim, a->poly_ofs_whole, a->face_ofs_whole, a->Ab_whole,
-                                 s.cand_ofs_w, mcw, a->max_faces_whole, a->max_poly_faces_whole, s.dt_w, s.sig_w, feas_w, cost_w,
-                                 nullptr, nullptr, st);
+    FqKernelArgs k = whole;
+    k.cand_ofs = s.cand_ofs_w; k.dt = s.dt_w; k.sigma = s.sig_w; k.feasible = feas_w; k.cost = cost_w;
+    k.sorted_dt = 1; k.ee_width = a->n_sig_whole;         // factor-major grid, ascending factors
+    int rc = fq_launch_solve_ctx(ctx, k, mcw, a->max_poly_faces_whole, st);
     if (rc) return rc;
     FqSelectMultiArgs sw;
     sw.n_prob = P; sw.N = Nw; sw.n_sig = a->n_sig_whole; sw.cand_ofs = s.cand_ofs_w; sw.dt = s.dt_w; sw.sigma = s.sig_w;
@@ -105,9 +109,9 @@ extern "C" int fq_replan_pairs_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_r
     sw.win_sigma = s.win_sig_w; sw.win_ofs = s.win_ofs;
     FQ_CUDA(fq_launch_select_multi(sw, st));
     // coefficients of the winners: one candidate per corridor through the same kernel (losers' dt is NaN -> "not solved")
-    rc = fq_launch_solve_ctx(ctx, Nw, 1, P, a->x0, a->xf_whole, a->lim, a->poly_ofs_whole, a->face_ofs_whole, a->Ab_whole, s.win_ofs, 1,
-                             a->max_faces_whole, a->max_poly_faces_whole, s.win_dt_w, s.win_sig_w, s.re_feas, s.re_cost, coeffs_w,
-                             nullptr, st);
+    k = whole;
+    k.cand_ofs = s.win_ofs; k.dt = s.win_dt_w; k.sigma = s.win_sig_w; k.feasible = s.re_feas; k.cost = s.re_cost; k.coeffs = coeffs_w;
+    rc = fq_launch_solve_ctx(ctx, k, 1, a->max_poly_faces_whole, st);
     if (rc) return rc;
     // ---- R (faster.cpp:474-475) and the safe sweep from it (faster.cpp:521-527)
     FqPairMidArgs m;
@@ -117,10 +121,10 @@ extern "C" int fq_replan_pairs_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_r
     FQ_CUDA(fq_launch_dtbase(P, Ns, a->DC, s.x0_safe, a->xf_safe, a->lim, s.dt_base_s, st));
     FQ_CUDA(fq_launch_expand_grid(P, Ns, a->n_fac_safe, a->n_sig_safe, a->factors_safe, a->sigmas_safe, s.dt_base_s, s.dt_s,
                                   s.sig_s, s.cand_ofs_s, st));
-    ctx->launch_sorted_dt = true; ctx->launch_ee_width = a->n_sig_safe;
-    rc = fq_launch_solve_ctx(ctx, Ns, 0, P, s.x0_safe, a->xf_safe, a->lim, a->poly_ofs_safe, a->face_ofs_safe, a->Ab_safe,
-                             s.cand_ofs_s, mcs, a->max_faces_safe, a->max_poly_faces_safe, s.dt_s, s.sig_s, feas_s, cost_s, nullptr,
-                             nullptr, st);
+    k = safe;
+    k.cand_ofs = s.cand_ofs_s; k.dt = s.dt_s; k.sigma = s.sig_s; k.feasible = feas_s; k.cost = cost_s;
+    k.sorted_dt = 1; k.ee_width = a->n_sig_safe;
+    rc = fq_launch_solve_ctx(ctx, k, mcs, a->max_poly_faces_safe, st);
     if (rc) return rc;
     FqSelectMultiArgs ss = sw;
     ss.N = Ns; ss.n_sig = a->n_sig_safe; ss.cand_ofs = s.cand_ofs_s; ss.dt = s.dt_s; ss.sigma = s.sig_s; ss.feasible = feas_s;
@@ -128,9 +132,9 @@ extern "C" int fq_replan_pairs_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_r
     FQ_CUDA(fq_launch_select_multi(ss, st));
     if (a->coeffs_safe)
     {
-      rc = fq_launch_solve_ctx(ctx, Ns, 0, P, s.x0_safe, a->xf_safe, a->lim, a->poly_ofs_safe, a->face_ofs_safe, a->Ab_safe, s.win_ofs,
-                               1, a->max_faces_safe, a->max_poly_faces_safe, s.win_dt_s, s.win_sig_s, s.re_feas, s.re_cost, coeffs_s,
-                               nullptr, st);
+      k = safe;
+      k.cand_ofs = s.win_ofs; k.dt = s.win_dt_s; k.sigma = s.win_sig_s; k.feasible = s.re_feas; k.cost = s.re_cost; k.coeffs = coeffs_s;
+      rc = fq_launch_solve_ctx(ctx, k, 1, a->max_poly_faces_safe, st);
       if (rc) return rc;
     }
     FqPairFinalArgs f;
@@ -152,10 +156,6 @@ extern "C" int fq_replan_pairs_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_r
   return 0;
 }
 
-int fq_replan_pairs_sharded(fq_ctx* g, const fq_pair_args* a, bool deferred);   // fq_multi.cu
-
-// d_results (may be NULL): receives the device address of the result records; copy_results = false leaves the caller's
-// `results` array untouched (the multi-GPU path reads the all-gathered table instead)
 int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results)
 {
   if (!ctx) return FQ_E_ARG;
@@ -163,27 +163,16 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   if (int rc = check_common(ctx, a)) return rc;
   const int P = a->n_prob, Nw = a->N_whole, Ns = a->N_safe;
   // ---- validate the two corridor descriptions
-  int mfw = 0, mpfw = 0, mfs = 0, mpfs = 0, n_poly_w = 0, n_poly_s = 0, n_face_w = 0, n_face_s = 0;
-  auto scan = [&](const int* po, const int* fo, const double* Ab, int* mf, int* mpf, int* n_poly, int* n_face) -> const char* {
+  auto check = [&](const int* po, const int* fo, const double* Ab, FqCorridorSizes* sizes) -> const char* {
     if (po[0] != 0 || fo[0] != 0) return "offset arrays must start at 0";
-    for (int j = 0; j < P; j++)
-    {
-      const int np = po[j + 1] - po[j];
-      if (np < 0 || np > FQ_MAX_POLY) return "polytope count out of range (0..FQ_MAX_POLY)";
-      for (int p = po[j]; p < po[j + 1]; p++)
-      {
-        if (fo[p + 1] < fo[p]) return "face_ofs not monotone";
-        *mpf = std::max(*mpf, fo[p + 1] - fo[p]);
-      }
-      *mf = std::max(*mf, fo[po[j + 1]] - fo[po[j]]);
-    }
-    *n_poly = po[P]; *n_face = fo[*n_poly];
-    if (*n_face > 0 && !Ab) return "polytopes given but Ab is NULL";
-    if (*n_face > 0 && !fq_scan_all_finite(Ab, 4 * (size_t)*n_face)) return "non-finite value in Ab";
+    if (const char* why = fq_scan_corridors(P, po, fo, sizes)) return why;
+    if (sizes->n_face > 0 && !Ab) return "polytopes given but Ab is NULL";
+    if (sizes->n_face > 0 && !fq_scan_all_finite(Ab, 4 * (size_t)sizes->n_face)) return "non-finite value in Ab";
     return nullptr;
   };
-  if (const char* why = scan(a->poly_ofs_whole, a->face_ofs_whole, a->Ab_whole, &mfw, &mpfw, &n_poly_w, &n_face_w)) return fq_fail(ctx, FQ_E_ARG, why);
-  if (const char* why = scan(a->poly_ofs_safe, a->face_ofs_safe, a->Ab_safe, &mfs, &mpfs, &n_poly_s, &n_face_s)) return fq_fail(ctx, FQ_E_ARG, why);
+  FqCorridorSizes cw, cs;
+  if (const char* why = check(a->poly_ofs_whole, a->face_ofs_whole, a->Ab_whole, &cw)) return fq_fail(ctx, FQ_E_ARG, why);
+  if (const char* why = check(a->poly_ofs_safe, a->face_ofs_safe, a->Ab_safe, &cs)) return fq_fail(ctx, FQ_E_ARG, why);
   if (!fq_scan_all_finite(a->x0, 9 * (size_t)P) || !fq_scan_all_finite(a->xf_whole, 9 * (size_t)P) || !fq_scan_all_finite(a->xf_safe, 9 * (size_t)P))
     return fq_fail(ctx, FQ_E_ARG, "non-finite value in x0/xf");
   if (!fq_scan_all_positive_finite(a->lim, 3 * (size_t)P) || !fq_scan_all_positive_finite(a->factors_whole, (size_t)a->n_fac_whole) ||
@@ -193,8 +182,8 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
     if (a->factors_whole[i] < a->factors_whole[i - 1]) return fq_fail(ctx, FQ_E_ARG, "factors_whole must be ascending");
   for (int i = 1; i < a->n_fac_safe; i++)
     if (a->factors_safe[i] < a->factors_safe[i - 1]) return fq_fail(ctx, FQ_E_ARG, "factors_safe must be ascending");
-  if (n_poly_w > 0 && !a->sigmas_whole) return fq_fail(ctx, FQ_E_ARG, "sigmas_whole is NULL");
-  if (n_poly_s > 0 && !a->sigmas_safe) return fq_fail(ctx, FQ_E_ARG, "sigmas_safe is NULL");
+  if (cw.n_poly > 0 && !a->sigmas_whole) return fq_fail(ctx, FQ_E_ARG, "sigmas_whole is NULL");
+  if (cs.n_poly > 0 && !a->sigmas_safe) return fq_fail(ctx, FQ_E_ARG, "sigmas_safe is NULL");
   // assignments must name existing polytopes of EVERY corridor they are applied to
   {
     int min_pw = FQ_MAX_POLY, min_ps = FQ_MAX_POLY;
@@ -211,11 +200,11 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   const size_t ncw = (size_t)P * a->n_fac_whole * a->n_sig_whole, ncs = (size_t)P * a->n_fac_safe * a->n_sig_safe;
   size_t o = 0;
   auto put = [&](size_t bytes) { const size_t at = o; o = fq_align16(o + bytes); return at; };
-  const size_t oAbw = put(32 * (size_t)std::max(n_face_w, 1)), oAbs = put(32 * (size_t)std::max(n_face_s, 1));
+  const size_t oAbw = put(32 * (size_t)std::max(cw.n_face, 1)), oAbs = put(32 * (size_t)std::max(cs.n_face, 1));
   const size_t ox0 = put(72 * (size_t)P), oxfw = put(72 * (size_t)P), oxfs = put(72 * (size_t)P), olim = put(24 * (size_t)P);
   const size_t ofw = put(8 * (size_t)a->n_fac_whole), ofs = put(8 * (size_t)a->n_fac_safe);
-  const size_t opow = put(4 * (size_t)(P + 1)), ofow = put(4 * (size_t)(n_poly_w + 1));
-  const size_t opos = put(4 * (size_t)(P + 1)), ofos = put(4 * (size_t)(n_poly_s + 1));
+  const size_t opow = put(4 * (size_t)(P + 1)), ofow = put(4 * (size_t)(cw.n_poly + 1));
+  const size_t opos = put(4 * (size_t)(P + 1)), ofos = put(4 * (size_t)(cs.n_poly + 1));
   const size_t osw = put((size_t)a->n_sig_whole * Nw), oss = put((size_t)a->n_sig_safe * Ns);
   const size_t in_bytes = o;
   o = 0;
@@ -228,14 +217,14 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   char* hi = (char*)ctx->h_in.p;
   char* din = (char*)ctx->d_pair_io.p;
   char* dout = din + in_bytes;
-  if (n_face_w) std::memcpy(hi + oAbw, a->Ab_whole, 32 * (size_t)n_face_w);
-  if (n_face_s) std::memcpy(hi + oAbs, a->Ab_safe, 32 * (size_t)n_face_s);
+  if (cw.n_face) std::memcpy(hi + oAbw, a->Ab_whole, 32 * (size_t)cw.n_face);
+  if (cs.n_face) std::memcpy(hi + oAbs, a->Ab_safe, 32 * (size_t)cs.n_face);
   std::memcpy(hi + ox0, a->x0, 72 * (size_t)P);      std::memcpy(hi + oxfw, a->xf_whole, 72 * (size_t)P);
   std::memcpy(hi + oxfs, a->xf_safe, 72 * (size_t)P); std::memcpy(hi + olim, a->lim, 24 * (size_t)P);
   std::memcpy(hi + ofw, a->factors_whole, 8 * (size_t)a->n_fac_whole);
   std::memcpy(hi + ofs, a->factors_safe, 8 * (size_t)a->n_fac_safe);
-  std::memcpy(hi + opow, a->poly_ofs_whole, 4 * (size_t)(P + 1)); std::memcpy(hi + ofow, a->face_ofs_whole, 4 * (size_t)(n_poly_w + 1));
-  std::memcpy(hi + opos, a->poly_ofs_safe, 4 * (size_t)(P + 1));  std::memcpy(hi + ofos, a->face_ofs_safe, 4 * (size_t)(n_poly_s + 1));
+  std::memcpy(hi + opow, a->poly_ofs_whole, 4 * (size_t)(P + 1)); std::memcpy(hi + ofow, a->face_ofs_whole, 4 * (size_t)(cw.n_poly + 1));
+  std::memcpy(hi + opos, a->poly_ofs_safe, 4 * (size_t)(P + 1));  std::memcpy(hi + ofos, a->face_ofs_safe, 4 * (size_t)(cs.n_poly + 1));
   if (a->sigmas_whole) std::memcpy(hi + osw, a->sigmas_whole, (size_t)a->n_sig_whole * Nw);
   if (a->sigmas_safe) std::memcpy(hi + oss, a->sigmas_safe, (size_t)a->n_sig_safe * Ns);
   cudaStream_t st = ctx->stream;
@@ -252,7 +241,7 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   d.feasible_safe = a->feasible_safe ? (uint8_t*)(dout + ofes) : nullptr;   d.cost_safe = a->cost_safe ? (double*)(dout + ocs) : nullptr;
   d.coeffs_whole = a->coeffs_whole ? (double*)(dout + ocow) : nullptr;       d.coeffs_safe = a->coeffs_safe ? (double*)(dout + ocos) : nullptr;
   d.results = (fq_pair_result*)(dout + ores);
-  d.max_faces_whole = std::max(mfw, 1); d.max_poly_faces_whole = mpfw; d.max_faces_safe = std::max(mfs, 1); d.max_poly_faces_safe = mpfs;
+  d.max_faces_whole = std::max(cw.max_faces, 1); d.max_poly_faces_whole = cw.max_poly_faces; d.max_faces_safe = std::max(cs.max_faces, 1); d.max_poly_faces_safe = cs.max_poly_faces;
   // a NULL cost/flag output still needs a device array of its own kind: the chain allocates it in its scratch
   if ((d.feasible_whole == nullptr) != (d.cost_whole == nullptr) || (d.feasible_safe == nullptr) != (d.cost_safe == nullptr))
     return fq_fail(ctx, FQ_E_ARG, "feasible_* and cost_* must be given (or omitted) together");

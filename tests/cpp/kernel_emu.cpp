@@ -41,7 +41,7 @@ int emu_solve_multi(int N, int force_final, const double* TZ, const double* T0, 
                     const double* xf, const double* lim, const int* poly_ofs, const int* face_ofs, const double* Ab, int max_faces,
                     int max_poly_faces, const int* cand_ofs, const double* dt, const uint8_t* sigma, double row_tol, uint8_t* feasible,
                     double* cost, double* coeffs, int32_t* iters);
-// options of the next emu_solve_multi call (what fq_launch_solve_ctx sets for the drop-in class's sweeps, fq_capi.cu):
+// options of the next emu_solve_multi call (the FqKernelArgs options the drop-in class's sweeps launch with, fq_capi.cu):
 //   early_exit != 0: "first feasible factor wins" (first_feasible + sorted_dt: candidates whose dt exceeds the smallest feasible dt
 //                    found so far are not evaluated, iters = -3);
 //   sweep_n_sigma > 0: single-problem sweep, dt-major with that many assignments per time allocation: the warp that finishes the

@@ -140,6 +140,33 @@ def test_gen_new_traj_matches_oracle_sweep(solver, oracle, demo_corridor):
             assert np.abs(g["coeffs"] - o["coeffs"]).max() <= 1e-6 * max(1.0, np.abs(o["coeffs"]).max())
 
 
+def test_face_ofs_start_is_free_for_sweeps_and_zero_for_batches(solver):
+    """fq_gen_new_traj takes a face_ofs whose first offset is not 0 (it stages rows 0 .. face_ofs[P]-1 of Ab and starts
+    the first polytope at row 0); the batch entries refuse it ("offset arrays must start at 0")."""
+    import ctypes as C
+    N = 10
+    pb = cr.make_corridor(300, 3, N)
+    P, ofs, Ab = capi.pack_polys(pb["polys"])
+    ofs1 = np.ascontiguousarray(ofs + 1, np.int32)
+    Ab1 = np.ascontiguousarray(np.vstack([Ab[:1], Ab]))
+    sig = np.ascontiguousarray(cr.monotone_sigmas(N, P), np.uint8)
+    x0, xf, lim = (np.ascontiguousarray(pb[k], np.float64) for k in ("x0", "xf", "lim"))
+    dts = np.arange(1.0, 11.0) * max(capi.dt_initial(x0, xf, lim, N), 0.02)
+    di, si, cost = C.c_int(-1), C.c_int(-1), C.c_double(np.inf)
+    co = np.zeros((N, 12))
+    rc = solver._check(solver._L.fq_gen_new_traj(solver._h, N, 1, x0.ctypes.data, xf.ctypes.data, lim.ctypes.data, P,
+                                                 ofs1.ctypes.data, Ab1.ctypes.data, dts.size, dts.ctypes.data, sig.shape[0],
+                                                 sig.ctypes.data, C.addressof(di), C.addressof(si), C.addressof(cost),
+                                                 co.ctypes.data))
+    assert rc in (0, 1)
+    feas, costs = np.zeros(len(sig), np.uint8), np.zeros(len(sig))
+    d = np.full(len(sig), dts[-1])
+    rc = solver._L.fq_solve_batch(solver._h, N, 1, x0.ctypes.data, xf.ctypes.data, lim.ctypes.data, P, ofs1.ctypes.data,
+                                  Ab1.ctypes.data, len(sig), d.ctypes.data, sig.ctypes.data, feas.ctypes.data,
+                                  costs.ctypes.data, None, None)
+    assert rc == -1 and solver._L.fq_last_error(solver._h).decode() == "offset arrays must start at 0"
+
+
 def test_large_batch_properties(solver):
     """BASELINE config sizes (1024 whole / 8192 safe candidates): size-independent properties.
     (i) every feasible solution satisfies the model rows when re-evaluated on the host from the returned
