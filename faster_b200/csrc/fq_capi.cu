@@ -148,7 +148,8 @@ extern "C" int fq_has_feature(const char* name)
 
 extern "C" const char* fq_last_error(const fq_ctx* ctx) { return ctx ? ctx->err.c_str() : g_create_error.c_str(); }
 
-int fq_launch_solve_ctx(fq_ctx* ctx, FqKernelArgs a, int max_cand, int max_poly_faces, cudaStream_t stream, bool* tail)
+int fq_launch_solve_ctx(fq_ctx* ctx, FqKernelArgs a, int max_cand, int max_poly_faces, cudaStream_t stream, bool* tail,
+                        bool early_exit_ok)
 {
   if (tail) *tail = false;
   FqPlanDev* pd = nullptr;
@@ -171,7 +172,7 @@ int fq_launch_solve_ctx(fq_ctx* ctx, FqKernelArgs a, int max_cand, int max_poly_
   }
   const unsigned slot = ctx->counters_pos++ % kFqCounterSlots;
   int* counters = ctx->d_counters + (size_t)slot * ctx->counters_cap;
-  if (ctx->early_exit && max_cand > 1)
+  if (ctx->early_exit && early_exit_ok && max_cand > 1)
   {
     if (!ctx->d_first) FQ_CUDA(cudaMalloc(&ctx->d_first, sizeof(unsigned long long) * (size_t)kFqCounterSlots * ctx->counters_cap));
     a.first_feasible = ctx->d_first + (size_t)slot * ctx->counters_cap;
@@ -679,7 +680,9 @@ int gen_new_traj_impl(fq_ctx* ctx, int N, int force_final, const double* x0, con
     }
   }
   bool tail = false;
-  int rc = fq_launch_solve_ctx(ctx, a, n_cand, cs.max_poly_faces, st, &tail);
+  // the early exit skips candidates by dt VALUE, the selection picks the first dt INDEX with a feasible assignment: the
+  // two agree only when the dt list is ascending, so a sweep over any other order evaluates every candidate
+  int rc = fq_launch_solve_ctx(ctx, a, n_cand, cs.max_poly_faces, st, &tail, a.sorted_dt != 0);
   if (rc) return rc;
   if (tr.on) cudaEventRecord(tev[2], st);
   FqSelectArgs sa;

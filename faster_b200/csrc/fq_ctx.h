@@ -98,7 +98,9 @@ int fq_settle(fq_ctx* ctx);
 // common launch of the batch solve.  `a` comes value-initialised with N, force_final, the problems and outputs (device
 // pointers), max_faces and this launch's options (sorted_dt, ee_width, sweep_*, cert); the launch adds the plan tables,
 // row_tol, item_cap (max_poly_faces <= 0: unknown) and the context's state.  *tail: the selection ran in the kernel's tail.
-int fq_launch_solve_ctx(fq_ctx* ctx, FqKernelArgs a, int max_cand, int max_poly_faces, cudaStream_t stream, bool* tail = nullptr);
+// early_exit_ok = false: this launch evaluates every candidate even with option "sweep_early_exit" set.
+int fq_launch_solve_ctx(fq_ctx* ctx, FqKernelArgs a, int max_cand, int max_poly_faces, cudaStream_t stream, bool* tail = nullptr,
+                        bool early_exit_ok = true);
 inline size_t fq_align16(size_t x) { return (x + 15) & ~(size_t)15; }
 // corridors of n_prob problems (problem j: polytopes poly_ofs[j] .. poly_ofs[j+1]-1; polytope p: rows face_ofs[p] ..
 // face_ofs[p+1]-1 of Ab).  fq_scan_corridors checks that every polytope count is in 0..FQ_MAX_POLY and that face_ofs is

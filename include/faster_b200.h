@@ -66,6 +66,8 @@ const char* fq_last_error(const fq_ctx* ctx);   /* ctx may be NULL: last creatio
  * problem has a feasible candidate, candidates with a larger dt cannot win; with this option they are not evaluated
  * (reported feasible = 0, cost = +inf, iters = -3) and claims run in ascending dt.  The winners (fq_replan_pairs results,
  * fq_gen_new_traj*, fq_solve_multi_sharded's winners) are unchanged; the per-candidate arrays are no longer complete.
+ * fq_gen_new_traj* pick the first dt INDEX with a feasible assignment, so they apply the option only to an ascending dt
+ * list; a list in any other order is evaluated in full.
  * Returns 0 or FQ_E_ARG. */
 int fq_set_option(fq_ctx* ctx, const char* key, int value);
 

@@ -84,10 +84,17 @@ int emu_solve_multi(int N, int force_final, const double* TZ, const double* T0, 
   switch (key)
   {
     case 4 * 2 + 0: return run<4, false>(c);
+    case 5 * 2 + 1: return run<5, true>(c);
     case 6 * 2 + 1: return run<6, true>(c);
     case 10 * 2 + 1: return run<10, true>(c);
     case 10 * 2 + 0: return run<10, false>(c);
+    case 11 * 2 + 0: return run<11, false>(c);
+    case 12 * 2 + 0: return run<12, false>(c);
+    case 13 * 2 + 1: return run<13, true>(c);
+    case 13 * 2 + 0: return run<13, false>(c);
+    case 14 * 2 + 1: return run<14, true>(c);
     case 15 * 2 + 1: return run<15, true>(c);
+    case 16 * 2 + 0: return run<16, false>(c);
     default: return -1;
   }
 }

@@ -107,10 +107,16 @@ def test_demo_corridor_sweep_through_the_emulated_kernel(oracle, demo_corridor):
 
 
 @pytest.mark.parametrize("name,N,P,ff,profile", [("cfg2", 10, 3, True, "uav"), ("cfg3", 10, 4, False, "uav"), ("cfg5", 15, 8, True, "ground"),
-                                                  ("yaml", 6, 3, True, "uav"), ("small-safe", 4, 2, False, "uav")])
+                                                  ("yaml", 6, 3, True, "uav"), ("small-safe", 4, 2, False, "uav"),
+                                                  ("whole-5", 5, 2, True, "uav"), ("safe-11", 11, 3, False, "uav"),
+                                                  ("safe-12", 12, 3, False, "uav"), ("whole-13", 13, 3, True, "uav"),
+                                                  ("safe-13", 13, 4, False, "ground"), ("whole-14", 14, 4, True, "uav"),
+                                                  ("safe-16", 16, 8, False, "uav")])
 def test_emulated_kernel_matches_the_cpu_restatement(oracle, name, N, P, ff, profile):
     """Several corridors per launch (warps adopt problems and claim candidates dynamically, as on the GPU), monotone and
-    arbitrary assignments, whole and safe mode, one and two slots per lane (N = 15: 36 unknowns)."""
+    arbitrary assignments, whole and safe mode, one and two slots per lane (N = 15: 36 unknowns).  The added shapes sit on
+    the lane-layout boundaries: the last one-slot shapes (whole 13, safe 12: 30 unknowns) and the first two-slot ones (whole
+    14, safe 13: 33), N = 5 (one Y row per lane) and N = 11 (the first with three), and the largest safe shape."""
     rng = np.random.default_rng(len(name) + N)
     b = _batch(oracle, N, P, ff, profile, [9100 + 7 * N + k for k in range(3)], 10, [0.3, 0.6, 1.0, 1.5, 2.0, 3.0, 5.0], rng)
     got = solve_multi(_emu(), N, ff, *b)

@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 from faster_b200 import capi, corridor as cr
+from shape_cases import SHAPES, shape_batches
 
 pytestmark = pytest.mark.gpu
 
@@ -224,6 +225,71 @@ def test_generic_and_specialised_kernels_agree(built_lib, N, P, ff):
         assert ita.max() > 0 and itb.max() > 0      # iteration counts differ: the two kernels use different pivot rules
     finally:
         s.close()
+
+
+@pytest.mark.parametrize("N,ff", SHAPES)
+def test_every_solver_shape_matches_the_restatement(solver, oracle, N, ff):
+    """Every (N, mode) the solver is compiled for (fq_solve_kernel_t<N, WHOLE>, N = 4..16) and the size-generic kernel on the
+    same batches, against the CPU restatement.  The shape sets the lane layout: NW-vector slots per lane (one up to whole
+    N = 13 / safe N = 12, two from whole 14 / safe 13), Y rows per lane (1, 2, 3, 4 from N = 4, 6, 11, 16) and the
+    register budget (N = 10/11, 15/16).  One corridor of each family of tests/shape_cases.py."""
+    n_feas = n_infeas = 0
+    try:
+        for P, profile, c, pb, dts, sigs in shape_batches(N, ff, 1):
+            fo, co_, coo = oracle.solve_batch(N, pb["x0"], pb["xf"], pb["lim"], pb["polys"], dts, sigs, ff, True, threads=8)
+            for generic in (0, 1):
+                solver.set_option("force_generic_kernel", generic)
+                fg, cg, cog, it = solver.solve_batch(N, pb["x0"], pb["xf"], pb["lim"], pb["polys"], dts, sigs, ff, True, True)
+                what = "N=%d ff=%d P=%d %s generic=%d" % (N, ff, P, profile, generic)
+                _compare(fg, cg, cog, fo, co_, coo, what)
+                assert (it >= 0).all(), what + ": iteration-cap or numeric give-ups"
+            n_feas += int(fo.sum())
+            n_infeas += int((fo == 0).sum())
+    finally:
+        solver.set_option("force_generic_kernel", 0)
+    assert n_feas >= 20 and n_infeas >= 20, (n_feas, n_infeas)
+
+
+@pytest.mark.parametrize("N,ff", [(3, True), (2, False), (3, False)])
+def test_generic_only_shapes_on_corridors(solver, oracle, N, ff):
+    """Shapes below the specialised range run on the size-generic kernel only: whole N = 3 and safe N = 2 have no degree
+    of freedom left (a feasibility check of the one trajectory through corridor rows), safe N = 3 has one."""
+    n_feas = n_infeas = 0
+    for seed in range(6):
+        for P in (2, 3):
+            pb = cr.make_corridor(61000 + 10 * seed + P, P, N, "uav", ff)
+            sig = np.vstack([cr.monotone_sigmas(N, P), np.random.default_rng(seed).integers(0, P, (4, N)).astype(np.uint8)])
+            dti = capi.dt_initial(pb["x0"], pb["xf"], pb["lim"], N)
+            facs = np.array([0.5, 1.0, 1.5, 2.0, 3.0, 5.0, 8.0])
+            dts = np.repeat(facs * max(dti, 2 * pb["DC"]), len(sig))
+            sigs = np.tile(sig, (len(facs), 1))
+            fg, cg, cog, it = solver.solve_batch(N, pb["x0"], pb["xf"], pb["lim"], pb["polys"], dts, sigs, ff, True, True)
+            fo, co_, coo = oracle.solve_batch(N, pb["x0"], pb["xf"], pb["lim"], pb["polys"], dts, sigs, ff, True)
+            _compare(fg, cg, cog, fo, co_, coo, "N=%d ff=%d P=%d seed=%d" % (N, ff, P, seed))
+            assert (it >= 0).all()
+            n_feas += int(fo.sum())
+            n_infeas += int((fo == 0).sum())
+    assert n_feas >= 5 and n_infeas >= 5, (n_feas, n_infeas)
+
+
+@pytest.mark.parametrize("N_whole,N_safe", [(10, 2), (3, 2), (6, 3)])
+def test_chained_replan_with_generic_only_shapes(solver, oracle, N_whole, N_safe):
+    """fq_replan_pairs with a generic-only shape on one side (N_safe = 2 is the smallest it accepts) against the CPU chain
+    (oracle/pair_oracle.py) on the device's own time-allocation bases."""
+    from oracle import pair_oracle
+    n = 12
+    whole = [cr.make_corridor(62000 + j, 3, N_whole, "uav", True) for j in range(n)]
+    safe = [cr.make_corridor(62000 + j, 2, N_safe, "uav", False) for j in range(n)]
+    fw = np.array([1.0, 1.5, 2.0, 3.0, 5.0, 8.0])
+    w = capi.make_pair_workload(whole, safe, fw, cr.monotone_sigmas(N_whole, 3)[:24], fw, cr.monotone_sigmas(N_safe, 2),
+                                DC=0.01, r_fraction=0.3)
+    g = solver.replan_pairs(w)
+    r = g["results"]
+    o = pair_oracle.replan_pairs(w, threads=4, dt_base_whole=r["whole_dt_base"], dt_base_safe=r["safe_dt_base"])
+    from test_pair_gpu import _check_against_oracle
+    _check_against_oracle(g, o, n)
+    assert (o["safe_dt_index"] >= 0).any() and o["feasible_safe"].any() and not o["feasible_safe"].all()
+    assert o["feasible_whole"].any() and not o["feasible_whole"].all()
 
 
 def test_edge_cases_through_the_abi(solver, oracle):
@@ -602,6 +668,44 @@ def test_exact_miqp_branch_and_bound_on_gpu(solver, oracle):
             assert g["exact"] and g["solved"] == o["solved"]
             if o["solved"]:
                 assert g["dt_index"] + 1 == o["trials"] and abs(g["cost"] - o["cost"]) <= REL * max(1.0, o["cost"])
+
+
+@pytest.mark.parametrize("N", [4, 5, 8, 11, 13, 14, 16])
+@pytest.mark.parametrize("ff", [True, False])
+def test_exact_miqp_branch_and_bound_across_shapes(solver, oracle, N, ff):
+    """The branch-and-bound level kernel (fqb::launch_level<N, WHOLE>) on the lane-layout boundaries, whole and safe mode,
+    against the oracle's branch-and-bound: single time allocations (solve_miqp) and sweeps (gen_new_traj over all
+    assignments).  Two or three polytopes keep the trees small enough that the node pool cannot overflow: exact = 1."""
+    P = 3 if N <= 11 else 2
+    n_solved = n_unsolved = 0
+    for seed in range(3):
+        pb = cr.make_corridor(63000 + 31 * N + seed, P, N, "uav", ff)
+        base = max(capi.dt_initial(pb["x0"], pb["xf"], pb["lim"], N), 0.02)
+        for f in ((1.0, 2.0, 4.0) if ff else (0.3, 0.6, 2.0)):
+            g = solver.gen_new_traj_exact(N, pb["x0"], pb["xf"], pb["lim"], pb["polys"], [f * base], ff)
+            rc, c, co, _, _ = oracle.solve_miqp(N, pb["x0"], pb["xf"], pb["lim"], f * base, pb["polys"], ff)
+            what = (N, ff, seed, f)
+            assert g["exact"], what
+            assert g["solved"] == (rc == 1), what
+            if rc == 1:
+                n_solved += 1
+                assert abs(g["cost"] - c) <= REL * max(1.0, c), what
+                assert np.abs(g["coeffs"] - co).max() <= 1e-6 * max(1.0, np.abs(co).max()), what
+                r2, c2, _, _ = oracle.solve_fixed(N, pb["x0"], pb["xf"], pb["lim"], f * base, pb["polys"], g["sigma"], ff)
+                assert r2 == 1 and abs(c2 - c) <= 1e-9 * max(1.0, c), what
+            else:
+                n_unsolved += 1
+        f0 = 1.0 if ff else 0.3
+        facs = [f0]
+        while facs[-1] + f0 <= 10.0 * f0:                        # the oracle's factor loop, with its rounding
+            facs.append(facs[-1] + f0)
+        facs = np.array(facs)
+        g = solver.gen_new_traj_exact(N, pb["x0"], pb["xf"], pb["lim"], pb["polys"], facs * base, ff)
+        o = oracle.gen_new_traj(N, pb["x0"], pb["xf"], pb["lim"], pb["polys"], 0.01, f0, 10.0 * f0, f0, None, ff)
+        assert g["exact"] and g["solved"] == o["solved"], (N, ff, seed)
+        if o["solved"]:
+            assert g["dt_index"] + 1 == o["trials"] and abs(g["cost"] - o["cost"]) <= REL * max(1.0, o["cost"]), (N, ff, seed)
+    assert n_solved >= 2 and n_unsolved >= 1, (n_solved, n_unsolved)
 
 
 def test_full_host_pipeline_then_gpu_solve(solver, oracle):
