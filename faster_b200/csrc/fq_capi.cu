@@ -129,8 +129,10 @@ extern "C" int fq_set_option(fq_ctx* ctx, const char* key, int value)
   if (std::string(key) == "cert_memo") { ctx->cert_memo = value != 0; return 0; }
   if (std::string(key) == "sweep_early_exit") { ctx->early_exit = value != 0; return 0; }
   if (std::string(key) == "row_tol_1e9")
-  { // row tolerance in units of 1e-9 (10 = the default 1e-8, 1000 = Gurobi's default FeasibilityTol 1e-6); >= 0
-    if (value < 0 || value > 1000000) return fq_fail(ctx, FQ_E_ARG, "row_tol_1e9 out of range (0..1000000)");
+  { // row tolerance in units of 1e-9 (10 = the default 1e-8, 1000 = Gurobi's default FeasibilityTol 1e-6).  0 is refused:
+    // a row just made active can still be violated by rounding, is picked again and the active set cycles to the
+    // iteration cap; 1e-9 is also the lowest FeasibilityTol Gurobi accepts
+    if (value < 1 || value > 1000000) return fq_fail(ctx, FQ_E_ARG, "row_tol_1e9 out of range (1..1000000, i.e. 1e-9 to 1e-3)");
     ctx->row_tol = 1e-9 * (double)value;
     return 0;
   }

@@ -87,11 +87,12 @@ def literal_row_index(N, polys, sigma):
     return box, cor, r
 
 
-def assert_infeasible(model, N, polys, sigma, cert_row, resid_tol=1e-7):
+def assert_infeasible(model, N, polys, sigma, cert_row, resid_tol=1e-7, gap_max=-1e-9):
     """cert_row = one row of fq_solve_batch_cert's output for a candidate reported "not solved".  Checks the Farkas
     certificate on the literal rows: multipliers y >= 0 on the named inequality rows, free multipliers mu on the equality
-    rows (least squares), sum y_k row_k + Aeq' mu = 0, y' bin + mu' beq < 0.  No point can satisfy rows that combine, with
-    non-negative weights, to 0 <= negative.  -> the gap (negative)."""
+    rows (least squares), sum y_k row_k + Aeq' mu = 0, y' bin + mu' beq < gap_max.  No point can satisfy rows that combine,
+    with non-negative weights, to 0 <= negative.  gap_max = minus the row tolerance the solve ran at: a solver that refuses
+    only violations beyond its tolerance leaves a gap below it.  -> the gap (negative)."""
     Q, Aeq, beq, Ain, bin_ = model
     n = int(cert_row[0])
     assert n >= 1, "infeasible candidate without certificate"
@@ -114,6 +115,6 @@ def assert_infeasible(model, N, polys, sigma, cert_row, resid_tol=1e-7):
     scale = max(1.0, np.abs(g).max())
     assert resid <= resid_tol * scale, (resid, scale)
     gap = float(bin_ @ y + beq @ mu)                   # < 0: the rows cannot hold together
-    assert gap < -1e-9, gap
+    assert gap < gap_max, (gap, gap_max)
     assert abs(gap + cert_row[1]) <= 1e-6 * max(1.0, abs(gap)), (gap, cert_row[1])   # = minus the violation the solver saw
     return gap

@@ -61,10 +61,13 @@ def solve_multi(L, N, ff, x0, xf, lim, poly_ofs, face_ofs, Ab, cand_ofs, dts, si
     return feas, cost, co, it
 
 
-def _batch(oracle, N, P, ff, profile, seeds, n_sig, factors, rng):
+def _batch(oracle, N, P, ff, profile, seeds, n_sig, factors, rng, change=None):
+    """change(pb) -> corridor, if given, modifies each corridor (final state, probe rows) before it is packed."""
     x0, xf, lim, po_, fo, rows, co_, dts, sigs = [], [], [], [0], [0], [], [0], [], []
     for seed in seeds:
         pb = cr.make_corridor(seed, P, N, profile, ff)
+        if change is not None:
+            pb = change(pb)
         allm = cr.monotone_sigmas(N, P) if P <= 4 else cr.sample_monotone_sigmas(N, P, 200, rng)
         sig = np.vstack([allm[rng.choice(len(allm), min(n_sig - 2, len(allm)), replace=False)], rng.integers(0, P, (2, N)).astype(np.uint8)])
         base = max(oracle.dt_initial(pb["x0"], pb["xf"], pb["lim"], N), 0.02)
@@ -111,17 +114,51 @@ def test_demo_corridor_sweep_through_the_emulated_kernel(oracle, demo_corridor):
                                                   ("whole-5", 5, 2, True, "uav"), ("safe-11", 11, 3, False, "uav"),
                                                   ("safe-12", 12, 3, False, "uav"), ("whole-13", 13, 3, True, "uav"),
                                                   ("safe-13", 13, 4, False, "ground"), ("whole-14", 14, 4, True, "uav"),
-                                                  ("safe-16", 16, 8, False, "uav")])
+                                                  ("safe-16", 16, 8, False, "uav"), ("whole-moving", 10, 3, True, "uav"),
+                                                  ("safe-moving", 10, 3, False, "uav")])
 def test_emulated_kernel_matches_the_cpu_restatement(oracle, name, N, P, ff, profile):
     """Several corridors per launch (warps adopt problems and claim candidates dynamically, as on the GPU), monotone and
     arbitrary assignments, whole and safe mode, one and two slots per lane (N = 15: 36 unknowns).  The added shapes sit on
     the lane-layout boundaries: the last one-slot shapes (whole 13, safe 12: 30 unknowns) and the first two-slot ones (whole
-    14, safe 13: 33), N = 5 (one Y row per lane) and N = 11 (the first with three), and the largest safe shape."""
+    14, safe 13: 33), N = 5 (one Y row per lane) and N = 11 (the first with three), and the largest safe shape.  The
+    "moving" batches end in a moving final state (nonzero velocity and acceleration)."""
+    from shape_cases import moving_final_state
     rng = np.random.default_rng(len(name) + N)
-    b = _batch(oracle, N, P, ff, profile, [9100 + 7 * N + k for k in range(3)], 10, [0.3, 0.6, 1.0, 1.5, 2.0, 3.0, 5.0], rng)
+    b = _batch(oracle, N, P, ff, profile, [9100 + 7 * N + k for k in range(3)], 10, [0.3, 0.6, 1.0, 1.5, 2.0, 3.0, 5.0], rng,
+               moving_final_state if name.endswith("moving") else None)
     got = solve_multi(_emu(), N, ff, *b)
     n_ok = _check(oracle, N, ff, b, got)
     assert n_ok >= 10
+    assert (got[3] >= 0).all()
+
+
+@pytest.mark.parametrize("ff,kind", [(True, "velocity"), (True, "x0_face"), (True, "xf_face"), (False, "x0_face")])
+def test_emulated_kernel_honours_the_row_tolerance(oracle, ff, kind):
+    """Corridors with one input-fixed row violated by 3e-7 (tests/shape_cases.py's probes) at row tolerance 1e-9 and 1e-3
+    against the restatement and the tuned CPU port at the same tolerance: every probed candidate is infeasible at 1e-9,
+    some are feasible at 1e-3, and the kernel never gives up."""
+    from shape_cases import probe
+    N, P = 10, 3
+    rng = np.random.default_rng(17)
+    seeds = [s for s in range(71000, 71100) if np.abs(cr.make_corridor(s, P, N, "uav", ff)["x0"][3:6]).max() >= 0.6][:2]
+    b = _batch(oracle, N, P, ff, "uav", seeds, 10, [1.0, 2.0, 3.0, 5.0, 8.0], rng, lambda pb: probe(pb, kind))
+    n_feas = {}
+    try:
+        for tol in (1e-9, 1e-3):
+            oracle.set_row_tol(tol)
+            oracle.port_lib().fqc_set_row_tol(tol)
+            got = solve_multi(_emu(), N, ff, *b, row_tol=tol)
+            assert (got[3] >= 0).all(), tol
+            fo, _ = oracle.solve_multi(N, ff, *b, threads=4)
+            assert np.array_equal(got[0], fo), tol
+            f = got[0].astype(bool)
+            if f.any() and (~f).any():
+                _check(oracle, N, ff, b, got)
+            n_feas[tol] = int(got[0].sum())
+    finally:
+        oracle.set_row_tol(1e-8)
+        oracle.port_lib().fqc_set_row_tol(1e-8)
+    assert n_feas[1e-9] == 0 and n_feas[1e-3] > 0, n_feas
 
 
 def test_compile_time_variants_compute_the_same_thing(oracle):

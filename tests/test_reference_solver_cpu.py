@@ -22,7 +22,8 @@ from faster_b200 import capi, corridor as cr
 from oracle import model_fullspace as mf, solver_ref as sr
 
 CASES = [("cfg1", 3, 0, True, "uav"), ("cfg2", 10, 3, True, "uav"), ("cfg3", 10, 4, False, "uav"), ("cfg5", 15, 8, True, "ground"),
-         ("yaml", 6, 3, True, "uav"), ("safe-small", 6, 2, False, "uav")]
+         ("yaml", 6, 3, True, "uav"), ("safe-small", 6, 2, False, "uav"), ("whole-moving", 10, 3, True, "uav"),
+         ("safe-moving", 6, 3, False, "uav")]
 
 
 @pytest.mark.parametrize("name,N,P,ff,profile", CASES)
@@ -31,9 +32,13 @@ def test_literal_model_equals_what_the_reference_code_builds(name, N, P, ff, pro
     setConstraintsX0 / setConstraintsXf / setDynamicConstraints / setObjective create (solverGurobi.cpp:70-120,:180-291,
     :332-407,:499-524): EXACTLY equal coefficients and right-hand sides (the same arithmetic on the same numbers); equalities and
     box rows in the same order, the corridor rows of a segment grouped by face then control point in the reference and by control
-    point then face in the restatement."""
+    point then face in the restatement.  The "moving" cases end in a moving final state, so that the final-velocity and
+    final-acceleration rows have nonzero right-hand sides."""
+    from shape_cases import moving_final_state
     rng = np.random.default_rng(len(name) + N)
     pb = cr.make_corridor(7000 + N + P, max(P, 1), N, profile, ff)
+    if name.endswith("moving"):
+        pb = moving_final_state(pb)
     polys = pb["polys"] if P else []
     base = max(capi.dt_initial(pb["x0"], pb["xf"], pb["lim"], N), 0.02)
     for dt in (1.3 * base, 2.7 * base):
@@ -105,6 +110,21 @@ def test_dt_initial_num_samples_and_fill_x_equal_the_reference_code(oracle):
         assert len(ref) == capi.num_samples(N, dt, DC) == len(ours)
         assert np.abs(ref - ours).max() <= 1e-12 * max(1.0, np.abs(ref).max())
         assert not ref[-1, 3:].any() and not ours[-1, 3:].any()  # :165-167
+    # a solution that arrives MOVING (nonzero final velocity and acceleration): fillX still writes the last sample with zero
+    # velocity, acceleration and jerk (:165-167), at the position the trajectory has there
+    from shape_cases import moving_final_state
+    for N, ff in ((10, True), (6, False)):
+        pb = moving_final_state(cr.make_corridor(7100 + N, 3, N, "uav", ff))
+        o = oracle.gen_new_traj(N, pb["x0"], pb["xf"], pb["lim"], pb["polys"], 0.01, 1.0, 10.0, 1.0, None, ff)
+        assert o["solved"]
+        assert capi.dt_initial(pb["x0"], pb["xf"], pb["lim"], N) == sr.dt_initial(pb["x0"], pb["xf"], pb["lim"], N)
+        ref = sr.fill_x(N, o["coeffs"], o["dt"], 0.01)
+        ours = capi.fill_x(N, o["coeffs"], o["dt"], 0.01)
+        assert len(ref) == len(ours) and np.abs(ref - ours).max() <= 1e-12 * max(1.0, np.abs(ref).max())
+        assert not ref[-1, 3:].any() and not ours[-1, 3:].any()
+        assert np.abs(ref[-2, 3:6] - pb["xf"][3:6]).max() <= 0.05     # one sample earlier the final velocity is there
+        if ff:
+            assert np.abs(ref[-1, :3] - pb["xf"][:3]).max() <= 0.01
 
 
 def _highs(q, Aeq, beq, Ain, bin_):
