@@ -101,7 +101,7 @@ __global__ void __launch_bounds__(W * 32, (N_ <= 10 ? 4 : (N_ <= 15 ? 3 : 2))) f
       double2 v = src[i];
       bad |= !(fabs(v.x) < 1e300) || !(fabs(v.y) < 1e300);
       if (i & 1) v.y += a.row_tol;
-      fqt::row_store(sAb, i, 2 * a.max_faces, v);
+      fqt::row_store(sAb, i, v);
     }
     for (int i = threadIdx.x; i <= P && i < 36; i += blockDim.x) sfo[i] = a.face_ofs[p0 + i] - f0;
     rows_bad = __syncthreads_or(bad) != 0;
@@ -123,7 +123,6 @@ __global__ void __launch_bounds__(W * 32, (N_ <= 10 ? 4 : (N_ <= 15 ? 3 : 2))) f
     m.d = p;   p += NW + 2;
     m.zb = p;  p += NW;
     m.items = reinterpret_cast<unsigned short*>(p);
-    m.half_ofs = 2 * a.max_faces;
     seg_ofs = sfo + 40 + warp * 32;
   }
   // ---- parent

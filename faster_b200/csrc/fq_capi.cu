@@ -110,7 +110,6 @@ extern "C" void fq_destroy(fq_ctx* ctx)
   ctx->d_in.release(); ctx->d_out.release(); ctx->d_bnb.release(); ctx->d_pair.release(); ctx->d_pair_io.release();
   ctx->h_in.release(); ctx->h_out.release();
   if (ctx->d_counters) cudaFree(ctx->d_counters);
-  if (ctx->d_memo) cudaFree(ctx->d_memo);
   if (ctx->d_first) cudaFree(ctx->d_first);
   if (ctx->ev_head) cudaEventDestroy(ctx->ev_head);
   if (ctx->stream2) cudaStreamDestroy(ctx->stream2);
@@ -126,7 +125,7 @@ extern "C" int fq_set_option(fq_ctx* ctx, const char* key, int value)
   if (std::string(key) == "force_generic_kernel") { ctx->force_generic = value != 0; return 0; }
   if (std::string(key) == "throughput_slices") { ctx->throughput_slices = value > 0 && value <= 64 ? value : 0; return 0; }
   if (std::string(key) == "max_faces_per_polytope") { ctx->max_poly_faces_hint = value > 0 ? value : 0; return 0; }
-  if (std::string(key) == "cert_memo") { ctx->cert_memo = value != 0; return 0; }
+  if (std::string(key) == "cert_memo") return 0;   // accepted and ignored: the GPU kernels have no certificate memo
   if (std::string(key) == "sweep_early_exit") { ctx->early_exit = value != 0; return 0; }
   if (std::string(key) == "row_tol_1e9")
   { // row tolerance in units of 1e-9 (10 = the default 1e-8, 1000 = Gurobi's default FeasibilityTol 1e-6).  0 is refused:
@@ -143,7 +142,6 @@ extern "C" int fq_has_feature(const char* name)
 {
   if (!name) return 0;
   const std::string n(name);
-  if (n == "cert_memo") return FQ_CERT_MEMO ? 1 : 0;
   if (n == "sweep_early_exit" || n == "replan_pairs" || n == "multi_gpu" || n == "row_tol" || n == "certificates") return 1;
   return 0;
 }
@@ -180,26 +178,6 @@ int fq_launch_solve_ctx(fq_ctx* ctx, FqKernelArgs a, int max_cand, int max_poly_
     a.first_feasible = ctx->d_first + (size_t)slot * ctx->counters_cap;
     FQ_CUDA(cudaMemsetAsync(a.first_feasible, 0xff, sizeof(unsigned long long) * (size_t)n_prob, stream));
   }
-#if FQ_CERT_MEMO
-  if (ctx->cert_memo && n_prob <= kFqMemoProbs && max_cand >= 32)
-  { // infeasibility certificates shared between the candidates of a problem (fq_kernels_t.cuh); entries of earlier
-    // launches are recognised by their salt, so nothing has to be cleared per launch
-    const size_t per_slot = (size_t)kFqMemoProbs * FQ_MEMO_NB * FQ_MEMO_BE;
-    if (!ctx->d_memo)
-    {
-      FQ_CUDA(cudaMalloc(&ctx->d_memo, sizeof(FqMemoEntry) * per_slot * kFqCounterSlots));
-      FQ_CUDA(cudaMemset(ctx->d_memo, 0, sizeof(FqMemoEntry) * per_slot * kFqCounterSlots));
-    }
-    if (++ctx->memo_salt == 0)
-    { // 2^32 launches later: start over with a clean table
-      FQ_CUDA(cudaDeviceSynchronize());
-      FQ_CUDA(cudaMemset(ctx->d_memo, 0, sizeof(FqMemoEntry) * per_slot * kFqCounterSlots));
-      ctx->memo_salt = 1;
-    }
-    a.memo = ctx->d_memo + per_slot * slot;
-    a.memo_salt = ctx->memo_salt;
-  }
-#endif
   const bool generic = ctx->force_generic || a.cert != nullptr;
   // the selection in the tail needs the specialised kernel, one problem and the coefficients of every candidate
   a.sweep_done = a.sweep_n_sigma > 0 && n_prob == 1 && a.coeffs && !generic ? counters + n_prob : nullptr;

@@ -69,9 +69,6 @@ struct fq_ctx
   int throughput_slices = 0;      // option "throughput_slices": launches a large host batch is cut into (0 = default 4)
   int max_poly_faces_hint = 0;    // option "max_faces_per_polytope" (device-pointer API only)
   double row_tol = FQ_ROW_TOL;    // option "row_tol_1e9": absolute row tolerance of every solve of this context
-  FqMemoEntry* d_memo = nullptr;  // ring of infeasibility-certificate memos: one slot per launch in flight (as d_counters)
-  unsigned memo_salt = 0;         // launch counter stamped into the memo entries (stale entries carry another value)
-  bool cert_memo = true;          // option "cert_memo"
   bool early_exit = false;        // option "sweep_early_exit": candidates that cannot win genNewTraj's selection are skipped
   unsigned long long* d_first = nullptr;   // ring (as d_counters) of per-problem "smallest feasible dt so far"
   // ---- multi-GPU (fq_multi.cu)
@@ -81,7 +78,6 @@ struct fq_ctx
   bool is_group = false;
 };
 static const int kFqCounterSlots = 64;
-static const int kFqMemoProbs = 256;      // launches with more problems run without the certificate memo
 
 // ---- helpers implemented in fq_capi.cu
 int fq_fail(fq_ctx* c, int code, const std::string& msg);

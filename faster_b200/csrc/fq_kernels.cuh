@@ -11,60 +11,10 @@
 #ifndef FQ_MIN_CTAS_WHOLE
 #define FQ_MIN_CTAS_WHOLE 4   // whole-mode kernels for N <= 10; 5 needs <= 96 registers and spills
 #endif
-#ifndef FQ_BACKSUB_PRESCALED
-#define FQ_BACKSUB_PRESCALED 1   // 0 keeps the division on the dependent chain
-#endif
-#ifndef FQ_PACKED_R
-#define FQ_PACKED_R 1         // 1: the triangular factor R is stored packed (column k at k(k+1)/2), half the bytes
-                              // (2: only in the safe-mode kernels, whose shared memory needs it); costs index arithmetic, but
-                              // it is what makes room for FQ_WARP_ADOPT
-#endif
-#ifndef FQ_WARP_ADOPT
-#define FQ_WARP_ADOPT 1       // 1: every warp adopts problems and stages polytope rows on its own (no block barriers):
-                              // faster than packed R alone
-#endif
-#ifndef FQ_SPLIT_ROWS
-#define FQ_SPLIT_ROWS 0       // 1: staged polytope rows as two arrays of 16-byte halves ([Ax Ay] and [Az b+tol]): both loads of
-                              // the row scan become bank-conflict free (rows 32 bytes apart give a two-way conflict)
-#endif
-#ifndef FQ_CONST_PRECHECK
-#define FQ_CONST_PRECHECK 1   // 1: before anything else is set up, test the three control points of segment 0 that x0 and dt fix
-                              // (cp0, cp1, cp2: their plan rows are zero) against the faces of sigma[0]; a violated one
-                              // refutes the candidate (what the solve would find in its first iteration, same arithmetic)
-#endif
-#ifndef FQ_EE_CAP_ALWAYS
-#define FQ_EE_CAP_ALWAYS 0     // 1: cap the grid of an early-exit sweep even when the whole sweep fits the GPU at once (tuning)
-#endif
-#ifndef FQ_SCAN_UNROLL
-#define FQ_SCAN_UNROLL 1       // unroll factor of the corridor-row scan (more loads in flight per warp)
-#endif
-#ifndef FQ_MIN_REDUX
-#define FQ_MIN_REDUX 1         // 1: the ratio test's warp minimum through two integer redux.sync on the order-preserving bit
-                               // pattern of the doubles (exact) instead of five dependent shuffle + min rounds
-                               // (a shorter dependent chain per iteration)
-#endif
-#ifndef FQ_GI_HOIST
-#define FQ_GI_HOIST 0          // 1: the lane's (axis, column) of the entering row's normal computed once per candidate and the
-                               // per-iteration code branch-free.  Slower (two more live registers): off
-#endif
-#ifndef FQ_ITEMS_BY_SEGMENT
-#define FQ_ITEMS_BY_SEGMENT 0  // 1: the corridor item list written by two lanes per segment (even / odd faces) instead of one
-                               // lane per item with a four-step search for its segment.  Slower: off
-#endif
 #ifndef FQ_MAX_N_3CTAS
 #define FQ_MAX_N_3CTAS 15      // largest N whose kernels are compiled for 3 CTAs per SM (<= 168 registers); beyond: 2 CTAs.  N = 14, 15
                                // run 2 CTAs per SM anyway (shared memory), yet letting the compiler take 223 registers there was
                                // slower on config 5: the bound stays
-#endif
-#ifndef FQ_LAZY_LEAVING
-#define FQ_LAZY_LEAVING 0      // 1: the index of the blocking row (ballot + shuffle) is looked up only when a partial step is taken.
-                               // No measurable change (tools/kernel_ab.py): off
-#endif
-#ifndef FQ_SCAN_ARGMAX
-#define FQ_SCAN_ARGMAX 0       // 1: the scan remembers WHICH control point of the winning (segment, face) item ranked highest (two
-                               // bits of the code) instead of re-evaluating the item's four points when the entering row is decoded:
-                               // same keys, same order, same choice.  Inside the noise
-                               // of a kernel A/B (alone and with FQ_LAZY_LEAVING): left off
 #endif
 #define FQ_EPS_DEP 1e-18      // squared sine below which a new normal counts as dependent on the active set
 #define FQ_ZZ_FLOOR 1e-30
@@ -97,9 +47,6 @@ struct FqKernelArgs
   double* coeffs;        // n_cand x N x 12 or nullptr
   int32_t* iters;        // or nullptr
   double row_tol;        // absolute row tolerance (default FQ_ROW_TOL; option "row_tol_1e9")
-  // infeasibility-certificate memo of this launch (fq_kernels_t.cuh), or nullptr: n_prob x FQ_MEMO_NB x FQ_MEMO_BE entries
-  struct FqMemoEntry* memo;
-  unsigned memo_salt;    // unique per launch of a context: entries carrying another salt are stale
   // "first feasible dt wins" early exit (option "sweep_early_exit"; specialised kernel only): per problem the smallest dt
   // (bit pattern) of a candidate found feasible so far, or nullptr.  Candidates with a larger dt are not evaluated.
   unsigned long long* first_feasible;
@@ -116,25 +63,6 @@ struct FqKernelArgs
   double* cert;
   int cert_stride;
 };
-
-// One shared infeasibility certificate: "at time allocation dt (bit pattern), the rows of the segments in `mask` with the
-// polytopes `sigpack` (4 bits per segment) have no common point with the box rows".  w0 = salt << 32 | mask << 16 | count
-// slot + 1; written last, after a fence.
-struct FqMemoEntry
-{
-  unsigned long long w0, dt_bits, sigpack;
-};
-#define FQ_MEMO_NB 16         // buckets per problem (hash of dt)
-#define FQ_MEMO_BE 16         // entries per bucket: one per lane of a half warp
-#ifndef FQ_CERT_MEMO
-#define FQ_CERT_MEMO 0        // 1 compiles the memo in.  Slower on the bench workload (tools/ab.sh, cfg4 chain), even
-                              // switched off (the bookkeeping of the active rows' segments).  With thousands of warps working on
-                              // 64 corridors at once and a few dozen candidates per warp per launch, few candidates start after a
-                              // useful proof exists (a scheduling model of the launch finds few hits), and the
-                              // commonest proofs (a constant control point of segment 0 outside its polytope) already cost a
-                              // single iteration.  It pays on the CPU port (few workers, deep queues), where it is on.
-#endif
-#define FQ_MEMO_MARGIN 1e-5   // certificates are recorded only when the violation exceeds this x (1 + sum |multipliers|)
 
 struct FqSelectArgs
 {

@@ -39,16 +39,15 @@ struct Dims
   static constexpr int NW = 3 * NZ;
   static constexpr int NY = 6 * N_ + 1;
   static constexpr int NYP = NY | 1;             // odd row stride of Y per axis
-  static constexpr int LD = NW | 1;              // odd leading dimension of J and R
+  static constexpr int LD = NW | 1;              // odd leading dimension of J
   static constexpr int TZLD = NZ | 1;            // odd row stride of TZ in shared memory
   static constexpr int SLOTS = (NW + 31) / 32;   // elements of an NW-vector per lane
   static constexpr int RPL = (NY + 31) / 32;     // Y rows per lane
-  static constexpr bool PACKED = FQ_PACKED_R == 2 ? !WHOLE_ : (FQ_PACKED_R != 0);   // 2: only where the room is needed
-  static constexpr int RSZ = PACKED ? NW * (NW + 1) / 2 : NW * LD;        // doubles of the triangular factor
-  static constexpr int JR = NW * LD + RSZ;                                // J then R, contiguous
+  static constexpr int RSZ = NW * (NW + 1) / 2;  // doubles of the packed triangular factor
+  static constexpr int JR = NW * LD + RSZ;       // J then R, contiguous
   static constexpr int PER_WARP_DOUBLES = JR + 3 * NYP + 3 * NW + 2;
-  // element (row j, column k), j <= k, of R
-  __host__ __device__ static constexpr int ri(int j, int k) { return PACKED ? (k * (k + 1)) / 2 + j : k * LD + j; }
+  // element (row j, column k), j <= k, of R: column k starts at k(k+1)/2
+  __host__ __device__ static constexpr int ri(int j, int k) { return (k * (k + 1)) / 2 + j; }
 };
 // per-warp bytes: solver state + item list (item_cap 16-bit entries)
 template <class D>
@@ -88,7 +87,6 @@ __device__ __forceinline__ double warp_sum(double v)
 }
 __device__ __forceinline__ double warp_min(double v)
 {
-#if FQ_MIN_REDUX
   // order-preserving integer image of a double (no NaN here): for negative values the magnitude bits are inverted, so the
   // signed order of the hi words and the unsigned order of the lo words are the numeric order; two redux.sync give the
   // exact minimum
@@ -99,43 +97,33 @@ __device__ __forceinline__ double warp_min(double v)
   const unsigned ml = __reduce_min_sync(FULL, khi == mh ? klo : 0xffffffffu);
   const int mneg = mh >> 31;
   return __hiloint2double(mh ^ (mneg & 0x7fffffff), (int)(ml ^ (unsigned)mneg));
-#else
-#pragma unroll
-  for (int o = 16; o; o >>= 1) v = fmin(v, __shfl_xor_sync(FULL, v, o));
-  return v;
-#endif
 }
 
-// staged polytope rows: row gf = (a01 = [Ax Ay], a23 = [Az b+tol]); interleaved (32-byte rows) or split into two arrays
-// of 16-byte halves `half_ofs` doubles apart (FQ_SPLIT_ROWS; half_ofs = 2 * max_faces)
-__device__ __forceinline__ double2 row_a01(const double* __restrict__ sAb, int gf, int half_ofs)
+// staged polytope rows, 32 bytes each: row gf = (a01 = [Ax Ay], a23 = [Az b+tol])
+__device__ __forceinline__ double2 row_a01(const double* __restrict__ sAb, int gf)
 {
-  (void)half_ofs;
-  return *reinterpret_cast<const double2*>(sAb + (FQ_SPLIT_ROWS ? 2 : 4) * gf);
+  return *reinterpret_cast<const double2*>(sAb + 4 * gf);
 }
-__device__ __forceinline__ double2 row_a23(const double* __restrict__ sAb, int gf, int half_ofs)
+__device__ __forceinline__ double2 row_a23(const double* __restrict__ sAb, int gf)
 {
-  return *reinterpret_cast<const double2*>(sAb + (FQ_SPLIT_ROWS ? half_ofs + 2 * gf : 4 * gf + 2));
+  return *reinterpret_cast<const double2*>(sAb + 4 * gf + 2);
 }
 // staging: double2 number i of the source rows (even: [Ax Ay] of row i/2, odd: [Az b] of row i/2)
-__device__ __forceinline__ void row_store(double* __restrict__ sAb, int i, int half_ofs, double2 v)
+__device__ __forceinline__ void row_store(double* __restrict__ sAb, int i, double2 v)
 {
-  double2* dst = reinterpret_cast<double2*>(sAb);
-  if (FQ_SPLIT_ROWS) dst[(i & 1) ? (half_ofs >> 1) + (i >> 1) : (i >> 1)] = v;
-  else dst[i] = v;
+  reinterpret_cast<double2*>(sAb)[i] = v;
 }
 
 template <class D>
 struct WarpState
 {
   double* J;            // NW x LD row-major
-  double* R;            // upper triangular, column-major: R(j,k) at R[D::ri(j,k)] (packed when FQ_PACKED_R)
+  double* R;            // upper triangular, packed column-major: R(j,k) at R[D::ri(j,k)]
   double* Y;            // 3 x NYP
   double* w;            // NW
   double* d;            // NW
   double* zb;           // NW: scratch for the re-orthogonalisation pass
   unsigned short* items;
-  int half_ofs;         // FQ_SPLIT_ROWS: distance in doubles between the two halves of the staged rows
 };
 
 // Ranking key of a row: hi word of (violation - tol) * S[y] as a signed int, S[y] = 1/|TZ[y]| (distance of the
@@ -192,43 +180,28 @@ __device__ __forceinline__ void update_Y(const WarpState<D>& m, const double* __
 }
 
 // remove active element l (0 <= l < q); lam / rdinv are per-lane register slots
-template <class D, bool CERT>
+template <class D>
 __device__ __forceinline__ void drop_row(const WarpState<D>& m, int lane, int l, int q, double (&lam)[D::SLOTS],
-                                         double (&rdinv)[D::SLOTS], int (&aseg)[D::SLOTS])
+                                         double (&rdinv)[D::SLOTS])
 {
   constexpr int LD = D::LD;
+  // The columns right of l move one place left and become upper Hessenberg: the element below the new diagonal of
+  // column k is the OLD diagonal of column k+1.  Packed storage has no room for it, so each lane keeps the old
+  // diagonal of "its" column in a register; rotation j reads it by shuffle (no earlier rotation touches row j+1).
   double dg[D::SLOTS];
-  if constexpr (D::PACKED)
+#pragma unroll
+  for (int s = 0; s < D::SLOTS; s++)
   {
-    // The columns right of l move one place left and become upper Hessenberg: the element below the new diagonal of
-    // column k is the OLD diagonal of column k+1.  Packed storage has no room for it, so each lane keeps the old
-    // diagonal of "its" column in a register; rotation j reads it by shuffle (no earlier rotation touches row j+1).
-#pragma unroll
-    for (int s = 0; s < D::SLOTS; s++)
-    {
-      const int k = lane + 32 * s;
-      dg[s] = k < q ? m.R[D::ri(k, k)] : 0.0;
-    }
-    __syncwarp();
-#pragma unroll
-    for (int s = 0; s < D::SLOTS; s++)
-    {
-      const int j = lane + 32 * s;                 // this lane moves row j of every column that keeps a row j
-      if (j < q)
-        for (int k = (l > j ? l : j); k < q - 1; k++) m.R[D::ri(j, k)] = m.R[D::ri(j, k + 1)];
-    }
+    const int k = lane + 32 * s;
+    dg[s] = k < q ? m.R[D::ri(k, k)] : 0.0;
   }
-  else
-  {
-    // R: columns l+1..q-1 move left (each lane moves its own rows)
+  __syncwarp();
 #pragma unroll
-    for (int s = 0; s < D::SLOTS; s++)
-    {
-      const int j = lane + 32 * s;
-      dg[s] = 0.0;
-      if (j < q)
-        for (int k = l; k < q - 1; k++) m.R[k * LD + j] = m.R[(k + 1) * LD + j];
-    }
+  for (int s = 0; s < D::SLOTS; s++)
+  {
+    const int j = lane + 32 * s;                 // this lane moves row j of every column that keeps a row j
+    if (j < q)
+      for (int k = (l > j ? l : j); k < q - 1; k++) m.R[D::ri(j, k)] = m.R[D::ri(j, k + 1)];
   }
   // lam: element k <- element k+1 for k in [l, q-1)
   {
@@ -246,35 +219,13 @@ __device__ __forceinline__ void drop_row(const WarpState<D>& m, int lane, int l,
       const int k = lane + 32 * s;
       if (k >= l && k < q - 1) lam[s] = nxt[s];
     }
-    if constexpr (CERT)
-    { // the segment tags of the active rows move with the multipliers
-      int nx[D::SLOTS];
-#pragma unroll
-      for (int s = 0; s < D::SLOTS; s++)
-      {
-        const int same = __shfl_sync(FULL, aseg[s], (lane + 1) & 31);
-        const int wrap = (s + 1 < D::SLOTS) ? __shfl_sync(FULL, aseg[(s + 1 < D::SLOTS) ? s + 1 : s], 0) : 0;
-        nx[s] = lane == 31 ? wrap : same;
-      }
-#pragma unroll
-      for (int s = 0; s < D::SLOTS; s++)
-      {
-        const int k = lane + 32 * s;
-        if (k >= l && k < q - 1) aseg[s] = nx[s];
-      }
-    }
   }
   __syncwarp();
   for (int j = l; j < q - 1; j++)
   {
-    double p, sb;
-    if constexpr (D::PACKED)
-    {
-      p = m.R[D::ri(j, j)];
-      const int js = (j + 1) >> 5;
-      sb = __shfl_sync(FULL, (D::SLOTS > 1 && js == 1) ? dg[D::SLOTS - 1] : dg[0], (j + 1) & 31);
-    }
-    else { p = m.R[j * LD + j]; sb = m.R[j * LD + j + 1]; }
+    const double p = m.R[D::ri(j, j)];
+    const int js = (j + 1) >> 5;
+    const double sb = __shfl_sync(FULL, (D::SLOTS > 1 && js == 1) ? dg[D::SLOTS - 1] : dg[0], (j + 1) & 31);
     const double h2 = fma(p, p, sb * sb);
     double c = 1.0, sn = 0.0, hi = 0.0;
     if (h2 > 0) { hi = fast_rsqrt(h2); c = p * hi; sn = sb * hi; }
@@ -283,26 +234,13 @@ __device__ __forceinline__ void drop_row(const WarpState<D>& m, int lane, int l,
     for (int s = 0; s < D::SLOTS; s++)
     {
       const int k = lane + 32 * s;
-      if constexpr (D::PACKED)
-      {
-        if (k > j && k < q - 1)
-        { // rows j, j+1 of R at column k (both inside the triangle)
-          const double u = m.R[D::ri(j, k)], v = m.R[D::ri(j + 1, k)];
-          m.R[D::ri(j, k)] = fma(c, u, sn * v);
-          m.R[D::ri(j + 1, k)] = fma(c, v, -sn * u);
-        }
-        if (k == j) { m.R[D::ri(j, j)] = fma(c, p, sn * sb); rdinv[s] = hi; }   // the element below it rotates to zero
+      if (k > j && k < q - 1)
+      { // rows j, j+1 of R at column k (both inside the triangle)
+        const double u = m.R[D::ri(j, k)], v = m.R[D::ri(j + 1, k)];
+        m.R[D::ri(j, k)] = fma(c, u, sn * v);
+        m.R[D::ri(j + 1, k)] = fma(c, v, -sn * u);
       }
-      else
-      {
-        if (k >= j && k < q - 1)
-        { // rows j, j+1 of R at column k
-          const double u = m.R[k * LD + j], v = m.R[k * LD + j + 1];
-          m.R[k * LD + j] = fma(c, u, sn * v);
-          m.R[k * LD + j + 1] = fma(c, v, -sn * u);
-        }
-        if (k == j) rdinv[s] = hi;                 // new diagonal is h = sqrt(h2)
-      }
+      if (k == j) { m.R[D::ri(j, j)] = fma(c, p, sn * sb); rdinv[s] = hi; }   // the element below it rotates to zero
       if (k < D::NW)
       { // columns j, j+1 of J at row k
         const double u = m.J[k * LD + j], v = m.J[k * LD + j + 1];
@@ -383,20 +321,6 @@ __device__ __forceinline__ int build_items(const WarpState<D>& m, const int* __r
   }
   const int total_rows = __shfl_sync(FULL, incl, n_seg - 1);
   if (total_rows > item_cap) return -1;     // a wrong max_faces_per_polytope hint (device-pointer entry): refuse, never overrun
-#if FQ_ITEMS_BY_SEGMENT
-  { // lanes tl and tl + 16 write the items of segment tl (even / odd faces), same order as the list built item by item
-    (void)seg_ofs;
-    const int tl = lane & 15;
-    const int first = __shfl_sync(FULL, incl - F, tl);
-    const int meta = __shfl_sync(FULL, (need0 << 11) | sfo[lane < n_seg ? p : 0], tl);
-    const int Ft = __shfl_sync(FULL, F, tl);                 // 0 beyond the last segment
-    const int Fmax = __reduce_max_sync(FULL, F);
-    for (int f = lane >> 4; f < Fmax; f += 2)
-      if (f < Ft) m.items[first + f] = (unsigned short)((tl << 12) | (meta + f));
-    __syncwarp();
-    return total_rows;
-  }
-#endif
   // seg_ofs[t] = first item of segment t; seg_ofs[16 + t] = (need_cp0 << 11) | first staged face of sigma[t]
   if (lane < n_seg) { seg_ofs[lane] = incl - F; seg_ofs[16 + lane] = (need0 << 11) | sfo[p]; }
   else if (lane < 16) seg_ofs[lane] = 0x7fffffff;
@@ -419,67 +343,38 @@ __device__ __forceinline__ int build_items(const WarpState<D>& m, const int* __r
 // cannot be reached (0) or the iteration cap / a NaN is hit (-1).  Enabled rows = box rows + the `total_rows` items of
 // m.items.  Used by the fixed-assignment solve below and by the branch-and-bound node solve (fq_bnb.cuh), which enters
 // with a parent's factorisation instead of the identity.
-// CERT: also keep, per active row, the segment it belongs to (0 = box row) and, when the iteration ends "infeasible" with
-// a violation well beyond the tolerance band, return in `cert_mask` the set of segments whose rows (together with box rows)
-// form the Farkas certificate: the entering row and the active rows with a negative multiplier r_k (g_e = sum r_k n_k,
-// r <= 0, active rows tight, row e violated => no point satisfies them all).  cert_mask < 0: no certificate recorded.
-template <class D, bool CERT = false>
+template <class D>
 __device__ __forceinline__ int gi_loop(const WarpState<D>& m, const double* __restrict__ TZ, const double* __restrict__ SY,
                                        const double* __restrict__ sAb, const double (&Yeq)[D::RPL][3],
                                        const double (&bthr)[D::RPL], int lane, int total_rows, double inv1, double inv2,
                                        double inv3, double lim0, double lim1, double lim2, double row_tol,
                                        double (&lam)[D::SLOTS], double (&rdinv)[D::SLOTS], int& q, int& it, int bkey,
-                                       unsigned bcode, int* cert_mask = nullptr)
+                                       unsigned bcode)
 {
   constexpr int N = D::N, NZ = D::NZ, NW = D::NW, NYP = D::NYP, LD = D::LD, SLOTS = D::SLOTS;
   double r[SLOTS], z[SLOTS], dreg[SLOTS];
-  int aseg[SLOTS];
 #pragma unroll
-  for (int s = 0; s < SLOTS; s++) { r[s] = 0; z[s] = 0; dreg[s] = 0; aseg[s] = 0; }
-#if FQ_GI_HOIST
-  int gcol[SLOTS];                                    // variable j = lane + 32 s of w: axis << 8 | column of the plan table
-#pragma unroll
-  for (int s = 0; s < SLOTS; s++)
-  {
-    const int j = lane + 32 * s, ax = j / NZ;
-    gcol[s] = j < NW ? (ax << 8) | (j - ax * NZ) : (3 << 8);
-  }
-#endif
+  for (int s = 0; s < SLOTS; s++) { r[s] = 0; z[s] = 0; dreg[s] = 0; }
   int status = -2;
   while (status == -2)
   {
     // ================= most violated corridor row (box rows were checked by update_Y) =================
-    constexpr int SCAN_UNROLL = FQ_SCAN_UNROLL;
-#pragma unroll SCAN_UNROLL
+#pragma unroll 1
     for (int i = lane; i < total_rows; i += 32)
     {
       const unsigned item = m.items[i];
       const int t = item >> 12, gf = item & 0x7ff;
-      const double2 a01 = row_a01(sAb, gf, m.half_ofs);
-      const double2 a23 = row_a23(sAb, gf, m.half_ofs);                             // a23.y = b + tol
+      const double2 a01 = row_a01(sAb, gf);
+      const double2 a23 = row_a23(sAb, gf);                                         // a23.y = b + tol
       const double* Y0 = m.Y; const double* Y1 = m.Y + NYP; const double* Y2 = m.Y + 2 * NYP;
       const int y1 = 4 * N + 1 + t, y2 = 5 * N + 1 + t;
       const double u1 = fma(a01.x, Y0[y1], fma(a01.y, Y1[y1], fma(a23.x, Y2[y1], -a23.y))) * SY[y1];
       const double u2 = fma(a01.x, Y0[y2], fma(a01.y, Y1[y2], fma(a23.x, Y2[y2], -a23.y))) * SY[y2];
       const double u3 = fma(a01.x, Y0[t + 1], fma(a01.y, Y1[t + 1], fma(a23.x, Y2[t + 1], -a23.y))) * SY[t + 1];
-#if FQ_SCAN_ARGMAX
-      // first maximum in the order (cp1, cp2, cp3, cp0): the order in which the decode below used to re-evaluate them
-      int km = rank_key(u1);
-      unsigned wq = 0;
-      { const int k2 = rank_key(u2); if (k2 > km) { km = k2; wq = 1u << 28; } }
-      { const int k3 = rank_key(u3); if (k3 > km) { km = k3; wq = 2u << 28; } }
-      if (item & 0x800u)
-      {
-        const int k0 = rank_key(fma(a01.x, Y0[t], fma(a01.y, Y1[t], fma(a23.x, Y2[t], -a23.y))) * SY[t]);
-        if (k0 > km) { km = k0; wq = 3u << 28; }
-      }
-      if (km > bkey) { bkey = km; bcode = (unsigned)i | wq; }
-#else
       int km = max(max(rank_key(u1), rank_key(u2)), rank_key(u3));
       if (item & 0x800u)
         km = max(km, rank_key(fma(a01.x, Y0[t], fma(a01.y, Y1[t], fma(a23.x, Y2[t], -a23.y))) * SY[t]));
       if (km > bkey) { bkey = km; bcode = (unsigned)i; }
-#endif
     }
     const int mk = __reduce_max_sync(FULL, bkey);
     if (mk <= 0) { status = 1; break; }
@@ -487,7 +382,7 @@ __device__ __forceinline__ int gi_loop(const WarpState<D>& m, const double* __re
     const int src = __ffs(__ballot_sync(FULL, key == mk)) - 1;
     const unsigned code = __shfl_sync(FULL, bcode, src);
     // ---- decode the chosen row: Y row y, weights (w0,w1,w2), right-hand side h
-    int y, eseg = 0;
+    int y;
     double w0 = 0, w1 = 0, w2 = 0, h;
     if (code & BOX_FLAG)
     {
@@ -503,15 +398,10 @@ __device__ __forceinline__ int gi_loop(const WarpState<D>& m, const double* __re
     {
       const unsigned item = m.items[code & 0x0fffffffu];
       const int t = item >> 12, gf = item & 0x7ff;
-      eseg = t + 1;
-      const double2 r01 = row_a01(sAb, gf, m.half_ofs), r23 = row_a23(sAb, gf, m.half_ofs);
+      const double2 r01 = row_a01(sAb, gf), r23 = row_a23(sAb, gf);
       w0 = r01.x; w1 = r01.y; w2 = r23.x;
       const double hb = r23.y;                      // b + tol
       h = hb - row_tol;
-#if FQ_SCAN_ARGMAX
-      const unsigned wq = (code >> 28) & 3u;        // the control point the scan ranked highest: cp1, cp2, cp3, cp0
-      y = wq == 0 ? 4 * N + 1 + t : (wq == 1 ? 5 * N + 1 + t : (wq == 2 ? t + 1 : t));
-#else
       const int ys[4] = { 4 * N + 1 + t, 5 * N + 1 + t, t + 1, t };
       y = ys[0];
       int best = -0x7fffffff;
@@ -522,10 +412,11 @@ __device__ __forceinline__ int gi_loop(const WarpState<D>& m, const double* __re
         const int kk = rank_key(fma(w0, m.Y[ys[k]], fma(w1, m.Y[NYP + ys[k]], fma(w2, m.Y[2 * NYP + ys[k]], -hb))) * SY[ys[k]]);
         if (kk > best) { best = kk; y = ys[k]; }
       }
-#endif
     }
     const double sy = SY[y];
-    const double gg = (w0 * w0 + w1 * w1 + w2 * w2) * fast_rcp(sy * sy);   // |g|^2 = |w|^2 |TZ[y]|^2
+    // |g|^2 = |w|^2 |TZ[y]|^2; the fma chain is spelled out so that the rounding of |w|^2 does not depend on which
+    // product the compiler chooses to contract
+    const double gg = fma(w2, w2, fma(w0, w0, w1 * w1)) * fast_rcp(sy * sy);
     double lam_p = 0;
     for (;;)
     {
@@ -564,14 +455,8 @@ __device__ __forceinline__ int gi_loop(const WarpState<D>& m, const double* __re
           dreg[s] = fma(w0, s0[s], fma(w1, s1[s], w2 * s2[s]));
           if (j < q) m.d[j] = dreg[s];
           // this lane's component of g: variable j = (axis, column) of the plan table
-#if FQ_GI_HOIST
-          const int ax = gcol[s] >> 8;
-          const double wsel = ax == 0 ? w0 : (ax == 1 ? w1 : (ax == 2 ? w2 : 0.0));
-          gi[s] = wsel * TZ[y * D::TZLD + (gcol[s] & 0xff)];
-#else
           const int ax = j / NZ, kk = j - ax * NZ;
           gi[s] = j < NW ? (ax == 0 ? w0 : (ax == 1 ? w1 : w2)) * TZ[y * D::TZLD + kk] : 0.0;
-#endif
         }
       }
       __syncwarp();
@@ -647,7 +532,6 @@ __device__ __forceinline__ int gi_loop(const WarpState<D>& m, const double* __re
         }
       }
       // ---- r = R^-1 d1 (registers + shuffles)
-#if FQ_BACKSUB_PRESCALED
       // every lane pre-divides its own row by the diagonal (R(j,k) / R(j,j) does not depend on r_k), so the chain from
       // one r_k to the next is a shuffle and one FMA
 #pragma unroll
@@ -663,23 +547,6 @@ __device__ __forceinline__ int gi_loop(const WarpState<D>& m, const double* __re
           if (j < k) r[s] = fma(-m.R[D::ri(j, k)] * rdinv[s], rk, r[s]);
         }
       }
-#else
-#pragma unroll
-      for (int s = 0; s < SLOTS; s++) r[s] = dreg[s];
-      for (int k = q - 1; k >= 0; k--)
-      {
-        const int ks = k >> 5;
-        double rk = (SLOTS > 1 && ks == 1) ? r[SLOTS - 1] * rdinv[SLOTS - 1] : r[0] * rdinv[0];
-        rk = __shfl_sync(FULL, rk, k & 31);
-#pragma unroll
-        for (int s = 0; s < SLOTS; s++)
-        {
-          const int j = lane + 32 * s;
-          if (j < k) r[s] = fma(-m.R[D::ri(j, k)], rk, r[s]);
-          else if (j == k) r[s] = rk;
-        }
-      }
-#endif
       // ---- dual ratio test and the step scalars
       double best = INFINITY;
       int bk = -1;
@@ -700,33 +567,13 @@ __device__ __forceinline__ int gi_loop(const WarpState<D>& m, const double* __re
       // further column would not fit the factorisation's storage)
       const bool dep = zz <= fmax(FQ_EPS_DEP * gg, FQ_ZZ_FLOOR) || q >= NW;
       int l = -1;
-#if !FQ_LAZY_LEAVING
       if (t1 < INFINITY)
       {
         const int s2 = __ffs(__ballot_sync(FULL, best == t1)) - 1;
         l = __shfl_sync(FULL, bk, s2);
       }
-#endif
       const double t2 = dep ? INFINITY : viol * rzz;
-      if (t1 == INFINITY && t2 == INFINITY)
-      {
-        status = 0;
-        if constexpr (CERT)
-        {
-          double sr = 0;
-          unsigned mk2 = eseg ? 1u << (eseg - 1) : 0u;
-#pragma unroll
-          for (int s = 0; s < SLOTS; s++)
-          {
-            const int k = lane + 32 * s;
-            if (k < q && r[s] < 0) { sr -= r[s]; if (aseg[s]) mk2 |= 1u << (aseg[s] - 1); }
-          }
-          sr = warp_sum(sr);
-          mk2 = __reduce_or_sync(FULL, mk2);
-          *cert_mask = viol > FQ_MEMO_MARGIN * (1.0 + sr) ? (int)mk2 : -1;
-        }
-        break;
-      }
+      if (t1 == INFINITY && t2 == INFINITY) { status = 0; break; }
       if (t2 <= t1)
       { // ---- full step: the row becomes active; new basis vector = normalised residual of g
         const double nrm = zz * rn;
@@ -740,7 +587,7 @@ __device__ __forceinline__ int gi_loop(const WarpState<D>& m, const double* __re
             m.J[i * LD + q] = -z[s] * rn;
           }
           if (i < q) { lam[s] = fma(-t2, r[s], lam[s]); m.R[D::ri(i, q)] = dreg[s]; }
-          if (i == q) { lam[s] = lam_p + t2; rdinv[s] = rn; m.R[D::ri(q, q)] = nrm; if constexpr (CERT) aseg[s] = eseg; }
+          if (i == q) { lam[s] = lam_p + t2; rdinv[s] = rn; m.R[D::ri(q, q)] = nrm; }
         }
         q++;
         __syncwarp();
@@ -749,13 +596,6 @@ __device__ __forceinline__ int gi_loop(const WarpState<D>& m, const double* __re
         break;
       }
       // ---- partial step: active element l leaves.  (l < 0 here means t1/t2 are NaN -- non-finite input: give up)
-#if FQ_LAZY_LEAVING
-      if (t1 < INFINITY)
-      {
-        const int s2 = __ffs(__ballot_sync(FULL, best == t1)) - 1;
-        l = __shfl_sync(FULL, bk, s2);
-      }
-#endif
       if (l < 0) { status = -1; break; }
 #pragma unroll
       for (int s = 0; s < SLOTS; s++)
@@ -766,7 +606,7 @@ __device__ __forceinline__ int gi_loop(const WarpState<D>& m, const double* __re
       }
       lam_p += t1;
       __syncwarp();
-      drop_row<D, CERT>(m, lane, l, q, lam, rdinv, aseg);
+      drop_row<D>(m, lane, l, q, lam, rdinv);
       q--;
       if (!dep)
       {
@@ -778,34 +618,6 @@ __device__ __forceinline__ int gi_loop(const WarpState<D>& m, const double* __re
   }
 
   return status;
-}
-
-// ---- infeasibility-certificate memo (FqMemoEntry, fq_kernels.cuh) ---------------------------------------------------
-// When gi_loop ends "infeasible", the entering row e and the active rows k with r_k < 0 form a Farkas certificate that
-// does not depend on the candidate's other rows: every candidate of the same problem with the same dt and the same
-// polytope on the segments those rows belong to contains the same rows (box rows are common to all) and is infeasible
-// too.  The ascending time-allocation sweep of genNewTraj starts at an optimistic dt by design (solverGurobi.cpp:445-446),
-// so whole runs of candidates are refuted by the |v|,|a|,|j| boxes alone or by the first segments' rows; they are
-// answered from the memo instead of being re-proved.  Flags stay exact: only proofs are shared, and only those whose
-// violation is far outside the tolerance band (FQ_MEMO_MARGIN).
-__device__ __forceinline__ int memo_bucket(unsigned long long dtb)
-{
-  return (int)((dtb * 0x9E3779B97F4A7C15ull) >> 40) & (FQ_MEMO_NB - 1);
-}
-__device__ __forceinline__ unsigned long long memo_sigpack(int lane, int N, int p)
-{ // 4 bits per segment
-  unsigned lo = 0, hi = 0;
-  if (lane < N) { if (lane < 8) lo = (unsigned)p << (4 * lane); else hi = (unsigned)p << (4 * (lane - 8)); }
-  lo = __reduce_or_sync(FULL, lo);
-  hi = __reduce_or_sync(FULL, hi);
-  return (unsigned long long)hi << 32 | lo;
-}
-__device__ __forceinline__ unsigned long long memo_nibbles(unsigned mask)
-{ // bit t of mask -> nibble t = 0xF
-  unsigned long long r = 0;
-#pragma unroll
-  for (int t = 0; t < 16; t++) r |= (unsigned long long)((mask >> t) & 1u) * (0xfull << (4 * t));
-  return r;
 }
 
 template <class D>
@@ -855,42 +667,6 @@ __device__ void solve_candidate(const FqKernelArgs& a, const double* __restrict_
       p = a.sigma[(size_t)cand * N + lane];
       if (p >= P) p = P - 1;
     }
-#if FQ_CERT_MEMO
-    // ---- has another candidate of this problem already proved these rows infeasible at this dt?  (see memo_insert)
-    if (a.memo && P <= 16)
-    {
-      const unsigned long long dtb = (unsigned long long)__double_as_longlong(dt);
-      const unsigned long long sigpack = memo_sigpack(lane, N, p);
-      const FqMemoEntry* e = a.memo + ((size_t)prob * FQ_MEMO_NB + memo_bucket(dtb)) * FQ_MEMO_BE;
-      bool hit = false;
-      if (lane < FQ_MEMO_BE)
-      {
-        const unsigned long long w0 = *reinterpret_cast<const volatile unsigned long long*>(&e[lane].w0);
-        if ((unsigned)(w0 >> 32) == a.memo_salt && (w0 & 0xffffu) != 0)
-        {
-          __threadfence();                               // the entry's other words were written before w0
-          const unsigned long long d = *reinterpret_cast<const volatile unsigned long long*>(&e[lane].dt_bits);
-          const unsigned long long sp = *reinterpret_cast<const volatile unsigned long long*>(&e[lane].sigpack);
-          __threadfence();
-          const unsigned long long w0b = *reinterpret_cast<const volatile unsigned long long*>(&e[lane].w0);
-          hit = w0b == w0 && d == dtb && ((sp ^ sigpack) & memo_nibbles((unsigned)(w0 >> 16) & 0xffffu)) == 0;
-        }
-      }
-      if (__any_sync(FULL, hit))
-      { // same rows, same dt: infeasible, by the recorded certificate (iters = 0 marks the shortcut)
-        if (lane == 0)
-        {
-          a.feasible[cand] = 0;
-          a.cost[cand] = INFINITY;
-          if (a.iters) a.iters[cand] = 0;
-        }
-        if (a.coeffs)
-          for (int idx = lane; idx < 12 * N; idx += 32) a.coeffs[(size_t)cand * N * 12 + idx] = 0.0;
-        return;
-      }
-    }
-#endif
-#if FQ_CONST_PRECHECK
     // ---- control points 0..2 of segment 0 depend on x0 and dt only (rows 0, 4N+1, 5N+1 of the plan are zero, SY = 1e15):
     //      one outside a face of sigma[0] refutes the candidate.  Same expression and rank key as the scan of gi_loop,
     //      which would pick such a row first (SY outranks everything) and stop on it: flags are unchanged, iters = 1.
@@ -907,7 +683,7 @@ __device__ void solve_candidate(const FqKernelArgs& a, const double* __restrict_
         bool out = false;
         for (int gf = sfo[p0] + lane; gf < sfo[p0 + 1]; gf += 32)
         {
-          const double2 a01 = row_a01(sAb, gf, m.half_ofs), a23 = row_a23(sAb, gf, m.half_ofs);
+          const double2 a01 = row_a01(sAb, gf), a23 = row_a23(sAb, gf);
 #pragma unroll
           for (int k = 0; k < 3; k++)
             out = out || rank_key(fma(a01.x, c[k][0], fma(a01.y, c[k][1], fma(a23.x, c[k][2], -a23.y))) * 1e15) > 0;
@@ -926,7 +702,6 @@ __device__ void solve_candidate(const FqKernelArgs& a, const double* __restrict_
         }
       }
     }
-#endif
     total_rows = build_items<D>(m, sfo, seg_ofs, lane, N, p, a.item_cap);
     if (total_rows < 0)
     { // the row list does not fit: report "not solved" (iters = -2 marks the cause)
@@ -957,38 +732,8 @@ __device__ void solve_candidate(const FqKernelArgs& a, const double* __restrict_
   int bkey = 0;
   unsigned bcode = 0;
   update_Y<D, true>(m, TZ, Yeq, bthr, SY, lane, bkey, bcode);
-#if FQ_CERT_MEMO
-  int cert = -1;
-  const int status = gi_loop<D, true>(m, TZ, SY, sAb, Yeq, bthr, lane, total_rows, inv1, inv2, inv3, lim0, lim1, lim2, a.row_tol,
-                                      lam, rdinv, q, it, bkey, bcode, &cert);
-  if (status == 0 && cert >= 0 && a.memo && P > 0 && P <= 16)
-  { // share the proof with the problem's other candidates: same dt + same polytopes on the certificate's segments
-    int p = 0;
-    if (lane < N) { p = a.sigma[(size_t)cand * N + lane]; if (p >= P) p = P - 1; }
-    const unsigned long long dtb = (unsigned long long)__double_as_longlong(dt);
-    const unsigned long long sigpack = memo_sigpack(lane, N, p);
-    if (lane == 0)
-    {
-      FqMemoEntry* e = a.memo + ((size_t)prob * FQ_MEMO_NB + memo_bucket(dtb)) * FQ_MEMO_BE;
-      // slot = first entry of the bucket not yet taken in this launch (the low 16 bits of w0 hold slot + 1)
-      for (int i = 0; i < FQ_MEMO_BE; i++)
-      {
-        const unsigned long long cur = *reinterpret_cast<volatile unsigned long long*>(&e[i].w0);
-        if ((unsigned)(cur >> 32) == a.memo_salt) continue;                 // taken (or being written) in this launch
-        const unsigned long long claim = (unsigned long long)a.memo_salt << 32;      // taken, not yet valid (count field 0)
-        if (atomicCAS(&e[i].w0, cur, claim) != cur) continue;
-        __threadfence();
-        e[i].dt_bits = dtb; e[i].sigpack = sigpack;
-        __threadfence();
-        *reinterpret_cast<volatile unsigned long long*>(&e[i].w0) = claim | ((unsigned long long)(cert & 0xffff) << 16) | (unsigned)(i + 1);
-        break;
-      }
-    }
-  }
-#else
   const int status = gi_loop<D>(m, TZ, SY, sAb, Yeq, bthr, lane, total_rows, inv1, inv2, inv3, lim0, lim1, lim2, a.row_tol,
                                 lam, rdinv, q, it, bkey, bcode);
-#endif
 
   // ================= outputs =================
   double cp = 0;
@@ -1065,24 +810,20 @@ __device__ void sweep_tail_select(const FqKernelArgs& a, int c_begin, int count,
   __threadfence_system();
 }
 
-// Persistent CTAs.  counters[j] = next unclaimed candidate of problem j (zeroed before the launch).  A CTA (or, with
-// FQ_WARP_ADOPT, every warp on its own) adopts a problem that still has unclaimed candidates (scanning from its own start
-// so the adopters spread over the problems), stages the problem's polytope rows once, and claims candidates one by one
-// with a global atomic until the problem is drained; several adopters may drain the same problem.
-//   FQ_WARP_ADOPT = 0: rows staged once per CTA; block-wide barriers when the CTA changes problem.
-//   FQ_WARP_ADOPT = 1: rows staged per warp (W copies); no barrier after the plan tables are staged, a warp never waits
-//                      for its CTA-mates' last solves.
+// Persistent CTAs.  counters[j] = next unclaimed candidate of problem j (zeroed before the launch).  Every warp on its own
+// adopts a problem that still has unclaimed candidates (scanning from its own start so the adopters spread over the
+// problems), stages the problem's polytope rows into its own copy, and claims candidates one by one with a global atomic
+// until the problem is drained; several adopters may drain the same problem.  No barrier follows the staging of the plan
+// tables: a warp never waits for its CTA-mates' last solves.
 template <int N_, bool WHOLE_>
 __global__ void __launch_bounds__(W * 32, (N_ <= 10 ? (WHOLE_ ? FQ_MIN_CTAS_WHOLE : FQ_MIN_CTAS_PER_SM) : (N_ <= FQ_MAX_N_3CTAS ? 3 : 2)))
     fq_solve_kernel_t(const FqKernelArgs a, int* __restrict__ counters)
 {
   using D = Dims<N_, WHOLE_>;
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  __shared__ int s_prob;
-  constexpr int SAB_COPIES = FQ_WARP_ADOPT ? W : 1;
 
   double* sm = reinterpret_cast<double*>(smem_raw);
-  double* sAb0 = sm;           sm += SAB_COPIES * 4 * a.max_faces;
+  double* sAb0 = sm;           sm += W * 4 * a.max_faces;
   double* TZ = sm;             sm += D::NY * D::TZLD;
   double* SY = sm;             sm += D::NY;
   unsigned char* wraw = reinterpret_cast<unsigned char*>(sm);
@@ -1113,13 +854,10 @@ __global__ void __launch_bounds__(W * 32, (N_ <= 10 ? (WHOLE_ ? FQ_MIN_CTAS_WHOL
     m.d = p;   p += D::NW + 2;
     m.zb = p;  p += D::NW;
     m.items = reinterpret_cast<unsigned short*>(p);
-    m.half_ofs = 2 * a.max_faces;
-    seg_ofs = sfo0 + 40 * SAB_COPIES + warp * 32;
+    seg_ofs = sfo0 + 40 * W + warp * 32;
   }
   __syncthreads();
   const int n_prob = a.n_prob;
-#if FQ_WARP_ADOPT
-  (void)s_prob;
   double* sAb = sAb0 + (size_t)warp * 4 * a.max_faces;
   int* sfo = sfo0 + 40 * warp;
   const long long me = (long long)blockIdx.x * W + warp, adopters = (long long)gridDim.x * W;
@@ -1158,12 +896,14 @@ __global__ void __launch_bounds__(W * 32, (N_ <= 10 ? (WHOLE_ ? FQ_MIN_CTAS_WHOL
         double2 v = src[i];
         bad |= !(fabs(v.x) < 1e300) || !(fabs(v.y) < 1e300);
         if (i & 1) v.y += a.row_tol;               // rows are staged as [Ax Ay Az b+tol]
-        row_store(sAb, i, m.half_ofs, v);
+        row_store(sAb, i, v);
       }
       for (int i = lane; i <= P && i < 36; i += 32) sfo[i] = a.face_ofs[p0 + i] - f0;
       rows_bad = __any_sync(FULL, bad) != 0 ? 1 : 0;
       __syncwarp();                                // publishes the staged rows to the warp
     }
+    // claim candidates one ahead: the global atomic for the NEXT candidate is issued before the current one is solved,
+    // so its round trip hides behind the solve instead of idling the warp between candidates
     int c = 0;
     if (lane == 0) c = atomicAdd(counters + prob, 1);
     c = __shfl_sync(FULL, c, 0);
@@ -1222,76 +962,10 @@ __global__ void __launch_bounds__(W * 32, (N_ <= 10 ? (WHOLE_ ? FQ_MIN_CTAS_WHOL
     }
     __syncwarp();
   }
-#else
-  double* sAb = sAb0;
-  int* sfo = sfo0;
-  int cursor = (int)(((long long)blockIdx.x * n_prob) / gridDim.x);   // CTA-specific starting problem
-  int visited = 0;
-  for (;;)
-  {
-    // ---- adopt the next problem (cyclically from `cursor`) that still has unclaimed candidates
-    if (warp == 0)
-    {
-      int found = -1;
-      while (visited < n_prob && found < 0)
-      {
-        const int j = visited + lane;
-        int pj = cursor + j;
-        if (pj >= n_prob) pj -= n_prob;
-        bool open = false;
-        if (j < n_prob)
-          open = *reinterpret_cast<volatile int*>(counters + pj) < a.cand_ofs[pj + 1] - a.cand_ofs[pj];
-        const unsigned bal = __ballot_sync(FULL, open);
-        if (bal) { const int first = __ffs(bal) - 1; found = cursor + visited + first; visited += first + 1; }
-        else visited += 32;
-      }
-      if (lane == 0) s_prob = found < 0 ? -1 : (found >= n_prob ? found - n_prob : found);
-    }
-    __syncthreads();
-    const int prob = s_prob;
-    if (prob < 0) break;
-    const int c_begin = a.cand_ofs[prob], count = a.cand_ofs[prob + 1] - c_begin;
-    const int p0 = a.poly_ofs[prob], P = a.poly_ofs[prob + 1] - p0;
-    const int f0 = a.face_ofs[p0];
-    const int nf = P > 0 ? a.face_ofs[p0 + P] - f0 : 0;
-    int rows_bad = 0;
-    {
-      const bool fits = nf >= 0 && nf <= a.max_faces;      // see the warp-adopting variant above
-      const double2* src = reinterpret_cast<const double2*>(a.Ab + (size_t)4 * f0);
-      int bad = 0;
-      for (int i = threadIdx.x; fits && i < 2 * nf; i += blockDim.x)
-      {
-        double2 v = src[i];
-        bad |= !(fabs(v.x) < 1e300) || !(fabs(v.y) < 1e300);
-        if (i & 1) v.y += a.row_tol;               // rows are staged as [Ax Ay Az b+tol]
-        row_store(sAb, i, m.half_ofs, v);
-      }
-      for (int i = threadIdx.x; i <= P && i < 36; i += blockDim.x) sfo[i] = a.face_ofs[p0 + i] - f0;
-      rows_bad = __syncthreads_or(bad) != 0 ? 1 : 0;       // also the barrier that publishes the staged rows
-      if (!fits) rows_bad = 2;
-    }
-    // claim candidates one ahead: the global atomic for the NEXT candidate is issued before the current one is solved,
-    // so its round trip (~1 us) hides behind the solve instead of idling the warp between candidates
-    int c = 0;
-    if (lane == 0) c = atomicAdd(counters + prob, 1);
-    c = __shfl_sync(FULL, c, 0);
-    while (c < count)
-    {
-      int cn = 0;
-      if (lane == 0) cn = atomicAdd(counters + prob, 1);
-      // claims run from the LAST candidate of the problem down: in a time-allocation sweep (dt-major candidate lists,
-      // increasing dt) the rare very long solves -- dozens of active-set changes against a mean of ~5 -- sit at the large
-      // dt end, and a long solve started last is a long tail for the whole launch
-      solve_candidate<D>(a, TZ, SY, sAb, sfo, m, seg_ofs, prob, c_begin + (count - 1 - c), lane, rows_bad);
-      c = __shfl_sync(FULL, cn, 0);
-    }
-    __syncthreads();                               // everyone is done with the staged rows
-  }
-#endif
 }
 
 template <int N_, bool WHOLE_>
-size_t smem_bytes_t(int max_faces, int item_cap, int sab_copies = (FQ_WARP_ADOPT ? W : 1))
+size_t smem_bytes_t(int max_faces, int item_cap, int sab_copies = W)
 {
   using D = Dims<N_, WHOLE_>;
   return (size_t)8 * ((size_t)sab_copies * 4 * max_faces + D::NY * D::TZLD + D::NY) + (size_t)W * per_warp_bytes<D>(item_cap) +
@@ -1333,7 +1007,7 @@ cudaError_t launch_t(const FqKernelArgs& a, long long total_cand_hint, cudaStrea
   long long grid = resident;
   const long long need = (total_cand_hint + W - 1) / W;      // no point in more CTAs than candidates / warps
   if (grid > need) grid = need;
-  if (a.first_feasible && a.sorted_dt && a.ee_width > 0 && (FQ_EE_CAP_ALWAYS || need > resident))
+  if (a.first_feasible && a.sorted_dt && a.ee_width > 0 && need > resident)
   { // early exit on an ascending sweep that does not fit the GPU at once: keep only ~two time allocations per problem in
     // flight, so that the larger ones -- which cannot win once a smaller one is feasible -- are mostly never started.
     // A sweep that fits (one genNewTraj: a few hundred candidates) starts everything: a cap would only serialise it

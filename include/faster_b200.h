@@ -40,8 +40,7 @@ extern "C" {
 typedef struct fq_ctx fq_ctx;     /* opaque: device, stream, plan tables, scratch             */
 
 int fq_abi_version(void);
-/* 1 if this build has the named feature: "cert_memo" (compile-time switch FQ_CERT_MEMO, off by default: see
- * faster_b200/csrc/fq_kernels.cuh), "sweep_early_exit", "replan_pairs", "multi_gpu", "row_tol", "certificates". */
+/* 1 if this build has the named feature: "sweep_early_exit", "replan_pairs", "multi_gpu", "row_tol", "certificates". */
 int fq_has_feature(const char* name);
 
 /* Threading: a context is used from one thread at a time, like a SolverGurobi instance in the reference (one replan
@@ -61,9 +60,8 @@ const char* fq_last_error(const fq_ctx* ctx);   /* ctx may be NULL: last creatio
  * tolerance of every later solve of the context in units of 1e-9 -- 10 is the default FQ_ROW_TOL = 1e-8, 1000 is Gurobi's
  * default FeasibilityTol 1e-6 (the reference sets no tolerance parameter, solverGurobi.cpp:479-487).  0 is refused
  * (FQ_E_ARG): at zero tolerance rounding alone keeps a row that was just made active violated, and the active set cycles
- * until the iteration cap gives up on solvable candidates.  1 (1e-9) is also the lowest FeasibilityTol Gurobi accepts.  "cert_memo" (0/1; only in builds with
- * fq_has_feature("cert_memo")): candidates of one problem share their infeasibility proofs (a candidate whose dt and polytopes on the proof's segments
- * match a recorded Farkas certificate is answered without a solve; same flags, iters = 0 marks them).
+ * until the iteration cap gives up on solvable candidates.  1 (1e-9) is also the lowest FeasibilityTol Gurobi accepts.  "cert_memo" (any
+ * value) is accepted and ignored: the GPU kernels have no infeasibility-certificate memo.
  * "sweep_early_exit" (0/1, default 0): genNewTraj keeps the FIRST feasible factor (solverGurobi.cpp:445-446), so once a
  * problem has a feasible candidate, candidates with a larger dt cannot win; with this option they are not evaluated
  * (reported feasible = 0, cost = +inf, iters = -3) and claims run in ascending dt.  The winners (fq_replan_pairs results,

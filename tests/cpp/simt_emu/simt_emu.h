@@ -18,9 +18,8 @@
 #define __device__
 #define __host__
 #ifndef __shared__
-#define __shared__            /* the dynamic shared array is one static buffer of the harness; the kernel's one static
-                                 __shared__ variable belongs to a build mode (FQ_WARP_ADOPT = 0) the harness does not compile.
-                                 A translation unit whose kernels use static __shared__ variables defines it as `static`. */
+#define __shared__            /* the dynamic shared array is one static buffer of the harness.  A translation unit whose
+                                 kernels use static __shared__ variables defines it as `static`. */
 #endif
 #define __forceinline__ inline
 #define __launch_bounds__(...)

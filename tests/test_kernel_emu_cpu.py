@@ -1,11 +1,10 @@
 """The product's CUDA kernel SOURCE, executed without a GPU: faster_b200/csrc/fq_kernels_t.cuh (fq_solve_kernel_t: persistent CTAs,
 claim counters, row staging, item lists, the warp-per-candidate dual active-set iteration) is compiled for the host and run under
 a lock-step emulation of one thread block (tests/cpp/simt_emu/: every CUDA thread is a fibre, warp collectives and block barriers
-are rendezvous points) and compared with the CPU restatement.  This checks the kernel's LOGIC in a container that has no GPU --
-including compile-time variants of it -- and is what the `-m gpu` parity tests then confirm on the hardware.  It is test
+are rendezvous points) and compared with the CPU restatement.  This checks the kernel's LOGIC in a container that has no GPU
+and is what the `-m gpu` parity tests then confirm on the hardware.  It is test
 infrastructure, not a CPU path of the product (the library still refuses to work without a GPU) and ~10^4 times too slow to be one."""
 import ctypes as C
-import hashlib
 import json
 import os
 import subprocess
@@ -16,28 +15,28 @@ import pytest
 from faster_b200 import capi, corridor as cr
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-_libs = {}
+_LIB = None
 
 
-def _emu(defines=()):
-    """The harness built with the given -D flags (cached per flag set under tests/cpp/_build, rebuilt when a source is newer)."""
-    key = hashlib.sha1(" ".join(defines).encode()).hexdigest()[:10]
-    if key in _libs:
-        return _libs[key]
-    out = os.path.join(ROOT, "tests", "cpp", "_build", "libkernel_emu_%s.so" % key)
+def _emu():
+    """The harness (built under tests/cpp/_build, rebuilt when a source is newer)."""
+    global _LIB
+    if _LIB is not None:
+        return _LIB
+    out = os.path.join(ROOT, "tests", "cpp", "_build", "libkernel_emu.so")
     srcs = [os.path.join(ROOT, "tests", "cpp", "kernel_emu.cpp"), os.path.join(ROOT, "tests", "cpp", "simt_emu", "simt_emu.h"),
             os.path.join(ROOT, "faster_b200", "csrc", "fq_kernels_t.cuh"), os.path.join(ROOT, "faster_b200", "csrc", "fq_kernels.cuh")]
     if not os.path.exists(out) or os.path.getmtime(out) < max(os.path.getmtime(s) for s in srcs):
         os.makedirs(os.path.dirname(out), exist_ok=True)
-        subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w"] + ["-D" + d for d in defines] +
-                              ["-I", os.path.join(ROOT, "tests", "cpp"), "-I", os.path.join(ROOT, "tests", "cpp", "simt_emu"),
+        subprocess.check_call(["g++", "-std=c++17", "-O1", "-fPIC", "-shared", "-w",
+                               "-I", os.path.join(ROOT, "tests", "cpp"), "-I", os.path.join(ROOT, "tests", "cpp", "simt_emu"),
                                "-I", os.path.join(ROOT, "faster_b200", "csrc"), "-I", os.path.join(ROOT, "include"), srcs[0], "-o", out])
     L = C.CDLL(out)
     L.emu_solve_multi.argtypes = [C.c_int, C.c_int] + [C.c_void_p] * 3 + [C.c_int] + [C.c_void_p] * 6 + [C.c_int, C.c_int] + \
                                  [C.c_void_p] * 3 + [C.c_double] + [C.c_void_p] * 4
     L.emu_set_sweep.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p]
     L.emu_set_sweep.restype = None
-    _libs[key] = L
+    _LIB = L
     return L
 
 
@@ -159,25 +158,6 @@ def test_emulated_kernel_honours_the_row_tolerance(oracle, ff, kind):
         oracle.set_row_tol(1e-8)
         oracle.port_lib().fqc_set_row_tol(1e-8)
     assert n_feas[1e-9] == 0 and n_feas[1e-3] > 0, n_feas
-
-
-def test_compile_time_variants_compute_the_same_thing(oracle):
-    """The ratio test's minimum through redux.sync on the order-preserving image of the doubles (on) against the shuffle tree
-    (FQ_MIN_REDUX=0), and the four variants left off by default (FQ_LAZY_LEAVING,
-    FQ_SCAN_ARGMAX, FQ_GI_HOIST, FQ_ITEMS_BY_SEGMENT): every one of them returns the same flags, the same iteration counts and
-    the same costs and coefficients BIT FOR BIT as the default build -- they reorganise the work, not the arithmetic."""
-    rng = np.random.default_rng(12)
-    base = {}
-    for N, P, ff in ((10, 3, True), (10, 4, False), (15, 8, True)):
-        b = _batch(oracle, N, P, ff, "uav" if N < 15 else "ground", [9300 + N + k for k in range(2)], 8, [1.0, 2.0, 3.0, 6.0], rng)
-        base[(N, ff)] = (b, solve_multi(_emu(), N, ff, *b))
-    for flags in (["FQ_MIN_REDUX=0"], ["FQ_LAZY_LEAVING=1"], ["FQ_SCAN_ARGMAX=1"], ["FQ_GI_HOIST=1"], ["FQ_ITEMS_BY_SEGMENT=1"],
-                  ["FQ_LAZY_LEAVING=1", "FQ_SCAN_ARGMAX=1", "FQ_GI_HOIST=1", "FQ_ITEMS_BY_SEGMENT=1", "FQ_MIN_REDUX=0"]):
-        L = _emu(flags)
-        for (N, ff), (b, ref) in base.items():
-            got = solve_multi(L, N, ff, *b)
-            assert np.array_equal(got[0], ref[0]) and np.array_equal(got[3], ref[3]), (flags, N, ff)
-            assert got[1].tobytes() == ref[1].tobytes() and got[2].tobytes() == ref[2].tobytes(), (flags, N, ff)
 
 
 def test_guards_of_the_kernel(oracle, demo_corridor):

@@ -783,45 +783,6 @@ def test_wrong_polytope_size_hint_is_refused_not_overrun(solver):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("N,P,ff", [(10, 3, True), (10, 4, False), (15, 8, True)])
-def test_certificate_memo_changes_nothing_but_the_work(solver, oracle, N, P, ff):
-    """Candidates of one problem share their infeasibility proofs (option "cert_memo"): with the memo on, the flags and
-    costs are those of the memo-less run (and of the oracle), and a good part of the infeasible candidates is answered
-    without a solve (iters == 0)."""
-    if not capi.has_feature("cert_memo"):
-        pytest.skip("library built without FQ_CERT_MEMO (the default: measured slower on the GPU, see fq_kernels.cuh)")
-    rng = np.random.default_rng(N * 100 + P)
-    n_prob = 5
-    sig = cr.monotone_sigmas(N, P) if P <= 4 else cr.sample_monotone_sigmas(N, P, 200, rng)
-    sig = sig[:200]
-    x0 = np.zeros((n_prob, 9)); xf = np.zeros((n_prob, 9)); lim = np.zeros((n_prob, 3))
-    po_, fo_, rows, co, dts, sgs = [0], [0], [], [0], [], []
-    probs = []
-    for j in range(n_prob):
-        pb = cr.make_corridor(8800 + j, P, N, "ground" if N == 15 else "uav", ff)
-        probs.append(pb)
-        x0[j], xf[j], lim[j] = pb["x0"], pb["xf"], pb["lim"]
-        for A, b in pb["polys"]:
-            rows.append(np.hstack([A, b[:, None]])); fo_.append(fo_[-1] + len(b))
-        po_.append(po_[-1] + P)
-        base = max(capi.dt_initial(pb["x0"], pb["xf"], pb["lim"], N), 0.02)
-        dts.append(np.repeat(np.arange(1.0, 11.0) * base, len(sig))); sgs.append(np.tile(sig, (10, 1)))
-        co.append(co[-1] + 10 * len(sig))
-    args = (N, ff, x0, xf, lim, np.array(po_, np.int32), np.array(fo_, np.int32), np.ascontiguousarray(np.vstack(rows)),
-            np.array(co, np.int32), np.concatenate(dts), np.ascontiguousarray(np.vstack(sgs)))
-    solver.set_option("cert_memo", 0)
-    f0, c0, _, it0 = solver.solve_multi(*args, want_iters=True)
-    solver.set_option("cert_memo", 1)
-    f1, c1, _, it1 = solver.solve_multi(*args, want_iters=True)
-    assert np.array_equal(f0, f1) and np.array_equal(c0, c1)
-    assert (it0[f0 == 0] != 0).all()                       # without the memo every infeasible flag comes from a solve
-    hits = (it1 == 0) & (f1 == 0)                          # infeasible without a single iteration: answered from the memo
-    assert hits.sum() > 0, (hits.sum(), (f0 == 0).sum())
-    fo, _ = oracle.solve_multi(*args, 8)
-    assert np.array_equal(fo, f1)
-
-
-@pytest.mark.gpu
 def test_full_active_set_is_handled(solver, oracle):
     """N = 15, free final position: 39 unknowns, and many infeasible candidates are only refuted once the active set holds
     39 rows.  With a full active set every further row is dependent by definition; the solver must say so whatever

@@ -272,3 +272,10 @@ def test_the_option_takes_1e9_to_1e3_only(solver):
             solver.set_option("row_tol_1e9", good)
     finally:
         solver.set_option("row_tol_1e9", 10)
+
+
+def test_cert_memo_is_accepted_and_ignored(solver):
+    """The GPU kernels have no certificate memo; the option stays accepted for callers that switch it (bench.py --no-memo)."""
+    for v in (0, 1):
+        solver.set_option("cert_memo", v)
+    assert not capi.has_feature("cert_memo")

@@ -1,6 +1,6 @@
 #!/bin/bash
 # A/B of library variants on ONE box (run under gpurun): tools/ab.sh lib1.so lib2.so ...  (names under faster_b200/lib;
-# a name may carry bench flags after a colon, e.g. libfaster_b200.so:--no-memo).  Each variant: bench.py --quick (cfg4
+# a name may carry bench flags after a colon, e.g. libfaster_b200.so:--single-stream).  Each variant: bench.py --quick (cfg4
 # chain, resident + e2e); AB_ROUNDS rounds (default 2) to see the noise.
 for round in $(seq 1 ${AB_ROUNDS:-2}); do
   for spec in "$@"; do

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Large parity sweep of the chained replan (run on the GPU box): every corridor of the committed cfg4 fixture through
-fq_replan_pairs (certificate memo on and off) against the CPU chains -- the tuned port (oracle/fq_cpu_port.c, all 512
+fq_replan_pairs against the CPU chains -- the tuned port (oracle/fq_cpu_port.c, all 512
 corridors) and the literal restatement (oracle/fq_oracle.c via pair_oracle, a slice).  Prints one JSON line."""
 import json
 import os
@@ -17,21 +17,16 @@ from oracle import pair_oracle, pyoracle as po  # noqa: E402
 n_batches = int(sys.argv[1]) if len(sys.argv) > 1 else 8
 s = capi.Solver(0)
 res = {"corridors": 0, "pairs": 0, "flag_mismatches_vs_port": 0, "winner_mismatches_vs_port": 0, "max_rel_cost_err": 0.0,
-       "memo_on_vs_off_flag_diffs": 0, "memo_on_vs_off_record_diffs": 0, "literal_slice": {}}
+       "literal_slice": {}}
 t0 = time.time()
 threads = os.cpu_count() or 1
 for b in range(n_batches):
     w = bench.load_cfg4(64 * b, 64)
-    s.set_option("cert_memo", 1)
     g = s.replan_pairs(w)
-    s.set_option("cert_memo", 0)
-    g0 = s.replan_pairs(w)
     r = g["results"]
-    res["memo_on_vs_off_record_diffs"] += int(r.tobytes() != g0["results"].tobytes())
     p = po.replan_pairs_port(w, threads)
     pr = p["results"]
     for k in ("whole", "safe"):
-        res["memo_on_vs_off_flag_diffs"] += int((g["feasible_" + k] != g0["feasible_" + k]).sum() + (g["cost_" + k] != g0["cost_" + k]).sum())
         res["flag_mismatches_vs_port"] += int((g["feasible_" + k] != p["feasible_" + k]).sum())
         ok = g["feasible_" + k].astype(bool) & p["feasible_" + k].astype(bool)
         if ok.any():
