@@ -47,14 +47,18 @@ def prove_optimal(Q, Aeq, beq, Ain, bin_, z, active_tol=1e-7):
         "resid": float(np.abs(rho).max() / max(1.0, np.abs(g).max())),
         "gap": float((lam @ np.abs(slack[act]) if len(act) else 0.0) + abs(mu @ req)) / max(1.0, f),
         "lam_min": float(lam.min()) if len(lam) else 0.0,
+        "lam_sum": float(lam.sum()),
+        "active": act,
         "cost": f,
     }
 
 
-def assert_optimal(model, z, cost=None, feas_tol=1e-7, resid_tol=1e-6, gap_tol=1e-7):
-    """model = model_fullspace.build(...) ; z = coefficients [N,12] reported with a "solved" flag ; cost = reported cost."""
+def assert_optimal(model, z, cost=None, feas_tol=1e-7, resid_tol=1e-6, gap_tol=1e-7, active_tol=1e-7):
+    """model = model_fullspace.build(...) ; z = coefficients [N,12] reported with a "solved" flag ; cost = reported cost.
+    active_tol: rows with less relative slack may carry multipliers (any choice gives a valid bound; a smaller one keeps
+    the fit off the slack twin of a nearly parallel tight row)."""
     Q, Aeq, beq, Ain, bin_ = model
-    r = prove_optimal(Q, Aeq, beq, Ain, bin_, z)
+    r = prove_optimal(Q, Aeq, beq, Ain, bin_, z, active_tol)
     assert r["eq"] <= feas_tol and r["ineq"] <= feas_tol, ("not feasible on the literal rows", r)
     assert r["lam_min"] >= 0.0
     assert r["resid"] <= resid_tol, ("no KKT multipliers: the point is not the optimum", r)

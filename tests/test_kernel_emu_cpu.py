@@ -160,6 +160,56 @@ def test_emulated_kernel_honours_the_row_tolerance(oracle, ff, kind):
     assert n_feas[1e-9] == 0 and n_feas[1e-3] > 0, n_feas
 
 
+def _prove_both(N, ff, b, i, answers, row_tol=1e-8):
+    """Candidate i of a _batch: every answer (cost, coeffs) proved optimal on the literal model; their cost gap must stay
+    below 2 row_tol times the larger multiplier sum (a point that violates rows by up to row_tol is at most that much cheaper)."""
+    from oracle import model_fullspace as mf, proofs
+    x0, xf, lim, po_, fo, Ab, co_, dts, sigs = b
+    j = int(np.searchsorted(co_, i, side="right")) - 1
+    polys = [(Ab[fo[p]:fo[p + 1], :3], Ab[fo[p]:fo[p + 1], 3]) for p in range(po_[j], po_[j + 1])]
+    model = mf.build(N, x0[j], xf[j], lim[j], dts[i], polys, sigs[i], ff)
+    lam = [proofs.assert_optimal(model, z, c, feas_tol=row_tol + 1e-7, active_tol=1e-9)["lam_sum"] for c, z in answers]
+    assert abs(answers[0][0] - answers[1][0]) <= 2 * row_tol * max(lam) + 1e-12 * answers[1][0], (i, answers[0][0], answers[1][0])
+
+
+@pytest.mark.parametrize("fam", ["fan", "dup", "slab", "near_parallel_1e-7", "near_parallel_1e-9", "near_parallel_1e-12", "x0_vertex"])
+@pytest.mark.parametrize("N,ff,P", [(6, True, 3), (10, True, 3), (10, False, 3), (13, False, 4)])
+def test_emulated_kernel_on_degenerate_corridors(oracle, fam, N, ff, P):
+    """tests/degenerate_cases.py's families through the emulated kernel against the tuned CPU port: faces fanned through
+    vertices and edges near the path, every face duplicated, the zero-width slab on the ground profile, copies rotated by
+    1e-7, 1e-9 (the dependency cut-off) and 1e-12 rad about a line inside the polytope, x0 on a vertex.  Identical flags and
+    no give-ups; fan and dup must also give the original corridor's answer.
+    Near a near-parallel pair's crossing line both rows hold within the row tolerance on a wedge row_tol / theta wide (0.1 m
+    at 1e-7, 10 m at 1e-9), so which row of the pair ends up active, and where, depends on the order the rows are picked in:
+    the kernel and the port differ there by up to 2e-8 in cost.  A candidate beyond the 1e-9 cost or 1e-7 coefficient bar must
+    then have both answers proved optimal, with a cost gap below the tolerance times the multipliers."""
+    import degenerate_cases as dc
+    change = {"fan": lambda pb: dc.fan(pb, 2), "dup": dc.dup, "slab": dc.slab, "x0_vertex": lambda pb: dc.on_boundary(pb, "x0", 3),
+              "near_parallel_1e-7": lambda pb: dc.near_parallel(pb, 1e-7), "near_parallel_1e-9": lambda pb: dc.near_parallel(pb, 1e-9),
+              "near_parallel_1e-12": lambda pb: dc.near_parallel(pb, 1e-12)}[fam]
+    profile = "ground" if fam == "slab" else "uav"
+    seeds, facs = [9300 + N + k for k in range(2)], [0.3, 0.6, 1.0, 2.0, 5.0]
+    b = _batch(oracle, N, P, ff, profile, seeds, 8, facs, np.random.default_rng(N), change)
+    got = solve_multi(_emu(), N, ff, *b)
+    assert (got[3] >= 0).all()
+    if not fam.startswith("near_parallel"):
+        _check(oracle, N, ff, b, got)
+    else:
+        f, c, cc = oracle.solve_multi_port(N, ff, *b, threads=4, want_coeffs=True)
+        assert np.array_equal(got[0], f) and f.any() and not f.all()
+        ok = np.flatnonzero(f)
+        rel = np.abs(got[1][ok] - c[ok]) / np.abs(c[ok])
+        err = np.abs(got[2][ok] - cc[ok]).max(axis=(1, 2))
+        for i in ok[(rel > 1e-9) | (err > 1e-7)]:
+            _prove_both(N, ff, b, i, [(got[1][i], got[2][i]), (c[i], cc[i])])
+    if fam in ("fan", "dup"):
+        b0 = _batch(oracle, N, P, ff, profile, seeds, 8, facs, np.random.default_rng(N))
+        got0 = solve_multi(_emu(), N, ff, *b0)
+        ok = got0[0].astype(bool)
+        assert np.array_equal(got[0], got0[0]) and (np.abs(got[1][ok] - got0[1][ok]) / got0[1][ok]).max() <= 1e-9
+        assert np.abs(got[2][ok] - got0[2][ok]).max() <= 1e-7
+
+
 def test_guards_of_the_kernel(oracle, demo_corridor):
     """What the kernel must refuse by itself because the device-pointer entry cannot validate it on the host: non-finite or
     non-positive inputs (candidate reported not solved, iters = -1), a row list that does not fit the caller's size hint
