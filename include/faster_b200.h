@@ -29,6 +29,12 @@ extern "C" {
 #define FQ_ABI_VERSION 2
 #define FQ_MAX_N 16               /* segments per trajectory                                  */
 #define FQ_MAX_POLY 32            /* polytopes per corridor problem                           */
+/* Faces per problem are bounded by shared memory, and the bound depends on N and mode: a problem's rows and per-warp
+ * solver state live in one block's shared memory (227 KB on an H100).  The size-specialised kernel takes up to 2047 faces
+ * and less as N grows (N = 10 whole: 951 faces in one polytope, 1279 in three equal ones; N = 16 safe: 463 / 695).  A
+ * larger problem runs on the size-generic kernel instead, with the same results to rounding (N = 10 whole: up to 5600
+ * faces; N = 16 safe: 2244).  Beyond that every solve entry point refuses the problem with FQ_E_ARG ("problem too large for
+ * shared memory").  DESIGN.md section 3.4 has the table. */
 #define FQ_ROW_TOL 1e-8           /* DEFAULT absolute row violation tolerance (m, m/s, m/s^2, m/s^3); run-time
                                      option "row_tol_1e9" of fq_set_option                                   */
 
@@ -154,8 +160,10 @@ int fq_gen_new_traj_sampled(fq_ctx* ctx, int N, int force_final, const double* x
  * allocation, which is what Gurobi's branch-and-bound over the binaries b[t][p] returns (solverGurobi.cpp:217-246,
  * :445-472).  Branch-and-bound on the GPU over the segments (dual warm starts from the parent node, bound pruning with the
  * best non-decreasing assignment as incumbent).  Outputs: winning dt index (-1 none), its assignment sigma_out[N], cost,
- * coefficients; *nodes_out = nodes evaluated; *exact_out = 0 if the tree had to be cut (node pool overflow, N < 4 or
- * more than 2047 faces) and the result is the best non-decreasing assignment instead.  Returns 1 / 0 / <0. */
+ * coefficients; *nodes_out = nodes evaluated; *exact_out = 0 if the tree had to be cut (more than 65536 open nodes on one
+ * level, a node's solve gave up, N < 4, more than 2047 faces, or the tree's shared-memory footprint is too large) and the
+ * result is the best non-decreasing assignment instead.  FQ_E_ARG if that assignment list is too long for the pre-sweep:
+ * C(N+P-1, N) > 2^20 or C(N+P-1, N) x n_dt > 2^24.  Returns 1 / 0 / <0. */
 int fq_gen_new_traj_exact(fq_ctx* ctx, int N, int force_final, const double* x0, const double* xf, const double* lim,
                           int P, const int* face_ofs, const double* Ab, int n_dt, const double* dts, int* dt_index,
                           uint8_t* sigma_out, double* cost, double* coeffs, long* nodes_out, int* exact_out);

@@ -92,10 +92,14 @@ public:
   //   ALL       every one of the P^N (the exact MIQP optimum, like Gurobi's branch-and-bound);
   //   MONOTONE  the non-decreasing ones only, C(N+P-1, P-1) (identical genNewTraj results in 960/960 measured sweeps,
   //             see DESIGN.md section 2);
-  //   EXACT     branch-and-bound over all P^N on the GPU (fq_gen_new_traj_exact): the exact MIQP optimum for any size,
-  //             ~125 us per sweep instead of ~80;
+  //   EXACT     branch-and-bound over all P^N on the GPU (fq_gen_new_traj_exact), ~125 us per sweep instead of ~80: the
+  //             exact MIQP optimum, reported with exact = 1.  It falls back to the best non-decreasing assignment, reported
+  //             with exact = 0, when the corridor has more than 2047 faces, when the tree's shared-memory footprint
+  //             exceeds the GPU's (N = 16 safe: ~750 faces in one polytope), when a level of the tree has more than 65536
+  //             open nodes, or when a node's solve gives up.  It refuses (FQ_E_ARG) when its non-decreasing pre-sweep is too
+  //             long: C(N+P-1, N) > 2^20 (e.g. N = 10 with P >= 16) or C(N+P-1, N) x (time allocations) > 2^24;
   //   AUTO      (default) ALL while P^N <= auto_all_limit (4096: covers the shipped yaml, N=6 and <=3 polytopes: 729),
-  //             EXACT beyond -- i.e. always the reference's MIQP optimum.
+  //             EXACT beyond -- i.e. the reference's MIQP optimum within EXACT's limits.
   void setAssignmentMode(AssignmentMode m, long max_assignments = 16384, long auto_all_limit = 4096)
   {
     amode_ = m; max_sigma_ = max_assignments < 1 ? 1 : max_assignments; auto_all_limit_ = auto_all_limit;

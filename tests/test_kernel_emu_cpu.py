@@ -210,6 +210,35 @@ def test_emulated_kernel_on_degenerate_corridors(oracle, fam, N, ff, P):
         assert np.abs(got[2][ok] - got0[2][ok]).max() <= 1e-7
 
 
+def test_emulated_kernel_at_its_shared_memory_limit(oracle):
+    """N = 10 whole with one polytope of ~950 faces: the largest problem the specialised kernel takes within an H100's 227 KB
+    of shared memory (tests/capacity_cases.py), its rows tangent to a capsule around the path so that they bind, the original
+    faces last (staged rows up to ~950, item lists of ~9500 entries).  Against the restatement."""
+    import capacity_cases as cc
+    N, ff, P = 10, True, 3
+    pb = cr.make_corridor(86000, P, N, "uav", ff)
+    base = [len(b) for _, b in pb["polys"]]
+    n = cc.limit("spec", N, ff, "dominant", base)
+    assert not cc.fits("spec", N, ff, cc.split_counts(n + 1, "dominant", base))
+    pb = cc.with_faces(pb, n, "dominant", seed=1)
+    counts = [len(b) for _, b in pb["polys"]]
+    assert sum(counts) == n and max(counts) >= 900
+    rng = np.random.default_rng(3)
+    sig = np.vstack([cr.monotone_sigmas(N, P)[[0, 10, 30, 45, 65]], rng.integers(0, P, (1, N)).astype(np.uint8)])
+    facs = [1.0, 2.0, 4.0]
+    base_dt = max(oracle.dt_initial(pb["x0"], pb["xf"], pb["lim"], N), 0.02)
+    dts, sigs = np.repeat(np.array(facs) * base_dt, len(sig)), np.tile(sig, (len(facs), 1))
+    Ab = np.vstack([np.hstack([A, np.asarray(b)[:, None]]) for A, b in pb["polys"]])
+    fo = np.concatenate([[0], np.cumsum(counts)])
+    b = ([pb["x0"]], [pb["xf"]], [pb["lim"]], [0, P], fo, Ab, [0, len(dts)], dts, sigs)
+    got = solve_multi(_emu(), N, ff, *b)
+    assert (got[3] >= 0).all()
+    f, c, cc_ = oracle.solve_batch(N, pb["x0"], pb["xf"], pb["lim"], pb["polys"], dts, sigs, ff, True, threads=4)
+    assert np.array_equal(got[0], f) and f.any() and not f.all()
+    ok = f.astype(bool)
+    assert (np.abs(got[1][ok] - c[ok]) / c[ok]).max() <= 1e-9 and np.abs(got[2][ok] - cc_[ok]).max() <= 1e-7
+
+
 def test_guards_of_the_kernel(oracle, demo_corridor):
     """What the kernel must refuse by itself because the device-pointer entry cannot validate it on the host: non-finite or
     non-positive inputs (candidate reported not solved, iters = -1), a row list that does not fit the caller's size hint
