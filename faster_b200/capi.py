@@ -14,7 +14,8 @@ EXPORTS = ["fq_abi_version", "fq_create", "fq_destroy", "fq_last_error", "fq_set
            "fq_solve_multi_async", "fq_wait", "fq_solve_multi_dev", "fq_gen_new_traj", "fq_gen_new_traj_sampled", "fq_gen_new_traj_exact", "fq_dt_initial", "fq_num_samples", "fq_fill_x",
            "fq_monotone_sigmas", "fq_plan_tables", "fq_ellipsoid_decomp", "fq_jps3d_plan", "fq_jps3d_plan_world", "fq_jps3d_rules",
            "fq_replan_pairs", "fq_replan_pairs_async", "fq_replan_pairs_dev", "fq_create_multi", "fq_comm_unique_id", "fq_comm_init",
-           "fq_comm_info", "fq_allgather_dev", "fq_shard_range", "fq_solve_multi_sharded", "fq_solve_batch_cert", "fq_has_feature"]
+           "fq_comm_info", "fq_allgather_dev", "fq_shard_range", "fq_solve_multi_sharded", "fq_solve_batch_cert", "fq_has_feature",
+           "fq_pair_assign_count", "fq_replan_pairs_assign", "fq_replan_pairs_assign_async", "fq_replan_pairs_assign_dev"]
 
 
 class FqError(RuntimeError):
@@ -49,6 +50,13 @@ class PairArgs(C.Structure):
                 ("coeffs_whole", C.c_void_p), ("coeffs_safe", C.c_void_p), ("results", C.c_void_p),
                 ("max_faces_whole", C.c_int), ("max_poly_faces_whole", C.c_int), ("max_faces_safe", C.c_int),
                 ("max_poly_faces_safe", C.c_int)]
+
+
+class PairAssign(C.Structure):
+    """fq_pair_assign of include/faster_b200.h: per-corridor assignment lists of the chained replan."""
+    _fields_ = [("all_limit", C.c_long), ("max_poly_whole", C.c_int), ("max_poly_safe", C.c_int), ("n_cand_whole", C.c_long),
+                ("n_cand_safe", C.c_long), ("cand_ofs_whole", C.c_void_p), ("cand_ofs_safe", C.c_void_p),
+                ("sigma_whole", C.c_void_p), ("sigma_safe", C.c_void_p)]
 
 
 def lib():
@@ -90,6 +98,11 @@ def lib():
         L.fq_replan_pairs.argtypes = [C.c_void_p, C.POINTER(PairArgs)]
         L.fq_replan_pairs_async.argtypes = [C.c_void_p, C.POINTER(PairArgs)]
         L.fq_replan_pairs_dev.argtypes = [C.c_void_p, C.POINTER(PairArgs), C.c_void_p, C.c_void_p]
+        L.fq_pair_assign_count.restype = C.c_long
+        L.fq_pair_assign_count.argtypes = [C.c_int, C.c_int, C.c_long]
+        L.fq_replan_pairs_assign.argtypes = [C.c_void_p, C.POINTER(PairArgs), C.POINTER(PairAssign)]
+        L.fq_replan_pairs_assign_async.argtypes = L.fq_replan_pairs_assign.argtypes
+        L.fq_replan_pairs_assign_dev.argtypes = [C.c_void_p, C.POINTER(PairArgs), C.POINTER(PairAssign), C.c_void_p, C.c_void_p]
         L.fq_create_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_void_p]
         L.fq_comm_unique_id.argtypes = [C.c_void_p]
         L.fq_comm_init.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
@@ -142,6 +155,19 @@ def monotone_sigmas(N, P):
     out = np.zeros((n, N), np.uint8)
     lib().fq_monotone_sigmas(int(N), int(P), out.ctypes.data, n)
     return out
+
+
+def assign_count(N, P, all_limit=0):
+    """fq_pair_assign_count: |L(N, P, all_limit)|, the per-factor candidates of a corridor with P polytopes (< 0: refused)."""
+    return lib().fq_pair_assign_count(int(N), int(P), int(all_limit))
+
+
+def assign_offsets(poly_ofs, N, n_fac, all_limit=0):
+    """Candidate offsets (n_prob + 1) of one sweep with per-corridor lists, computed on the host from poly_ofs."""
+    counts = [assign_count(N, int(poly_ofs[j + 1] - poly_ofs[j]), all_limit) for j in range(len(poly_ofs) - 1)]
+    if min(counts, default=0) < 0:
+        raise FqError("assignment list of a corridor refused (longer than 2^20)")
+    return np.concatenate([[0], np.cumsum(np.asarray(counts, np.int64) * int(n_fac))]).astype(np.int32)
 
 
 def ellipsoid_decomp(path, obs, bbox=(2.0, 2.0, 1.0), inflate=0.42, z_ground=0.0, cap_rows=4096):
@@ -304,6 +330,17 @@ def pair_args(w, ptr, out_ptrs):
     return a
 
 
+def assign_args(all_limit, out_ptrs, max_poly_whole=0, max_poly_safe=0, n_cand_whole=0, n_cand_safe=0):
+    """PairAssign; out_ptrs: addresses of cand_ofs_whole, cand_ofs_safe, sigma_whole, sigma_safe (0/None/missing = NULL);
+    the max_poly_* / n_cand_* hints matter for the _dev entry only."""
+    s = PairAssign()
+    s.all_limit, s.max_poly_whole, s.max_poly_safe = int(all_limit), int(max_poly_whole), int(max_poly_safe)
+    s.n_cand_whole, s.n_cand_safe = int(n_cand_whole), int(n_cand_safe)
+    for k in ("cand_ofs_whole", "cand_ofs_safe", "sigma_whole", "sigma_safe"):
+        setattr(s, k, out_ptrs.get(k) or None)
+    return s
+
+
 class Solver:
     """Owns an fq_ctx on one GPU (or, with n_gpus > 1, a single-process multi-GPU group: fq_create_multi)."""
 
@@ -351,6 +388,32 @@ class Solver:
         fn = self._L.fq_replan_pairs_async if deferred else self._L.fq_replan_pairs
         self._check(fn(self._h, C.byref(a)))
         return out
+
+    def replan_pairs_assign(self, w, all_limit=0, want_candidates=True, want_coeffs=True, deferred=False):
+        """fq_replan_pairs_assign on a make_pair_workload dict (host arrays; its sigmas_* are not used: every corridor
+        gets its own list L(N, P_j, all_limit)).  -> dict(results, feasible_*/cost_* (per candidate, corridor j at
+        cand_ofs_*[j] .. cand_ofs_*[j+1]), coeffs_*, cand_ofs_whole, cand_ofs_safe, sigma_whole, sigma_safe (the winners'
+        assignments, 0s: none)).  deferred: valid after wait()."""
+        n = w["n_prob"]
+        ow = assign_offsets(w["poly_ofs_whole"], w["N_whole"], len(w["factors_whole"]), all_limit)
+        os_ = assign_offsets(w["poly_ofs_safe"], w["N_safe"], len(w["factors_safe"]), all_limit)
+        out = dict(results=np.zeros(n, PAIR_RESULT_DTYPE), cand_ofs_whole=np.zeros(n + 1, np.int32), cand_ofs_safe=np.zeros(n + 1, np.int32),
+                   sigma_whole=np.zeros((n, w["N_whole"]), np.uint8), sigma_safe=np.zeros((n, w["N_safe"]), np.uint8))
+        if want_candidates:
+            out.update(feasible_whole=np.zeros(int(ow[-1]), np.uint8), cost_whole=np.zeros(int(ow[-1])),
+                       feasible_safe=np.zeros(int(os_[-1]), np.uint8), cost_safe=np.zeros(int(os_[-1])))
+        if want_coeffs:
+            out.update(coeffs_whole=np.zeros((n, w["N_whole"], 12)), coeffs_safe=np.zeros((n, w["N_safe"], 12)))
+        a = pair_args(w, lambda k: None if k.startswith("sigmas_") else w[k].ctypes.data, {k: v.ctypes.data for k, v in out.items()})
+        a.n_sig_whole = a.n_sig_safe = 0
+        s = assign_args(all_limit, {k: out[k].ctypes.data for k in ("cand_ofs_whole", "cand_ofs_safe", "sigma_whole", "sigma_safe")})
+        fn = self._L.fq_replan_pairs_assign_async if deferred else self._L.fq_replan_pairs_assign
+        self._check(fn(self._h, C.byref(a), C.byref(s)))
+        return out
+
+    def replan_pairs_assign_dev(self, a, s, results_all=0, stream=0):
+        """fq_replan_pairs_assign_dev: `a` (PairArgs) and `s` (PairAssign) hold device addresses and the host hints."""
+        self._check(self._L.fq_replan_pairs_assign_dev(self._h, C.byref(a), C.byref(s), results_all or None, stream or None))
 
     def replan_pairs_dev(self, a, results_all=0, stream=0):
         """fq_replan_pairs_dev: `a` is a PairArgs holding device addresses."""

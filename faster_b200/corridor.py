@@ -313,6 +313,85 @@ def make_forest_pair_safe(whole, R, N=10, P_safe=4):
                 verts=path, seed=whole["seed"], profile="uav")
 
 
+def clip_path_to_sphere(path, centre, Ra):
+    """The path up to where it first leaves the sphere of radius Ra around `centre`, ending ON the sphere (the reference
+    clips its JPS path at Ra before trimming it, faster.cpp:361-393)."""
+    out = [np.asarray(path[0], float)]
+    for a, b in zip(path[:-1], path[1:]):
+        if np.linalg.norm(b - centre) <= Ra:
+            out.append(np.asarray(b, float))
+            continue
+        d = b - a                                      # |a + t d - centre| = Ra, t in [0, 1]
+        f = a - centre
+        qa, qb, qc = d @ d, 2 * (f @ d), f @ f - Ra * Ra
+        t = (-qb + np.sqrt(max(qb * qb - 4 * qa * qc, 0.0))) / (2 * qa) if qa > 0 else 0.0
+        out.append(a + np.clip(t, 0.0, 1.0) * d)
+        break
+    return np.array(out)
+
+
+def make_forest_pair_mixed(seed, N=10, max_poly_whole=3, max_poly_safe=4, Ra=4.0, r_fraction=0.6, n_trees=60, query=(0.6, 7.0),
+                           DC=0.01):
+    """One replan's (whole, safe) corridors in a random forest, with polytope counts as Faster::replan produces them: the JPS
+    path (product host code) to a goal `query` metres away, clipped at Ra, vertices at most 1.5 m apart (createMoreVertexes),
+    then deleteVertexes (utils.cpp:1117-1124: at most max_poly + 1 vertices), one polytope per segment.  So
+    P_whole = min(segments within Ra, max_poly_whole): a goal close by gives 1 or 2 polytopes.  The safe corridor starts at an
+    estimate of R -- the point r_fraction along the whole path (the device computes the true R from the whole winner) --
+    and follows the rest of the path, clipped at Ra around it and trimmed to max_poly_safe segments: near the goal it has
+    fewer too.  Nothing is padded.  -> (whole, safe) dicts as make_forest_pair_whole / make_forest_pair_safe."""
+    from . import capi
+    prof = UAV
+    rng = np.random.default_rng(seed)
+    _, centres, radii = make_forest(seed, n_trees=n_trees)
+    grid_jps, origin, res = voxelise_forest(centres, radii, inflation=0.47)
+    grid, _, _ = voxelise_forest(centres, radii)
+    for _ in range(400):
+        s = np.array([rng.uniform(-6, 6), rng.uniform(-6, 6), rng.uniform(0.8, 1.4)])
+        ang = rng.uniform(-np.pi, np.pi)
+        t = s + rng.uniform(*query) * np.array([np.cos(ang), np.sin(ang), 0.0])
+        t[2] = rng.uniform(0.8, 1.4)
+        if np.abs(t[:2]).max() > 7.5:
+            continue
+        path, _ = capi.jps3d_plan_world(grid_jps, origin, res, s, t, True)
+        if len(path) >= 2 and np.linalg.norm(path[-1] - path[0]) > 0.3:
+            break
+    else:
+        raise RuntimeError("no path found")
+    path_all = split_long_segments(path, 1.5)
+    verts = split_long_segments(clip_path_to_sphere(path, path[0], Ra), 1.5)[:max_poly_whole + 1]
+    obs = (np.argwhere(grid > 0)[:, ::-1] + 0.5) * res + origin
+    polys_w = capi.ellipsoid_decomp(verts, obs, prof["bbox"], prof["drone_radius"], prof["z_ground"], cap_rows=8192)
+    d0 = verts[1] - verts[0]
+    d0 /= np.linalg.norm(d0)
+    x0 = np.zeros(9)
+    x0[:3] = verts[0]
+    x0[3:6] = d0 * rng.uniform(*prof["v0"])
+    xf = np.zeros(9)
+    xf[:3] = verts[-1]
+    lim = np.array(prof["lim"])
+    whole = dict(N=N, P=len(polys_w), x0=x0, xf=xf, lim=lim, polys=polys_w, force_final=True, DC=DC, verts=verts,
+                 verts_all=path_all, obs=obs, seed=seed, profile="uav")
+    # R estimate: r_fraction of the whole path's length; the safe path continues along the full path from there
+    seg = np.linalg.norm(np.diff(verts, axis=0), axis=1)
+    at = r_fraction * seg.sum()
+    k = min(int(np.searchsorted(np.cumsum(seg), at)), len(seg) - 1)
+    u = (at - (np.cumsum(seg)[k] - seg[k])) / max(seg[k], 1e-12)
+    R = verts[k] + np.clip(u, 0.0, 1.0) * (verts[k + 1] - verts[k])
+    i = int(np.argmin([np.linalg.norm(v - verts[k + 1]) for v in path_all]))          # verts[k+1] in the full path
+    rest = [R] + [v for v in path_all[i:] if np.linalg.norm(v - R) > 0.3]
+    if len(rest) < 2:
+        rest = [R, verts[-1] if np.linalg.norm(verts[-1] - R) > 1e-3 else R + 0.5 * d0]
+    spath = split_long_segments(clip_path_to_sphere(np.array(rest), R, Ra), 1.5)[:max_poly_safe + 1]
+    polys_s = capi.ellipsoid_decomp(spath, obs, prof["bbox"], prof["drone_radius"], prof["z_ground"], cap_rows=8192)
+    R9 = np.zeros(9)
+    R9[:3] = R
+    xfs = np.zeros(9)
+    xfs[:3] = spath[-1]
+    safe = dict(N=N, P=len(polys_s), x0=R9, xf=xfs, lim=lim.copy(), polys=polys_s, force_final=False, DC=DC, verts=spath,
+                seed=seed, profile="uav")
+    return whole, safe
+
+
 # ------------------------------------------------------------------------------------------------------------------
 # Feasibility margins (SURVEY.md section 7, "hard parts"): Gurobi decides feasibility with FeasibilityTol 1e-6 on its own
 # scaled rows, this library with an absolute row tolerance (default 1e-8).  Candidates whose feasibility depends on

@@ -142,7 +142,9 @@ extern "C" int fq_has_feature(const char* name)
 {
   if (!name) return 0;
   const std::string n(name);
-  if (n == "sweep_early_exit" || n == "replan_pairs" || n == "multi_gpu" || n == "row_tol" || n == "certificates") return 1;
+  if (n == "sweep_early_exit" || n == "replan_pairs" || n == "multi_gpu" || n == "row_tol" || n == "certificates" ||
+      n == "replan_pairs_assign")
+    return 1;
   return 0;
 }
 

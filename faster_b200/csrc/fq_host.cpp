@@ -1,6 +1,7 @@
 // Host-side pieces of the hot path that need no GPU: plan tables, getDTInitial, resetX/fillX, sigma lists.
 #include "fq_plan.h"
 #include "fq_dtinit.h"
+#include "fq_assign.h"
 #include "../../include/faster_b200.h"
 
 #include <algorithm>
@@ -186,6 +187,13 @@ extern "C" long fq_monotone_sigmas(int N, int P, uint8_t* out, long cap)
     for (int j = i; j < N; j++) s[j] = v;
   }
   return count;
+}
+
+extern "C" long fq_pair_assign_count(int N, int P, long all_limit)
+{
+  if (N < 1 || N > FQ_MAX_N || P < 0 || P > FQ_MAX_POLY || all_limit < 0) return FQ_E_ARG;
+  const long long n = fqa::list_len(N, P, all_limit);
+  return n < 0 ? FQ_E_ARG : (long)n;
 }
 
 extern "C" int fq_abi_version(void) { return FQ_ABI_VERSION; }

@@ -655,6 +655,22 @@ cudaError_t fq_launch_expand_grid(int n_prob, int N, int n_fac, int n_sig, const
   return cudaGetLastError();
 }
 
+cudaError_t fq_launch_assign_offsets(int n_prob, int N, int n_fac, long long all_limit, int max_poly, long long n_cand,
+                                     const int* poly_ofs, int* cand_ofs, cudaStream_t stream)
+{
+  if (n_prob <= 0) return cudaSuccess;
+  fqp::fq_assign_offsets_kernel<<<1, 1024, 0, stream>>>(n_prob, N, n_fac, all_limit, max_poly, n_cand, poly_ofs, cand_ofs);
+  return cudaGetLastError();
+}
+
+cudaError_t fq_launch_expand_assign(int n_prob, int N, int n_fac, long long all_limit, const double* factors, const double* dt_base,
+                                    const int* poly_ofs, const int* cand_ofs, double* dt, uint8_t* sigma, cudaStream_t stream)
+{
+  if (n_prob <= 0) return cudaSuccess;
+  fqp::fq_expand_assign_kernel<<<n_prob, 256, 0, stream>>>(n_prob, N, n_fac, all_limit, factors, dt_base, poly_ofs, cand_ofs, dt, sigma);
+  return cudaGetLastError();
+}
+
 cudaError_t fq_launch_select_multi(const FqSelectMultiArgs& a, cudaStream_t stream)
 {
   if (a.n_prob <= 0) return cudaSuccess;

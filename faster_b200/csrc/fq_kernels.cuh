@@ -153,12 +153,28 @@ struct FqPairFinalArgs
   const int *win_idx_w, *win_idx_s, *n_samples, *k_safe;
   const double *win_cost_w, *win_cost_s, *win_dt_w, *win_dt_s, *dt_base_w, *dt_base_s, *x0_safe;
   fq_pair_result* out;
+  // per-corridor assignment lists (fq_replan_pairs_assign*): the sweeps' candidate offsets, whose ranges are n_fac x the
+  // corridor's list, replace n_sig_*; the winners' assignments (N x n_prob each) are copied to sigma_out_* if set.
+  // All NULL / 0: one shared list of n_sig_* assignments.
+  const int* cand_ofs_w = nullptr;
+  const int* cand_ofs_s = nullptr;
+  int n_fac_w = 0, n_fac_s = 0, N_w = 0, N_s = 0;
+  const uint8_t* win_sig_w = nullptr;
+  const uint8_t* win_sig_s = nullptr;
+  uint8_t* sigma_out_w = nullptr;
+  uint8_t* sigma_out_s = nullptr;
 };
 
 cudaError_t fq_launch_dtbase(int n_prob, int N, double DC, const double* x0, const double* xf, const double* lim,
                              double* dt_base, cudaStream_t stream);
 cudaError_t fq_launch_expand_grid(int n_prob, int N, int n_fac, int n_sig, const double* factors, const uint8_t* sig_list,
                                   const double* dt_base, double* dt, uint8_t* sigma, int* cand_ofs, cudaStream_t stream);
+// per-corridor assignment lists (fq_pair.cuh, fq_assign.h): offsets of n_fac x |L_j| (emptied when a corridor has more than
+// max_poly polytopes or the total is not n_cand), then the factor x list grid with unranked assignments
+cudaError_t fq_launch_assign_offsets(int n_prob, int N, int n_fac, long long all_limit, int max_poly, long long n_cand,
+                                     const int* poly_ofs, int* cand_ofs, cudaStream_t stream);
+cudaError_t fq_launch_expand_assign(int n_prob, int N, int n_fac, long long all_limit, const double* factors, const double* dt_base,
+                                    const int* poly_ofs, const int* cand_ofs, double* dt, uint8_t* sigma, cudaStream_t stream);
 cudaError_t fq_launch_select_multi(const FqSelectMultiArgs& a, cudaStream_t stream);
 cudaError_t fq_launch_pair_mid(const FqPairMidArgs& a, cudaStream_t stream);
 cudaError_t fq_launch_pair_final(const FqPairFinalArgs& a, cudaStream_t stream);

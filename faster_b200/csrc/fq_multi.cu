@@ -6,6 +6,7 @@
 //   * one process, several GPUs (what the reference's single planner process would do): fq_create_multi.
 // NCCL is loaded lazily with dlopen (libnccl.so.2; FQ_NCCL_LIB overrides), so the library has no link-time dependency
 // on it and single-GPU use needs no NCCL at all.
+#include "fq_assign.h"
 #include "fq_ctx.h"
 
 #include <algorithm>
@@ -265,7 +266,10 @@ int exchange(fq_ctx* g, const std::vector<T*>& send, const std::vector<T*>& recv
 // per-candidate arrays travel straight from each member into the caller's arrays.  Rank context (one process per GPU):
 // every rank passes the SAME full description and solves its own shard; after the all-gather every rank holds every
 // corridor's result record, while per-candidate outputs are filled for the rank's own corridors only.
-int fq_replan_pairs_sharded(fq_ctx* g, const fq_pair_args* a, bool deferred)
+// Per-corridor assignment lists (as != NULL): the corridors' candidate counts differ, so the shards are balanced by
+// candidates -- fq_shard_range over the offsets of whole + safe candidates, computed here from poly_ofs -- and each shard's
+// per-candidate outputs start at the shard's first offset.  The caller's cand_ofs_* come from the same host offsets.
+int fq_replan_pairs_sharded(fq_ctx* g, const fq_pair_args* a, bool deferred, const fq_pair_assign* as)
 {
   fq_ctx* ctx = g;
   if (!a || a->n_prob <= 0 || !a->results) return fq_fail(g, FQ_E_ARG, "bad arguments");
@@ -274,8 +278,10 @@ int fq_replan_pairs_sharded(fq_ctx* g, const fq_pair_args* a, bool deferred)
   if (!a->x0 || !a->xf_whole || !a->xf_safe || !a->lim || !a->poly_ofs_whole || !a->face_ofs_whole || !a->poly_ofs_safe ||
       !a->face_ofs_safe)
     return fq_fail(g, FQ_E_ARG, "NULL argument");
-  if (a->n_fac_whole <= 0 || a->n_fac_safe <= 0 || a->n_sig_whole <= 0 || a->n_sig_safe <= 0)
+  if (a->n_fac_whole <= 0 || a->n_fac_safe <= 0 || (!as && (a->n_sig_whole <= 0 || a->n_sig_safe <= 0)))
     return fq_fail(g, FQ_E_ARG, "empty factor / assignment grid");
+  if (as && (a->sigmas_whole || a->sigmas_safe || a->n_sig_whole != 0 || a->n_sig_safe != 0))
+    return fq_fail(g, FQ_E_ARG, "per-corridor assignment lists: sigmas_* must be NULL and n_sig_* 0");
   for (int j = 0; j < a->n_prob; j++)
     if (a->poly_ofs_whole[j + 1] < a->poly_ofs_whole[j] || a->poly_ofs_safe[j + 1] < a->poly_ofs_safe[j])
       return fq_fail(g, FQ_E_ARG, "poly_ofs not monotone");
@@ -283,9 +289,39 @@ int fq_replan_pairs_sharded(fq_ctx* g, const fq_pair_args* a, bool deferred)
   const bool group = g->is_group;
   const int n_local = group ? world : 1;
   const size_t ncw1 = (size_t)a->n_fac_whole * a->n_sig_whole, ncs1 = (size_t)a->n_fac_safe * a->n_sig_safe;
+  // per-corridor lists: candidate offsets of the two sweeps and of both together (the shards' weights)
+  std::vector<long long> ofw, ofs;
+  std::vector<int> ofb;
+  if (as)
+  {
+    if (a->N_whole < 1 || a->N_whole > FQ_MAX_N || a->N_safe < 1 || a->N_safe > FQ_MAX_N || as->all_limit < 0)
+      return fq_fail(g, FQ_E_ARG, "N out of range or all_limit < 0");
+    ofw.assign(P + 1, 0); ofs.assign(P + 1, 0); ofb.assign(P + 1, 0);
+    for (int j = 0; j < P; j++)
+    {
+      const int pw = a->poly_ofs_whole[j + 1] - a->poly_ofs_whole[j], ps = a->poly_ofs_safe[j + 1] - a->poly_ofs_safe[j];
+      if (pw > FQ_MAX_POLY || ps > FQ_MAX_POLY) return fq_fail(g, FQ_E_ARG, "more than FQ_MAX_POLY polytopes in a corridor");
+      const long long lw = fqa::list_len(a->N_whole, pw, as->all_limit), ls = fqa::list_len(a->N_safe, ps, as->all_limit);
+      if (lw < 0 || ls < 0) return fq_fail(g, FQ_E_ARG, "assignment list of a corridor longer than 2^20");
+      ofw[j + 1] = ofw[j] + lw * a->n_fac_whole;
+      ofs[j + 1] = ofs[j] + ls * a->n_fac_safe;
+      if (ofw[j + 1] > (1LL << 30) || ofs[j + 1] > (1LL << 30)) return fq_fail(g, FQ_E_ARG, "too many candidates");
+      ofb[j + 1] = (int)std::min<long long>(ofw[j + 1] + ofs[j + 1], 0x7fffffffLL);
+    }
+  }
   int pad = 0;
   std::vector<int> lo(world), hi(world);
-  for (int r = 0; r < world; r++) { fq_shard_range(P, nullptr, r, world, &lo[r], &hi[r]); pad = std::max(pad, hi[r] - lo[r]); }
+  for (int r = 0; r < world; r++)
+  {
+    fq_shard_range(P, as ? ofb.data() : nullptr, r, world, &lo[r], &hi[r]);
+    pad = std::max(pad, hi[r] - lo[r]);
+  }
+  if (as)
+    for (int j = 0; j <= P; j++)
+    {
+      if (as->cand_ofs_whole) as->cand_ofs_whole[j] = (int)ofw[j];
+      if (as->cand_ofs_safe) as->cand_ofs_safe[j] = (int)ofs[j];
+    }
   std::vector<fq_pair_result*> d_res(n_local, nullptr), d_all(n_local, nullptr);
   for (int i = 0; i < n_local; i++)
   {
@@ -311,13 +347,22 @@ int fq_replan_pairs_sharded(fq_ctx* g, const fq_pair_args* a, bool deferred)
     s.lim = a->lim + 3 * (size_t)lo[r];
     s.poly_ofs_whole = cw.poly_ofs.data(); s.face_ofs_whole = cw.face_ofs.data(); s.Ab_whole = cw.Ab;
     s.poly_ofs_safe = cs.poly_ofs.data(); s.face_ofs_safe = cs.face_ofs.data(); s.Ab_safe = cs.Ab;
-    if (a->feasible_whole) { s.feasible_whole = a->feasible_whole + ncw1 * lo[r]; s.cost_whole = a->cost_whole + ncw1 * lo[r]; }
-    if (a->feasible_safe) { s.feasible_safe = a->feasible_safe + ncs1 * lo[r]; s.cost_safe = a->cost_safe + ncs1 * lo[r]; }
+    // first candidate of the shard in the caller's per-candidate arrays
+    const size_t cw0 = as ? (size_t)ofw[lo[r]] : ncw1 * lo[r], cs0 = as ? (size_t)ofs[lo[r]] : ncs1 * lo[r];
+    if (a->feasible_whole) { s.feasible_whole = a->feasible_whole + cw0; s.cost_whole = a->cost_whole + cw0; }
+    if (a->feasible_safe) { s.feasible_safe = a->feasible_safe + cs0; s.cost_safe = a->cost_safe + cs0; }
     if (a->coeffs_whole) s.coeffs_whole = a->coeffs_whole + 12 * (size_t)a->N_whole * lo[r];
     if (a->coeffs_safe) s.coeffs_safe = a->coeffs_safe + 12 * (size_t)a->N_safe * lo[r];
     s.results = a->results + lo[r];            // not copied back (copy_results = false): the gathered table is
+    fq_pair_assign sa{};
+    if (as)
+    { // the offsets were written above; the winners' assignments go straight into the caller's rows of the shard
+      sa.all_limit = as->all_limit;
+      sa.sigma_whole = as->sigma_whole ? as->sigma_whole + (size_t)a->N_whole * lo[r] : nullptr;
+      sa.sigma_safe = as->sigma_safe ? as->sigma_safe + (size_t)a->N_safe * lo[r] : nullptr;
+    }
     fq_pair_result* dr = nullptr;
-    int rc = fq_replan_pairs_host_ex(c, &s, true, &dr, false);
+    int rc = fq_replan_pairs_host_ex(c, &s, true, &dr, false, as ? &sa : nullptr);
     if (rc) { if (c != g) g->err = c->err; return rc; }
     e = cudaMemcpyAsync(d_res[i], dr, sizeof(fq_pair_result) * (size_t)n, cudaMemcpyDeviceToDevice, c->stream);
     if (e != cudaSuccess) return fq_cuda_fail(g, e, "gather staging");

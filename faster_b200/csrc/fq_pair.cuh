@@ -4,6 +4,7 @@
 // without a host round trip.  The solves are the ordinary batch kernel (fq_kernels_t.cuh); this file holds the small
 // kernels between them.  All of them are latency-trivial (one thread / one CTA per corridor, or a grid-stride copy).
 #pragma once
+#include "fq_assign.h"
 #include "fq_dtinit.h"
 
 namespace fqp
@@ -50,6 +51,81 @@ __global__ void fq_expand_grid_kernel(int n_prob, int N, int n_fac, int n_sig, c
   }
   for (long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x; j <= n_prob; j += (long long)gridDim.x * blockDim.x)
     cand_ofs[j] = (int)(j * per);
+}
+
+// ---- per-corridor assignment lists (fq_replan_pairs_assign*; the lists are defined in fq_assign.h)
+
+// cand_ofs[0 .. n_prob] = exclusive scan of n_fac x |L(N, P_j, all_limit)|, P_j from poly_ofs.  One CTA (any size up to
+// 1024): every thread scans a contiguous run of corridors.  The sweep's buffers were sized for n_cand candidates; when a
+// corridor has more than max_poly polytopes, a list is refused (longer than 2^20) or the total is not n_cand, EVERY range
+// is left empty (cand_ofs all 0): no candidate is expanded or solved and every corridor's winner of the sweep is "none".
+__global__ void __launch_bounds__(1024) fq_assign_offsets_kernel(int n_prob, int N, int n_fac, long long all_limit, int max_poly,
+                                                                 long long n_cand, const int* __restrict__ poly_ofs,
+                                                                 int* __restrict__ cand_ofs)
+{
+  __shared__ long long s_run[1024];
+  __shared__ long long s_total;
+  __shared__ int s_bad;
+  const int T = blockDim.x, tid = threadIdx.x;
+  const int per = (n_prob + T - 1) / T;
+  const int j0 = min(n_prob, tid * per), j1 = min(n_prob, j0 + per);
+  if (tid == 0) s_bad = 0;
+  __syncthreads();
+  long long sum = 0;
+  bool bad = false;
+  for (int j = j0; j < j1; j++)
+  {
+    const int P = poly_ofs[j + 1] - poly_ofs[j];
+    const long long L = fqa::list_len(N, P, all_limit);
+    if (P < 0 || P > max_poly || L < 0) bad = true;
+    else sum += L * n_fac;
+  }
+  if (bad) s_bad = 1;
+  s_run[tid] = sum;
+  __syncthreads();
+  if (tid == 0)
+  {
+    long long run = 0;
+    for (int i = 0; i < T; i++) { const long long x = s_run[i]; s_run[i] = run; run += x; }
+    s_total = run;
+    if (run != n_cand) s_bad = 1;
+  }
+  __syncthreads();
+  const bool empty = s_bad != 0;
+  long long run = s_run[tid];
+  for (int j = j0; j < j1; j++)
+  {
+    cand_ofs[j] = empty ? 0 : (int)run;
+    if (!empty) run += fqa::list_len(N, poly_ofs[j + 1] - poly_ofs[j], all_limit) * n_fac;
+  }
+  if (tid == 0) cand_ofs[n_prob] = empty ? 0 : (int)s_total;
+}
+
+// candidates of corridor j = factors x L_j, factor-major: dt = factor * dt_base[j] (as fq_expand_grid_kernel), sigma =
+// the assignment's unranked index within L_j.  One CTA per corridor, grid-striding over its own candidates; the binomials
+// of the non-decreasing unranking sit in shared memory.
+__global__ void __launch_bounds__(256) fq_expand_assign_kernel(int n_prob, int N, int n_fac, long long all_limit,
+                                                               const double* __restrict__ factors, const double* __restrict__ dt_base,
+                                                               const int* __restrict__ poly_ofs, const int* __restrict__ cand_ofs,
+                                                               double* __restrict__ dt, uint8_t* __restrict__ sigma)
+{
+  __shared__ long long s_binom[48 * 17];
+  for (int i = threadIdx.x; i < 48 * 17; i += blockDim.x) s_binom[i] = fqa::binom(i / 17, i % 17);
+  __syncthreads();
+  const int j = blockIdx.x;
+  if (j >= n_prob) return;
+  const int c0 = cand_ofs[j], n = cand_ofs[j + 1] - c0;
+  const int P = poly_ofs[j + 1] - poly_ofs[j];
+  const long long L = fqa::list_len(N, P, all_limit);
+  if (n <= 0 || L <= 0 || (long long)n != L * n_fac) return;        // an emptied sweep (fq_assign_offsets_kernel)
+  const bool all = fqa::use_all(N, P, all_limit);
+  const double base = dt_base[j];
+  for (int i = threadIdx.x; i < n; i += blockDim.x)
+  {
+    const int f = (int)(i / L);
+    dt[c0 + i] = FQ_MUL(factors[f], base);
+    fqa::unrank(N, P, all, i - (long long)f * L, s_binom, sigma + (size_t)(c0 + i) * N);
+  }
 }
 
 // genNewTraj's selection (solverGurobi.cpp:445-472) for every problem of a batch: the winner is the feasible candidate
@@ -153,10 +229,17 @@ __global__ void fq_pair_final_kernel(const FqPairFinalArgs a)
   if (j >= a.n_prob) return;
   fq_pair_result r;
   const int ww = a.win_idx_w[j], ws = a.win_idx_s[j];
-  r.whole_dt_index = ww >= 0 ? ww / a.n_sig_w : -1;
-  r.whole_sigma_index = ww >= 0 ? ww % a.n_sig_w : -1;
-  r.safe_dt_index = ws >= 0 ? ws / a.n_sig_s : -1;
-  r.safe_sigma_index = ws >= 0 ? ws % a.n_sig_s : -1;
+  // list lengths: shared (n_sig_*), or per corridor (its candidates / n_fac; a corridor without candidates has no winner)
+  const int lw = a.cand_ofs_w ? (a.cand_ofs_w[j + 1] - a.cand_ofs_w[j]) / a.n_fac_w : a.n_sig_w;
+  const int ls = a.cand_ofs_s ? (a.cand_ofs_s[j + 1] - a.cand_ofs_s[j]) / a.n_fac_s : a.n_sig_s;
+  r.whole_dt_index = ww >= 0 ? ww / lw : -1;
+  r.whole_sigma_index = ww >= 0 ? ww % lw : -1;
+  r.safe_dt_index = ws >= 0 ? ws / ls : -1;
+  r.safe_sigma_index = ws >= 0 ? ws % ls : -1;
+  if (a.sigma_out_w)
+    for (int t = 0; t < a.N_w; t++) a.sigma_out_w[(size_t)j * a.N_w + t] = a.win_sig_w[(size_t)j * a.N_w + t];
+  if (a.sigma_out_s)
+    for (int t = 0; t < a.N_s; t++) a.sigma_out_s[(size_t)j * a.N_s + t] = a.win_sig_s[(size_t)j * a.N_s + t];
   r.whole_cost = a.win_cost_w[j]; r.safe_cost = a.win_cost_s[j];
   r.whole_dt = a.win_dt_w[j]; r.safe_dt = a.win_dt_s[j];
   r.whole_dt_base = a.dt_base_w[j]; r.safe_dt_base = a.dt_base_s[j];

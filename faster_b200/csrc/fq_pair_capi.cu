@@ -1,6 +1,7 @@
 // Chained replan (include/faster_b200.h: fq_replan_pairs*): whole sweep -> selection -> R -> safe sweep -> selection for
 // many corridors in one submission.  Reference data flow: faster/src/faster.cpp:406-430 (whole), :474-475 (R), :521-537
 // (safe).  Kernels: the batch solve (fq_kernels_t.cuh) and the small kernels of fq_pair.cuh.
+#include "fq_assign.h"
 #include "fq_ctx.h"
 
 #include <algorithm>
@@ -25,33 +26,53 @@ T* carve(char*& p, size_t count)
   return r;
 }
 
-int check_common(fq_ctx* ctx, const fq_pair_args* a)
+// shared = false: per-corridor lists (fq_replan_pairs_assign*), whose candidate counts the callers check themselves
+int check_common(fq_ctx* ctx, const fq_pair_args* a, bool shared = true)
 {
   if (!a) return fq_fail(ctx, FQ_E_ARG, "args is NULL");
   if (a->n_prob <= 0) return fq_fail(ctx, FQ_E_ARG, "n_prob <= 0");
   if (a->N_whole < 3 || a->N_whole > FQ_MAX_N || a->N_safe < 2 || a->N_safe > FQ_MAX_N) return fq_fail(ctx, FQ_E_ARG, "N out of range");
   if (!(a->DC > 0) || !(a->r_fraction >= 0 && a->r_fraction <= 1)) return fq_fail(ctx, FQ_E_ARG, "DC must be > 0 and r_fraction in [0, 1]");
-  if (a->n_fac_whole <= 0 || a->n_fac_safe <= 0 || a->n_sig_whole <= 0 || a->n_sig_safe <= 0)
+  if (!shared)
+  {
+    if (a->n_fac_whole <= 0 || a->n_fac_safe <= 0) return fq_fail(ctx, FQ_E_ARG, "empty factor grid");
+    if (a->sigmas_whole || a->sigmas_safe || a->n_sig_whole != 0 || a->n_sig_safe != 0)
+      return fq_fail(ctx, FQ_E_ARG, "per-corridor assignment lists: sigmas_* must be NULL and n_sig_* 0");
+  }
+  else if (a->n_fac_whole <= 0 || a->n_fac_safe <= 0 || a->n_sig_whole <= 0 || a->n_sig_safe <= 0)
     return fq_fail(ctx, FQ_E_ARG, "empty factor / assignment grid");
-  if ((long long)a->n_prob * a->n_fac_whole * a->n_sig_whole > (1LL << 30) || (long long)a->n_prob * a->n_fac_safe * a->n_sig_safe > (1LL << 30))
+  if (shared &&
+      ((long long)a->n_prob * a->n_fac_whole * a->n_sig_whole > (1LL << 30) || (long long)a->n_prob * a->n_fac_safe * a->n_sig_safe > (1LL << 30)))
     return fq_fail(ctx, FQ_E_ARG, "too many candidates");
   if (!a->x0 || !a->xf_whole || !a->xf_safe || !a->lim || !a->poly_ofs_whole || !a->face_ofs_whole || !a->poly_ofs_safe ||
       !a->face_ofs_safe || !a->factors_whole || !a->factors_safe || !a->results)
     return fq_fail(ctx, FQ_E_ARG, "NULL argument");
   return 0;
 }
-}  // namespace
 
-// every pointer of `a` is a device pointer
-extern "C" int fq_replan_pairs_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_result* results_all, void* stream_v)
+// the assignment lists of one chain: one shared list per sweep (fq_replan_pairs*), or a list per corridor generated on the
+// device (fq_replan_pairs_assign*)
+struct Lists
 {
-  if (!ctx) return FQ_E_ARG;
-  if (int rc = check_common(ctx, a)) return rc;
-  if (((uintptr_t)a->Ab_whole & 15) || ((uintptr_t)a->Ab_safe & 15)) return fq_fail(ctx, FQ_E_ARG, "Ab must be 16-byte aligned");
-  FQ_CUDA(cudaSetDevice(ctx->device));
-  cudaStream_t st = stream_v ? (cudaStream_t)stream_v : ctx->stream;
+  const fq_pair_assign* as = nullptr;   // per-corridor lists (outputs are device pointers), or nullptr: fq_pair_args' lists
+  size_t ncw = 0, ncs = 0;              // candidates of the whole / safe sweep
+  int mcw = 0, mcs = 0;                 // largest candidate count of one corridor
+  int eew = 0, ees = 0;                 // candidates per time allocation (sizes an early-exit grid): the longest list
+};
+
+// largest |L(N, P, all_limit)| over P = 0 .. max_poly, or -1 when the list of max_poly polytopes is refused
+long long longest_list(int N, int max_poly, long long all_limit)
+{
+  long long m = 0;
+  for (int p = 0; p <= max_poly; p++) m = std::max(m, fqa::list_len(N, p, all_limit));
+  return fqa::list_len(N, max_poly, all_limit) < 0 ? -1 : m;
+}
+
+// the chain itself, every pointer a device pointer; `a` and the lists are checked
+int run_chain(fq_ctx* ctx, const fq_pair_args* a, const Lists& l, fq_pair_result* results_all, cudaStream_t st)
+{
   const int P = a->n_prob, Nw = a->N_whole, Ns = a->N_safe;
-  const size_t ncw = (size_t)P * a->n_fac_whole * a->n_sig_whole, ncs = (size_t)P * a->n_fac_safe * a->n_sig_safe;
+  const size_t ncw = l.ncw, ncs = l.ncs;
   // ---- scratch
   size_t need = 0;
   {
@@ -86,7 +107,7 @@ extern "C" int fq_replan_pairs_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_r
     double* cost_s = a->cost_safe ? a->cost_safe : s.cost_s;
     double* coeffs_w = a->coeffs_whole ? a->coeffs_whole : s.coeffs_w;
     double* coeffs_s = a->coeffs_safe ? a->coeffs_safe : s.coeffs_s;
-    const int mcw = a->n_fac_whole * a->n_sig_whole, mcs = a->n_fac_safe * a->n_sig_safe;
+    const int mcw = l.mcw, mcs = l.mcs;
     // the corridors of the two sweeps; each launch adds its candidates and outputs
     FqKernelArgs whole{}, safe{};
     whole.N = Nw; whole.force_final = 1; whole.n_prob = P; whole.x0 = a->x0; whole.xf = a->xf_whole; whole.lim = a->lim;
@@ -96,11 +117,19 @@ extern "C" int fq_replan_pairs_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_r
 
     // ---- whole sweep (faster.cpp:406-418)
     FQ_CUDA(fq_launch_dtbase(P, Nw, a->DC, a->x0, a->xf_whole, a->lim, s.dt_base_w, st));
-    FQ_CUDA(fq_launch_expand_grid(P, Nw, a->n_fac_whole, a->n_sig_whole, a->factors_whole, a->sigmas_whole, s.dt_base_w, s.dt_w,
-                                  s.sig_w, s.cand_ofs_w, st));
+    if (!l.as)
+      FQ_CUDA(fq_launch_expand_grid(P, Nw, a->n_fac_whole, a->n_sig_whole, a->factors_whole, a->sigmas_whole, s.dt_base_w, s.dt_w,
+                                    s.sig_w, s.cand_ofs_w, st));
+    else
+    {
+      FQ_CUDA(fq_launch_assign_offsets(P, Nw, a->n_fac_whole, l.as->all_limit, l.as->max_poly_whole, (long long)ncw, a->poly_ofs_whole,
+                                       s.cand_ofs_w, st));
+      FQ_CUDA(fq_launch_expand_assign(P, Nw, a->n_fac_whole, l.as->all_limit, a->factors_whole, s.dt_base_w, a->poly_ofs_whole,
+                                      s.cand_ofs_w, s.dt_w, s.sig_w, st));
+    }
     FqKernelArgs k = whole;
     k.cand_ofs = s.cand_ofs_w; k.dt = s.dt_w; k.sigma = s.sig_w; k.feasible = feas_w; k.cost = cost_w;
-    k.sorted_dt = 1; k.ee_width = a->n_sig_whole;         // factor-major grid, ascending factors
+    k.sorted_dt = 1; k.ee_width = l.eew;                  // factor-major grid, ascending factors
     int rc = fq_launch_solve_ctx(ctx, k, mcw, a->max_poly_faces_whole, st);
     if (rc) return rc;
     FqSelectMultiArgs sw;
@@ -119,11 +148,19 @@ extern "C" int fq_replan_pairs_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_r
     m.win_idx = s.win_idx_w; m.x0_safe = s.x0_safe; m.n_samples = s.n_samples; m.k_safe = s.k_safe;
     FQ_CUDA(fq_launch_pair_mid(m, st));
     FQ_CUDA(fq_launch_dtbase(P, Ns, a->DC, s.x0_safe, a->xf_safe, a->lim, s.dt_base_s, st));
-    FQ_CUDA(fq_launch_expand_grid(P, Ns, a->n_fac_safe, a->n_sig_safe, a->factors_safe, a->sigmas_safe, s.dt_base_s, s.dt_s,
-                                  s.sig_s, s.cand_ofs_s, st));
+    if (!l.as)
+      FQ_CUDA(fq_launch_expand_grid(P, Ns, a->n_fac_safe, a->n_sig_safe, a->factors_safe, a->sigmas_safe, s.dt_base_s, s.dt_s,
+                                    s.sig_s, s.cand_ofs_s, st));
+    else
+    {
+      FQ_CUDA(fq_launch_assign_offsets(P, Ns, a->n_fac_safe, l.as->all_limit, l.as->max_poly_safe, (long long)ncs, a->poly_ofs_safe,
+                                       s.cand_ofs_s, st));
+      FQ_CUDA(fq_launch_expand_assign(P, Ns, a->n_fac_safe, l.as->all_limit, a->factors_safe, s.dt_base_s, a->poly_ofs_safe,
+                                      s.cand_ofs_s, s.dt_s, s.sig_s, st));
+    }
     k = safe;
     k.cand_ofs = s.cand_ofs_s; k.dt = s.dt_s; k.sigma = s.sig_s; k.feasible = feas_s; k.cost = cost_s;
-    k.sorted_dt = 1; k.ee_width = a->n_sig_safe;
+    k.sorted_dt = 1; k.ee_width = l.ees;
     rc = fq_launch_solve_ctx(ctx, k, mcs, a->max_poly_faces_safe, st);
     if (rc) return rc;
     FqSelectMultiArgs ss = sw;
@@ -142,6 +179,16 @@ extern "C" int fq_replan_pairs_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_r
     f.n_samples = s.n_samples; f.k_safe = s.k_safe; f.win_cost_w = s.win_cost_w; f.win_cost_s = s.win_cost_s;
     f.win_dt_w = s.win_dt_w; f.win_dt_s = s.win_dt_s; f.dt_base_w = s.dt_base_w; f.dt_base_s = s.dt_base_s; f.x0_safe = s.x0_safe;
     f.out = a->results;
+    if (l.as)
+    {
+      f.cand_ofs_w = s.cand_ofs_w; f.cand_ofs_s = s.cand_ofs_s; f.n_fac_w = a->n_fac_whole; f.n_fac_s = a->n_fac_safe;
+      f.N_w = Nw; f.N_s = Ns; f.win_sig_w = s.win_sig_w; f.win_sig_s = s.win_sig_s;
+      f.sigma_out_w = l.as->sigma_whole; f.sigma_out_s = l.as->sigma_safe;
+      if (l.as->cand_ofs_whole)
+        FQ_CUDA(cudaMemcpyAsync(l.as->cand_ofs_whole, s.cand_ofs_w, sizeof(int) * (size_t)(P + 1), cudaMemcpyDeviceToDevice, st));
+      if (l.as->cand_ofs_safe)
+        FQ_CUDA(cudaMemcpyAsync(l.as->cand_ofs_safe, s.cand_ofs_s, sizeof(int) * (size_t)(P + 1), cudaMemcpyDeviceToDevice, st));
+    }
     FQ_CUDA(fq_launch_pair_final(f, st));
     // ---- the path's one exchange: every rank's result records to every rank (north_star: one all-gather, only when the
     //      batch is spread over several GPUs)
@@ -155,12 +202,56 @@ extern "C" int fq_replan_pairs_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_r
   }
   return 0;
 }
+}  // namespace
 
-int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results)
+// every pointer of `a` is a device pointer
+extern "C" int fq_replan_pairs_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_result* results_all, void* stream_v)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (int rc = check_common(ctx, a)) return rc;
+  if (((uintptr_t)a->Ab_whole & 15) || ((uintptr_t)a->Ab_safe & 15)) return fq_fail(ctx, FQ_E_ARG, "Ab must be 16-byte aligned");
+  FQ_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = stream_v ? (cudaStream_t)stream_v : ctx->stream;
+  Lists l;
+  l.ncw = (size_t)a->n_prob * a->n_fac_whole * a->n_sig_whole; l.ncs = (size_t)a->n_prob * a->n_fac_safe * a->n_sig_safe;
+  l.mcw = a->n_fac_whole * a->n_sig_whole; l.mcs = a->n_fac_safe * a->n_sig_safe;
+  l.eew = a->n_sig_whole; l.ees = a->n_sig_safe;
+  return run_chain(ctx, a, l, results_all, st);
+}
+
+// every pointer of `a` and of `as` is a device pointer; the sweeps' sizes come from the hints of `as`
+extern "C" int fq_replan_pairs_assign_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, fq_pair_result* results_all,
+                                          void* stream_v)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (int rc = check_common(ctx, a, false)) return rc;
+  if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
+  if (as->all_limit < 0) return fq_fail(ctx, FQ_E_ARG, "all_limit < 0");
+  if (as->max_poly_whole < 0 || as->max_poly_whole > FQ_MAX_POLY || as->max_poly_safe < 0 || as->max_poly_safe > FQ_MAX_POLY)
+    return fq_fail(ctx, FQ_E_ARG, "max_poly_* out of range (0..FQ_MAX_POLY)");
+  if (as->n_cand_whole < 0 || as->n_cand_whole > (1L << 30) || as->n_cand_safe < 0 || as->n_cand_safe > (1L << 30))
+    return fq_fail(ctx, FQ_E_ARG, "too many candidates (n_cand_* out of 0..2^30)");
+  const long long lw = longest_list(a->N_whole, as->max_poly_whole, as->all_limit);
+  const long long ls = longest_list(a->N_safe, as->max_poly_safe, as->all_limit);
+  if (lw < 0 || ls < 0) return fq_fail(ctx, FQ_E_ARG, "assignment list longer than 2^20");
+  if (lw * a->n_fac_whole > (1LL << 30) || ls * a->n_fac_safe > (1LL << 30)) return fq_fail(ctx, FQ_E_ARG, "too many candidates");
+  if (((uintptr_t)a->Ab_whole & 15) || ((uintptr_t)a->Ab_safe & 15)) return fq_fail(ctx, FQ_E_ARG, "Ab must be 16-byte aligned");
+  FQ_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = stream_v ? (cudaStream_t)stream_v : ctx->stream;
+  Lists l;
+  l.as = as;
+  l.ncw = (size_t)as->n_cand_whole; l.ncs = (size_t)as->n_cand_safe;
+  l.mcw = (int)(lw * a->n_fac_whole); l.mcs = (int)(ls * a->n_fac_safe);
+  l.eew = (int)lw; l.ees = (int)ls;
+  return run_chain(ctx, a, l, results_all, st);
+}
+
+int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results,
+                            const fq_pair_assign* as)
 {
   if (!ctx) return FQ_E_ARG;
   if (int rc = fq_settle(ctx)) return rc;
-  if (int rc = check_common(ctx, a)) return rc;
+  if (int rc = check_common(ctx, a, as == nullptr)) return rc;
   const int P = a->n_prob, Nw = a->N_whole, Ns = a->N_safe;
   // ---- validate the two corridor descriptions
   auto check = [&](const int* po, const int* fo, const double* Ab, FqCorridorSizes* sizes) -> const char* {
@@ -182,9 +273,29 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
     if (a->factors_whole[i] < a->factors_whole[i - 1]) return fq_fail(ctx, FQ_E_ARG, "factors_whole must be ascending");
   for (int i = 1; i < a->n_fac_safe; i++)
     if (a->factors_safe[i] < a->factors_safe[i - 1]) return fq_fail(ctx, FQ_E_ARG, "factors_safe must be ascending");
-  if (cw.n_poly > 0 && !a->sigmas_whole) return fq_fail(ctx, FQ_E_ARG, "sigmas_whole is NULL");
-  if (cs.n_poly > 0 && !a->sigmas_safe) return fq_fail(ctx, FQ_E_ARG, "sigmas_safe is NULL");
+  size_t ncw = (size_t)P * a->n_fac_whole * a->n_sig_whole, ncs = (size_t)P * a->n_fac_safe * a->n_sig_safe;
+  fq_pair_assign da{};                 // per-corridor lists: the device-side outputs and exact sizes
+  if (as)
+  {
+    if (as->all_limit < 0) return fq_fail(ctx, FQ_E_ARG, "all_limit < 0");
+    long long tw = 0, ts = 0;
+    int mpw = 0, mps = 0;
+    for (int j = 0; j < P; j++)
+    {
+      const int pw = a->poly_ofs_whole[j + 1] - a->poly_ofs_whole[j], ps = a->poly_ofs_safe[j + 1] - a->poly_ofs_safe[j];
+      const long long lw = fqa::list_len(Nw, pw, as->all_limit), ls = fqa::list_len(Ns, ps, as->all_limit);
+      if (lw < 0 || ls < 0) return fq_fail(ctx, FQ_E_ARG, "assignment list of a corridor longer than 2^20");
+      tw += lw * a->n_fac_whole; ts += ls * a->n_fac_safe;
+      mpw = std::max(mpw, pw); mps = std::max(mps, ps);
+    }
+    if (tw > (1LL << 30) || ts > (1LL << 30)) return fq_fail(ctx, FQ_E_ARG, "too many candidates");
+    ncw = (size_t)tw; ncs = (size_t)ts;
+    da.all_limit = as->all_limit; da.max_poly_whole = mpw; da.max_poly_safe = mps; da.n_cand_whole = (long)tw; da.n_cand_safe = (long)ts;
+  }
+  if (!as && cw.n_poly > 0 && !a->sigmas_whole) return fq_fail(ctx, FQ_E_ARG, "sigmas_whole is NULL");
+  if (!as && cs.n_poly > 0 && !a->sigmas_safe) return fq_fail(ctx, FQ_E_ARG, "sigmas_safe is NULL");
   // assignments must name existing polytopes of EVERY corridor they are applied to
+  if (!as)
   {
     int min_pw = FQ_MAX_POLY, min_ps = FQ_MAX_POLY;
     for (int j = 0; j < P; j++)
@@ -197,7 +308,6 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   }
   FQ_CUDA(cudaSetDevice(ctx->device));
   // ---- one packed upload
-  const size_t ncw = (size_t)P * a->n_fac_whole * a->n_sig_whole, ncs = (size_t)P * a->n_fac_safe * a->n_sig_safe;
   size_t o = 0;
   auto put = [&](size_t bytes) { const size_t at = o; o = fq_align16(o + bytes); return at; };
   const size_t oAbw = put(32 * (size_t)std::max(cw.n_face, 1)), oAbs = put(32 * (size_t)std::max(cs.n_face, 1));
@@ -211,6 +321,8 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   const size_t ores = put(sizeof(fq_pair_result) * (size_t)P);
   const size_t ocow = put(96 * (size_t)Nw * P), ocos = put(96 * (size_t)Ns * P);
   const size_t ocw = put(8 * ncw), ocs = put(8 * ncs), ofew = put(ncw), ofes = put(ncs);
+  size_t ocaw = 0, ocas = 0, osgw = 0, osgs = 0;        // per-corridor lists: offsets and winners' assignments
+  if (as) { ocaw = put(4 * (size_t)(P + 1)); ocas = put(4 * (size_t)(P + 1)); osgw = put((size_t)P * Nw); osgs = put((size_t)P * Ns); }
   const size_t out_bytes = o;
   FQ_CUDA(ctx->h_in.reserve(in_bytes));
   FQ_CUDA(ctx->d_pair_io.reserve(in_bytes + out_bytes));
@@ -245,7 +357,12 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   // a NULL cost/flag output still needs a device array of its own kind: the chain allocates it in its scratch
   if ((d.feasible_whole == nullptr) != (d.cost_whole == nullptr) || (d.feasible_safe == nullptr) != (d.cost_safe == nullptr))
     return fq_fail(ctx, FQ_E_ARG, "feasible_* and cost_* must be given (or omitted) together");
-  int rc = fq_replan_pairs_dev(ctx, &d, nullptr, st);
+  if (as)
+  {
+    da.cand_ofs_whole = as->cand_ofs_whole ? (int*)(dout + ocaw) : nullptr; da.cand_ofs_safe = as->cand_ofs_safe ? (int*)(dout + ocas) : nullptr;
+    da.sigma_whole = as->sigma_whole ? (uint8_t*)(dout + osgw) : nullptr;  da.sigma_safe = as->sigma_safe ? (uint8_t*)(dout + osgs) : nullptr;
+  }
+  int rc = as ? fq_replan_pairs_assign_dev(ctx, &d, &da, nullptr, st) : fq_replan_pairs_dev(ctx, &d, nullptr, st);
   if (rc) return rc;
   // ---- results straight into the caller's arrays (asynchronous when they are pinned)
   if (d_results) *d_results = (fq_pair_result*)(dout + ores);
@@ -262,6 +379,13 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
     FQ_CUDA(cudaMemcpyAsync(a->cost_safe, dout + ocs, 8 * ncs, cudaMemcpyDeviceToHost, st));
     FQ_CUDA(cudaMemcpyAsync(a->feasible_safe, dout + ofes, ncs, cudaMemcpyDeviceToHost, st));
   }
+  if (as)
+  {
+    if (as->cand_ofs_whole) FQ_CUDA(cudaMemcpyAsync(as->cand_ofs_whole, dout + ocaw, 4 * (size_t)(P + 1), cudaMemcpyDeviceToHost, st));
+    if (as->cand_ofs_safe) FQ_CUDA(cudaMemcpyAsync(as->cand_ofs_safe, dout + ocas, 4 * (size_t)(P + 1), cudaMemcpyDeviceToHost, st));
+    if (as->sigma_whole) FQ_CUDA(cudaMemcpyAsync(as->sigma_whole, dout + osgw, (size_t)P * Nw, cudaMemcpyDeviceToHost, st));
+    if (as->sigma_safe) FQ_CUDA(cudaMemcpyAsync(as->sigma_safe, dout + osgs, (size_t)P * Ns, cudaMemcpyDeviceToHost, st));
+  }
   if (deferred) { ctx->pending = true; return 0; }
   FQ_CUDA(cudaStreamSynchronize(st));
   return 0;
@@ -276,4 +400,19 @@ extern "C" int fq_replan_pairs_async(fq_ctx* ctx, const fq_pair_args* a)
 {
   if (ctx && (ctx->is_group || ctx->comm)) return fq_replan_pairs_sharded(ctx, a, true);
   return fq_replan_pairs_host_ex(ctx, a, true, nullptr, true);
+}
+
+extern "C" int fq_replan_pairs_assign(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
+  if (ctx->is_group || ctx->comm) return fq_replan_pairs_sharded(ctx, a, false, as);
+  return fq_replan_pairs_host_ex(ctx, a, false, nullptr, true, as);
+}
+extern "C" int fq_replan_pairs_assign_async(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
+  if (ctx->is_group || ctx->comm) return fq_replan_pairs_sharded(ctx, a, true, as);
+  return fq_replan_pairs_host_ex(ctx, a, true, nullptr, true, as);
 }

@@ -46,7 +46,8 @@ extern "C" {
 typedef struct fq_ctx fq_ctx;     /* opaque: device, stream, plan tables, scratch             */
 
 int fq_abi_version(void);
-/* 1 if this build has the named feature: "sweep_early_exit", "replan_pairs", "multi_gpu", "row_tol", "certificates". */
+/* 1 if this build has the named feature: "sweep_early_exit", "replan_pairs", "multi_gpu", "row_tol", "certificates",
+ * "replan_pairs_assign". */
 int fq_has_feature(const char* name);
 
 /* Threading: a context is used from one thread at a time, like a SolverGurobi instance in the reference (one replan
@@ -235,6 +236,53 @@ int fq_replan_pairs_async(fq_ctx* ctx, const fq_pair_args* args);
  * `results_all` != NULL the chain ends with the path's one collective: an all-gather of the n_prob result records of
  * every rank into results_all[world x n_prob] (device). */
 int fq_replan_pairs_dev(fq_ctx* ctx, const fq_pair_args* args, fq_pair_result* results_all, void* stream);
+
+/* ---- chained replan with a per-corridor assignment list -------------------------------------------------------------
+ *
+ * Corridors of one batch need not have the same polytope count: Faster::replan trims the JPS paths to at most max_poly + 1
+ * vertices (deleteVertexes, faster.cpp:393,:495) and every segment becomes one polytope, so near the goal or at the first
+ * unknown cell a corridor has fewer.  The entry points below give every corridor j of a sweep with N segments its OWN list
+ * L(N, P_j, all_limit), P_j = its polytope count, generated on the device (nothing is enumerated on the host):
+ *   P_j = 0                   the single all-zero assignment
+ *   P_j^N <= all_limit        all P_j^N assignments, lexicographic with segment 0 most significant (base-P_j digits)
+ *   otherwise                 the non-decreasing assignments in the order of fq_monotone_sigmas, C(N + P_j - 1, N)
+ * all_limit = 0: always non-decreasing.  all_limit = 4096 with N = 6, P <= 3 (729 assignments) enumerates every assignment
+ * and so returns the exact MIQP optimum over the factors, as SolverGurobi's AUTO mode does.
+ *
+ * Corridor j's candidates are n_fac x |L_j|, factor-major (index f * |L_j| + s), at cand_ofs[j] .. cand_ofs[j+1]-1 of the
+ * per-candidate outputs (feasible_* / cost_*).  The selection is fq_replan_pairs's; the result records' *_sigma_index is
+ * the index in the corridor's own list.  fq_pair_args is used as for fq_replan_pairs except that sigmas_* must be NULL and
+ * n_sig_* 0 (FQ_E_ARG otherwise: a caller must not believe that a shared list was used).  FQ_E_ARG also for all_limit < 0,
+ * a corridor list longer than 2^20 and more than 2^30 candidates in a sweep. */
+typedef struct fq_pair_assign
+{
+  long all_limit;                          /* rule above                                                             */
+  int max_poly_whole, max_poly_safe;       /* _dev only: largest polytope count of one corridor (hint)               */
+  long n_cand_whole, n_cand_safe;          /* _dev only: total candidates of each sweep (hint, checked)              */
+  int* cand_ofs_whole;                     /* out, n_prob + 1: candidate offsets of the whole sweep, or NULL         */
+  int* cand_ofs_safe;                      /* out, n_prob + 1, or NULL                                               */
+  uint8_t* sigma_whole;                    /* out, n_prob x N_whole: the whole winners' assignments (0s: none), or NULL */
+  uint8_t* sigma_safe;                     /* out, n_prob x N_safe, or NULL                                          */
+} fq_pair_assign;
+
+/* |L(N, P, all_limit)|: candidates per factor of a corridor with P polytopes.  < 0 (FQ_E_ARG) if N is not in 1..FQ_MAX_N,
+ * P not in 0..FQ_MAX_POLY, all_limit < 0 or the list is longer than 2^20.  Pure host code. */
+long fq_pair_assign_count(int N, int P, long all_limit);
+/* HOST pointers everywhere; blocks until every output is in the caller's arrays.  On a multi-GPU context the corridors
+ * are sharded by candidate count, whole + safe (fq_shard_range over the summed per-corridor offsets, which the host knows
+ * from poly_ofs): the shards balance the work, not the corridor count.  DESIGN.md section 6. */
+int fq_replan_pairs_assign(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign);
+/* The same, returning once everything is enqueued; outputs are valid after fq_wait(ctx).  Arrays must stay alive. */
+int fq_replan_pairs_assign_async(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign);
+/* DEVICE pointers everywhere (both structs live on the host), as fq_replan_pairs_dev.  The library cannot read poly_ofs, so
+ * the caller passes max_poly_* (largest polytope count of one corridor) and n_cand_* (the sweeps' total candidates:
+ * n_fac_* x the sum of |L_j|; the per-candidate outputs hold that many).  The device computes the offsets and checks them:
+ * if a corridor has more polytopes than max_poly_* or the total is not n_cand_*, that sweep gets NO candidates -- every
+ * cand_ofs entry of it is 0, nothing is written to its per-candidate outputs, and every corridor's winner of that sweep is
+ * "none" (indices -1; a corridor without a whole winner has no safe winner either).  The call itself still returns 0: it
+ * does not synchronise.  Refused up front (FQ_E_ARG): max_poly_* outside 0..FQ_MAX_POLY, n_cand_* outside 0..2^30. */
+int fq_replan_pairs_assign_dev(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, fq_pair_result* results_all,
+                               void* stream);
 
 /* ---- several GPUs behind the boundary (SURVEY.md 8b/8e) ---------------------------------------------------------
  *
