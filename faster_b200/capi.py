@@ -15,7 +15,8 @@ EXPORTS = ["fq_abi_version", "fq_create", "fq_destroy", "fq_last_error", "fq_set
            "fq_monotone_sigmas", "fq_plan_tables", "fq_ellipsoid_decomp", "fq_jps3d_plan", "fq_jps3d_plan_world", "fq_jps3d_rules",
            "fq_replan_pairs", "fq_replan_pairs_async", "fq_replan_pairs_dev", "fq_create_multi", "fq_comm_unique_id", "fq_comm_init",
            "fq_comm_info", "fq_allgather_dev", "fq_shard_range", "fq_solve_multi_sharded", "fq_solve_batch_cert", "fq_has_feature",
-           "fq_pair_assign_count", "fq_replan_pairs_assign", "fq_replan_pairs_assign_async", "fq_replan_pairs_assign_dev"]
+           "fq_pair_assign_count", "fq_replan_pairs_assign", "fq_replan_pairs_assign_async", "fq_replan_pairs_assign_dev",
+           "fq_pair_window_factors", "fq_replan_pairs_window", "fq_replan_pairs_window_async", "fq_replan_pairs_window_dev"]
 
 
 class FqError(RuntimeError):
@@ -57,6 +58,21 @@ class PairAssign(C.Structure):
     _fields_ = [("all_limit", C.c_long), ("max_poly_whole", C.c_int), ("max_poly_safe", C.c_int), ("n_cand_whole", C.c_long),
                 ("n_cand_safe", C.c_long), ("cand_ofs_whole", C.c_void_p), ("cand_ofs_safe", C.c_void_p),
                 ("sigma_whole", C.c_void_p), ("sigma_safe", C.c_void_p)]
+
+
+class PairWindow(C.Structure):
+    """fq_pair_window of include/faster_b200.h: per-corridor time-allocation windows of the chained replan."""
+    _fields_ = [("init_whole", C.c_void_p), ("final_whole", C.c_void_p), ("init_safe", C.c_void_p), ("final_safe", C.c_void_p),
+                ("inc_whole", C.c_double), ("inc_safe", C.c_double), ("gamma_whole", C.c_double), ("gammap_whole", C.c_double),
+                ("gamma_safe", C.c_double), ("gammap_safe", C.c_double), ("max_fac_whole", C.c_int), ("max_fac_safe", C.c_int),
+                ("factor_whole", C.c_void_p), ("factor_safe", C.c_void_p), ("trials_whole", C.c_void_p), ("trials_safe", C.c_void_p),
+                ("next_init_whole", C.c_void_p), ("next_final_whole", C.c_void_p), ("next_init_safe", C.c_void_p),
+                ("next_final_safe", C.c_void_p)]
+
+
+WINDOW_IN_KEYS = ["init_whole", "final_whole", "init_safe", "final_safe"]
+WINDOW_OUT_KEYS = ["factor_whole", "factor_safe", "trials_whole", "trials_safe", "next_init_whole", "next_final_whole",
+                   "next_init_safe", "next_final_safe"]
 
 
 def lib():
@@ -103,6 +119,12 @@ def lib():
         L.fq_replan_pairs_assign.argtypes = [C.c_void_p, C.POINTER(PairArgs), C.POINTER(PairAssign)]
         L.fq_replan_pairs_assign_async.argtypes = L.fq_replan_pairs_assign.argtypes
         L.fq_replan_pairs_assign_dev.argtypes = [C.c_void_p, C.POINTER(PairArgs), C.POINTER(PairAssign), C.c_void_p, C.c_void_p]
+        L.fq_pair_window_factors.restype = C.c_long
+        L.fq_pair_window_factors.argtypes = [C.c_double, C.c_double, C.c_double, C.c_void_p, C.c_long]
+        L.fq_replan_pairs_window.argtypes = [C.c_void_p, C.POINTER(PairArgs), C.POINTER(PairAssign), C.POINTER(PairWindow)]
+        L.fq_replan_pairs_window_async.argtypes = L.fq_replan_pairs_window.argtypes
+        L.fq_replan_pairs_window_dev.argtypes = [C.c_void_p, C.POINTER(PairArgs), C.POINTER(PairAssign), C.POINTER(PairWindow),
+                                                 C.c_void_p, C.c_void_p]
         L.fq_create_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_void_p]
         L.fq_comm_unique_id.argtypes = [C.c_void_p]
         L.fq_comm_init.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
@@ -168,6 +190,43 @@ def assign_offsets(poly_ofs, N, n_fac, all_limit=0):
     if min(counts, default=0) < 0:
         raise FqError("assignment list of a corridor refused (longer than 2^20)")
     return np.concatenate([[0], np.cumsum(np.asarray(counts, np.int64) * int(n_fac))]).astype(np.int32)
+
+
+def window_factors(fi, ff, inc):
+    """fq_pair_window_factors: the factors genNewTraj's loop visits for the window (fi, ff, inc), as float64; raises
+    FqError when the window is refused."""
+    L = lib()
+    n = L.fq_pair_window_factors(float(fi), float(ff), float(inc), None, 0)
+    if n < 0:
+        raise FqError("time-allocation window refused: (%r, %r, %r)" % (fi, ff, inc))
+    out = np.zeros(n)
+    L.fq_pair_window_factors(float(fi), float(ff), float(inc), out.ctypes.data, n)
+    return out
+
+
+def window_offsets(poly_ofs, N, n_fac, all_limit=0):
+    """Candidate offsets (n_prob + 1) of one sweep with per-corridor lists and per-corridor factor counts n_fac[j]."""
+    counts = [assign_count(N, int(poly_ofs[j + 1] - poly_ofs[j]), all_limit) for j in range(len(poly_ofs) - 1)]
+    if min(counts, default=0) < 0:
+        raise FqError("assignment list of a corridor refused (longer than 2^20)")
+    return np.concatenate([[0], np.cumsum(np.asarray(counts, np.int64) * np.asarray(n_fac, np.int64))]).astype(np.int32)
+
+
+def window_args(win, out_ptrs, inc=1.0, gamma=20.0, max_fac_whole=0, max_fac_safe=0):
+    """PairWindow; win(key) -> address of the window input `key` (WINDOW_IN_KEYS), out_ptrs: addresses of WINDOW_OUT_KEYS
+    (0/None/missing = NULL).  inc: one value or (whole, safe); gamma: one value or (gamma_whole, gammap_whole, gamma_safe,
+    gammap_safe).  The max_fac_* hints matter for the _dev entry only."""
+    inc = (inc, inc) if np.isscalar(inc) else tuple(inc)
+    gamma = (gamma,) * 4 if np.isscalar(gamma) else tuple(gamma)
+    s = PairWindow()
+    for k in WINDOW_IN_KEYS:
+        setattr(s, k, win(k))
+    s.inc_whole, s.inc_safe = float(inc[0]), float(inc[1])
+    s.gamma_whole, s.gammap_whole, s.gamma_safe, s.gammap_safe = (float(g) for g in gamma)
+    s.max_fac_whole, s.max_fac_safe = int(max_fac_whole), int(max_fac_safe)
+    for k in WINDOW_OUT_KEYS:
+        setattr(s, k, out_ptrs.get(k) or None)
+    return s
 
 
 def ellipsoid_decomp(path, obs, bbox=(2.0, 2.0, 1.0), inflate=0.42, z_ground=0.0, cap_rows=4096):
@@ -410,6 +469,43 @@ class Solver:
         fn = self._L.fq_replan_pairs_assign_async if deferred else self._L.fq_replan_pairs_assign
         self._check(fn(self._h, C.byref(a), C.byref(s)))
         return out
+
+    def replan_pairs_window(self, w, windows, all_limit=0, inc=1.0, gamma=20.0, want_candidates=True, want_coeffs=True, deferred=False):
+        """fq_replan_pairs_window on a make_pair_workload dict (host arrays; its factors_* and sigmas_* are not used: corridor
+        j sweeps its own window F_j and list L_j).  windows: dict of n_prob-arrays init_whole, final_whole, init_safe,
+        final_safe; inc / gamma as window_args.  -> the dict of replan_pairs_assign plus factor_*, trials_* and the next
+        windows next_init_* / next_final_*.  deferred: valid after wait()."""
+        n = w["n_prob"]
+        wins = {k: np.ascontiguousarray(windows[k], np.float64) for k in WINDOW_IN_KEYS}
+        incs = (inc, inc) if np.isscalar(inc) else tuple(inc)
+        offs = {}
+        for kind, ik in (("whole", incs[0]), ("safe", incs[1])):
+            nf = [len(window_factors(a, b, ik)) for a, b in zip(wins["init_" + kind], wins["final_" + kind])]
+            offs[kind] = window_offsets(w["poly_ofs_" + kind], w["N_" + kind], nf, all_limit)
+        out = dict(results=np.zeros(n, PAIR_RESULT_DTYPE), cand_ofs_whole=np.zeros(n + 1, np.int32), cand_ofs_safe=np.zeros(n + 1, np.int32),
+                   sigma_whole=np.zeros((n, w["N_whole"]), np.uint8), sigma_safe=np.zeros((n, w["N_safe"]), np.uint8),
+                   factor_whole=np.zeros(n), factor_safe=np.zeros(n), trials_whole=np.zeros(n, np.int32), trials_safe=np.zeros(n, np.int32),
+                   next_init_whole=np.zeros(n), next_final_whole=np.zeros(n), next_init_safe=np.zeros(n), next_final_safe=np.zeros(n))
+        if want_candidates:
+            ncw, ncs = int(offs["whole"][-1]), int(offs["safe"][-1])
+            out.update(feasible_whole=np.zeros(ncw, np.uint8), cost_whole=np.zeros(ncw), feasible_safe=np.zeros(ncs, np.uint8),
+                       cost_safe=np.zeros(ncs))
+        if want_coeffs:
+            out.update(coeffs_whole=np.zeros((n, w["N_whole"], 12)), coeffs_safe=np.zeros((n, w["N_safe"], 12)))
+        a = pair_args(w, lambda k: None if k.startswith(("sigmas_", "factors_")) else w[k].ctypes.data,
+                      {k: v.ctypes.data for k, v in out.items()})
+        a.n_sig_whole = a.n_sig_safe = a.n_fac_whole = a.n_fac_safe = 0
+        s = assign_args(all_limit, {k: out[k].ctypes.data for k in ("cand_ofs_whole", "cand_ofs_safe", "sigma_whole", "sigma_safe")})
+        wa = window_args(lambda k: wins[k].ctypes.data, {k: out[k].ctypes.data for k in WINDOW_OUT_KEYS}, inc, gamma)
+        fn = self._L.fq_replan_pairs_window_async if deferred else self._L.fq_replan_pairs_window
+        self._check(fn(self._h, C.byref(a), C.byref(s), C.byref(wa)))
+        return out
+
+    def replan_pairs_window_dev(self, a, s, win, results_all=0, stream=0):
+        """fq_replan_pairs_window_dev: `a` (PairArgs), `s` (PairAssign) and `win` (PairWindow) hold device addresses and the
+        host hints (s.n_cand_* is a capacity here, win.max_fac_* bounds every |F_j|)."""
+        self._check(self._L.fq_replan_pairs_window_dev(self._h, C.byref(a), C.byref(s), C.byref(win), results_all or None,
+                                                       stream or None))
 
     def replan_pairs_assign_dev(self, a, s, results_all=0, stream=0):
         """fq_replan_pairs_assign_dev: `a` (PairArgs) and `s` (PairAssign) hold device addresses and the host hints."""

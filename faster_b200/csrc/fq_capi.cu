@@ -143,7 +143,7 @@ extern "C" int fq_has_feature(const char* name)
   if (!name) return 0;
   const std::string n(name);
   if (n == "sweep_early_exit" || n == "replan_pairs" || n == "multi_gpu" || n == "row_tol" || n == "certificates" ||
-      n == "replan_pairs_assign")
+      n == "replan_pairs_assign" || n == "replan_pairs_window")
     return 1;
   return 0;
 }

@@ -116,13 +116,15 @@ int fq_solve_multi_host_ex(fq_ctx* ctx, int N, int force_final, int n_prob, cons
                            int** d_win_idx, double** d_win_cost);
 // fq_pair_capi.cu.  d_results (may be NULL): receives the device address of the result records; copy_results = false
 // leaves the caller's `results` array untouched (the multi-GPU path reads the all-gathered table instead).  as != NULL:
-// per-corridor assignment lists (fq_replan_pairs_assign*, host pointers)
+// per-corridor assignment lists (fq_replan_pairs_assign*, host pointers); win != NULL (with as): per-corridor windows
+// (fq_replan_pairs_window*, host pointers)
 int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results,
-                            const fq_pair_assign* as = nullptr);
+                            const fq_pair_assign* as = nullptr, const fq_pair_window* win = nullptr);
 // fq_multi.cu
 void fq_comm_release(fq_ctx* ctx);
 // all-gather on one context's communicator (one process per GPU): `bytes` from every rank, rank order
 int fq_comm_allgather(fq_ctx* ctx, const void* d_send, void* d_recv, size_t bytes, cudaStream_t stream);
 // fq_replan_pairs on a multi-GPU context (a group or a rank of a communicator)
-// (as != NULL: fq_replan_pairs_assign*, shards balanced by candidate count)
-int fq_replan_pairs_sharded(fq_ctx* g, const fq_pair_args* a, bool deferred, const fq_pair_assign* as = nullptr);
+// (as != NULL: fq_replan_pairs_assign*, shards balanced by candidate count; win != NULL as well: fq_replan_pairs_window*)
+int fq_replan_pairs_sharded(fq_ctx* g, const fq_pair_args* a, bool deferred, const fq_pair_assign* as = nullptr,
+                            const fq_pair_window* win = nullptr);

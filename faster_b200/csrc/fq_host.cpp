@@ -2,6 +2,7 @@
 #include "fq_plan.h"
 #include "fq_dtinit.h"
 #include "fq_assign.h"
+#include "fq_window.h"
 #include "../../include/faster_b200.h"
 
 #include <algorithm>
@@ -194,6 +195,12 @@ extern "C" long fq_pair_assign_count(int N, int P, long all_limit)
   if (N < 1 || N > FQ_MAX_N || P < 0 || P > FQ_MAX_POLY || all_limit < 0) return FQ_E_ARG;
   const long long n = fqa::list_len(N, P, all_limit);
   return n < 0 ? FQ_E_ARG : (long)n;
+}
+
+extern "C" long fq_pair_window_factors(double fi, double ff, double inc, double* out, long cap)
+{
+  const int n = fqw::factors(fi, ff, inc, out, (int)std::max(0L, std::min(cap, (long)fqw::kMaxFactors)));
+  return n < 0 ? FQ_E_ARG : n;
 }
 
 extern "C" int fq_abi_version(void) { return FQ_ABI_VERSION; }

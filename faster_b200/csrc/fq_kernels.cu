@@ -671,6 +671,39 @@ cudaError_t fq_launch_expand_assign(int n_prob, int N, int n_fac, long long all_
   return cudaGetLastError();
 }
 
+cudaError_t fq_launch_window_factors(int n_prob, int max_fac, const double* init, const double* final_, double inc, double* fac,
+                                     int* n_fac_j, cudaStream_t stream)
+{
+  if (n_prob <= 0) return cudaSuccess;
+  fqp::fq_window_factors_kernel<<<(n_prob + 63) / 64, 64, 0, stream>>>(n_prob, max_fac, init, final_, inc, fac, n_fac_j);
+  return cudaGetLastError();
+}
+
+cudaError_t fq_launch_window_offsets(int n_prob, int N, int max_fac, long long all_limit, int max_poly, long long cap,
+                                     const int* poly_ofs, const int* n_fac_j, int* cand_ofs, cudaStream_t stream)
+{
+  if (n_prob <= 0) return cudaSuccess;
+  fqp::fq_assign_offsets_kernel<<<1, 1024, 0, stream>>>(n_prob, N, max_fac, all_limit, max_poly, cap, poly_ofs, cand_ofs, n_fac_j);
+  return cudaGetLastError();
+}
+
+cudaError_t fq_launch_expand_window(int n_prob, int N, int max_fac, long long all_limit, const double* fac, const int* n_fac_j,
+                                    const double* dt_base, const int* poly_ofs, const int* cand_ofs, double* dt, uint8_t* sigma,
+                                    cudaStream_t stream)
+{
+  if (n_prob <= 0) return cudaSuccess;
+  fqp::fq_expand_assign_kernel<<<n_prob, 256, 0, stream>>>(n_prob, N, max_fac, all_limit, fac, dt_base, poly_ofs, cand_ofs, dt, sigma,
+                                                           n_fac_j);
+  return cudaGetLastError();
+}
+
+cudaError_t fq_launch_pair_window(const FqPairWindowArgs& a, cudaStream_t stream)
+{
+  if (a.n_prob <= 0) return cudaSuccess;
+  fqp::fq_pair_window_kernel<<<(a.n_prob + 127) / 128, 128, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+
 cudaError_t fq_launch_select_multi(const FqSelectMultiArgs& a, cudaStream_t stream)
 {
   if (a.n_prob <= 0) return cudaSuccess;

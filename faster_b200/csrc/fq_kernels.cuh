@@ -163,6 +163,24 @@ struct FqPairFinalArgs
   const uint8_t* win_sig_s = nullptr;
   uint8_t* sigma_out_w = nullptr;
   uint8_t* sigma_out_s = nullptr;
+  // per-corridor windows (fq_replan_pairs_window*): corridor j's factor count, which then replaces n_fac_* in the split
+  const int* n_fac_j_w = nullptr;
+  const int* n_fac_j_s = nullptr;
+};
+
+// factor_*, trials_* and the next windows of fq_replan_pairs_window* (fq_window.h), from the result records
+struct FqPairWindowArgs
+{
+  int n_prob, max_fac_w, max_fac_s;
+  const fq_pair_result* rec;            // n_prob records of the chain
+  const int *cand_ofs_w, *cand_ofs_s;   // n_prob + 1 each (all 0: the sweep was emptied)
+  const int *n_fac_w, *n_fac_s;         // n_prob: |F_j| (-1 refused)
+  const double *fac_w, *fac_s;          // n_prob x max_fac_*: F_j
+  const double *init_w, *final_w, *init_s, *final_s;
+  double gamma_w, gammap_w, gamma_s, gammap_s;
+  double *factor_w, *factor_s;          // out, or NULL
+  int *trials_w, *trials_s;             // out, or NULL
+  double *next_init_w, *next_final_w, *next_init_s, *next_final_s;   // out, or NULL; may alias init_* / final_*
 };
 
 cudaError_t fq_launch_dtbase(int n_prob, int N, double DC, const double* x0, const double* xf, const double* lim,
@@ -175,6 +193,16 @@ cudaError_t fq_launch_assign_offsets(int n_prob, int N, int n_fac, long long all
                                      const int* poly_ofs, int* cand_ofs, cudaStream_t stream);
 cudaError_t fq_launch_expand_assign(int n_prob, int N, int n_fac, long long all_limit, const double* factors, const double* dt_base,
                                     const int* poly_ofs, const int* cand_ofs, double* dt, uint8_t* sigma, cudaStream_t stream);
+// per-corridor windows (fq_window.h): F_j into rows of max_fac factors and |F_j| (-1 refused); the offsets and the
+// expansion with those rows and counts (n_fac = max_fac; the total must be at most n_cand); the records' window outputs
+cudaError_t fq_launch_window_factors(int n_prob, int max_fac, const double* init, const double* final_, double inc, double* fac,
+                                     int* n_fac_j, cudaStream_t stream);
+cudaError_t fq_launch_window_offsets(int n_prob, int N, int max_fac, long long all_limit, int max_poly, long long cap,
+                                     const int* poly_ofs, const int* n_fac_j, int* cand_ofs, cudaStream_t stream);
+cudaError_t fq_launch_expand_window(int n_prob, int N, int max_fac, long long all_limit, const double* fac, const int* n_fac_j,
+                                    const double* dt_base, const int* poly_ofs, const int* cand_ofs, double* dt, uint8_t* sigma,
+                                    cudaStream_t stream);
+cudaError_t fq_launch_pair_window(const FqPairWindowArgs& a, cudaStream_t stream);
 cudaError_t fq_launch_select_multi(const FqSelectMultiArgs& a, cudaStream_t stream);
 cudaError_t fq_launch_pair_mid(const FqPairMidArgs& a, cudaStream_t stream);
 cudaError_t fq_launch_pair_final(const FqPairFinalArgs& a, cudaStream_t stream);

@@ -8,6 +8,7 @@
 // on it and single-GPU use needs no NCCL at all.
 #include "fq_assign.h"
 #include "fq_ctx.h"
+#include "fq_window.h"
 
 #include <algorithm>
 #include <cstdlib>
@@ -269,7 +270,9 @@ int exchange(fq_ctx* g, const std::vector<T*>& send, const std::vector<T*>& recv
 // Per-corridor assignment lists (as != NULL): the corridors' candidate counts differ, so the shards are balanced by
 // candidates -- fq_shard_range over the offsets of whole + safe candidates, computed here from poly_ofs -- and each shard's
 // per-candidate outputs start at the shard's first offset.  The caller's cand_ofs_* come from the same host offsets.
-int fq_replan_pairs_sharded(fq_ctx* g, const fq_pair_args* a, bool deferred, const fq_pair_assign* as)
+// Per-corridor windows (win != NULL, with as): corridor j has |F_j| factors (fq_window.h) instead of n_fac_*, and every
+// shard gets its rows of the window arrays.
+int fq_replan_pairs_sharded(fq_ctx* g, const fq_pair_args* a, bool deferred, const fq_pair_assign* as, const fq_pair_window* win)
 {
   fq_ctx* ctx = g;
   if (!a || a->n_prob <= 0 || !a->results) return fq_fail(g, FQ_E_ARG, "bad arguments");
@@ -278,7 +281,9 @@ int fq_replan_pairs_sharded(fq_ctx* g, const fq_pair_args* a, bool deferred, con
   if (!a->x0 || !a->xf_whole || !a->xf_safe || !a->lim || !a->poly_ofs_whole || !a->face_ofs_whole || !a->poly_ofs_safe ||
       !a->face_ofs_safe)
     return fq_fail(g, FQ_E_ARG, "NULL argument");
-  if (a->n_fac_whole <= 0 || a->n_fac_safe <= 0 || (!as && (a->n_sig_whole <= 0 || a->n_sig_safe <= 0)))
+  if (win && (!win->init_whole || !win->final_whole || !win->init_safe || !win->final_safe))
+    return fq_fail(g, FQ_E_ARG, "window arrays must not be NULL");
+  if (!win && (a->n_fac_whole <= 0 || a->n_fac_safe <= 0 || (!as && (a->n_sig_whole <= 0 || a->n_sig_safe <= 0))))
     return fq_fail(g, FQ_E_ARG, "empty factor / assignment grid");
   if (as && (a->sigmas_whole || a->sigmas_safe || a->n_sig_whole != 0 || a->n_sig_safe != 0))
     return fq_fail(g, FQ_E_ARG, "per-corridor assignment lists: sigmas_* must be NULL and n_sig_* 0");
@@ -303,8 +308,15 @@ int fq_replan_pairs_sharded(fq_ctx* g, const fq_pair_args* a, bool deferred, con
       if (pw > FQ_MAX_POLY || ps > FQ_MAX_POLY) return fq_fail(g, FQ_E_ARG, "more than FQ_MAX_POLY polytopes in a corridor");
       const long long lw = fqa::list_len(a->N_whole, pw, as->all_limit), ls = fqa::list_len(a->N_safe, ps, as->all_limit);
       if (lw < 0 || ls < 0) return fq_fail(g, FQ_E_ARG, "assignment list of a corridor longer than 2^20");
-      ofw[j + 1] = ofw[j] + lw * a->n_fac_whole;
-      ofs[j + 1] = ofs[j] + ls * a->n_fac_safe;
+      int nfw = a->n_fac_whole, nfs = a->n_fac_safe;
+      if (win)
+      {
+        nfw = fqw::factors(win->init_whole[j], win->final_whole[j], win->inc_whole, nullptr, 0);
+        nfs = fqw::factors(win->init_safe[j], win->final_safe[j], win->inc_safe, nullptr, 0);
+        if (nfw < 0 || nfs < 0) return fq_fail(g, FQ_E_ARG, "time-allocation window refused (not finite, init <= 0, more than 4096 factors or a stalled accumulation)");
+      }
+      ofw[j + 1] = ofw[j] + lw * nfw;
+      ofs[j + 1] = ofs[j] + ls * nfs;
       if (ofw[j + 1] > (1LL << 30) || ofs[j + 1] > (1LL << 30)) return fq_fail(g, FQ_E_ARG, "too many candidates");
       ofb[j + 1] = (int)std::min<long long>(ofw[j + 1] + ofs[j + 1], 0x7fffffffLL);
     }
@@ -361,8 +373,21 @@ int fq_replan_pairs_sharded(fq_ctx* g, const fq_pair_args* a, bool deferred, con
       sa.sigma_whole = as->sigma_whole ? as->sigma_whole + (size_t)a->N_whole * lo[r] : nullptr;
       sa.sigma_safe = as->sigma_safe ? as->sigma_safe + (size_t)a->N_safe * lo[r] : nullptr;
     }
+    fq_pair_window sw{};
+    if (win)
+    { // the shard's rows of every window array
+      const size_t o = (size_t)lo[r];
+      auto in = [o](const double* p) { return p + o; };
+      auto out = [o](auto* p) { return p ? p + o : p; };
+      sw = *win;
+      sw.init_whole = in(win->init_whole); sw.final_whole = in(win->final_whole); sw.init_safe = in(win->init_safe); sw.final_safe = in(win->final_safe);
+      sw.factor_whole = out(win->factor_whole); sw.factor_safe = out(win->factor_safe);
+      sw.trials_whole = out(win->trials_whole); sw.trials_safe = out(win->trials_safe);
+      sw.next_init_whole = out(win->next_init_whole); sw.next_final_whole = out(win->next_final_whole);
+      sw.next_init_safe = out(win->next_init_safe); sw.next_final_safe = out(win->next_final_safe);
+    }
     fq_pair_result* dr = nullptr;
-    int rc = fq_replan_pairs_host_ex(c, &s, true, &dr, false, as ? &sa : nullptr);
+    int rc = fq_replan_pairs_host_ex(c, &s, true, &dr, false, as ? &sa : nullptr, win ? &sw : nullptr);
     if (rc) { if (c != g) g->err = c->err; return rc; }
     e = cudaMemcpyAsync(d_res[i], dr, sizeof(fq_pair_result) * (size_t)n, cudaMemcpyDeviceToDevice, c->stream);
     if (e != cudaSuccess) return fq_cuda_fail(g, e, "gather staging");

@@ -6,6 +6,7 @@
 #pragma once
 #include "fq_assign.h"
 #include "fq_dtinit.h"
+#include "fq_window.h"
 
 namespace fqp
 {
@@ -55,13 +56,27 @@ __global__ void fq_expand_grid_kernel(int n_prob, int N, int n_fac, int n_sig, c
 
 // ---- per-corridor assignment lists (fq_replan_pairs_assign*; the lists are defined in fq_assign.h)
 
+// per-corridor windows (fq_replan_pairs_window*, fq_window.h): one thread per corridor accumulates F_j = F(init[j],
+// final[j], inc) into row j of fac (its first max_fac factors) and writes |F_j|, or -1 when the window is refused.  A count
+// above max_fac makes fq_assign_offsets_kernel empty the sweep.
+__global__ void fq_window_factors_kernel(int n_prob, int max_fac, const double* __restrict__ init, const double* __restrict__ final_,
+                                         double inc, double* __restrict__ fac, int* __restrict__ n_fac_j)
+{
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n_prob) return;
+  n_fac_j[j] = fqw::factors(init[j], final_[j], inc, fac + (size_t)j * max_fac, max_fac);
+}
+
 // cand_ofs[0 .. n_prob] = exclusive scan of n_fac x |L(N, P_j, all_limit)|, P_j from poly_ofs.  One CTA (any size up to
 // 1024): every thread scans a contiguous run of corridors.  The sweep's buffers were sized for n_cand candidates; when a
 // corridor has more than max_poly polytopes, a list is refused (longer than 2^20) or the total is not n_cand, EVERY range
 // is left empty (cand_ofs all 0): no candidate is expanded or solved and every corridor's winner of the sweep is "none".
+// Per-corridor windows (n_fac_j != NULL): corridor j has n_fac_j[j] factors instead of n_fac, which then bounds them (a
+// refused window, -1, or more than n_fac factors also empties the sweep), and n_cand is a capacity: the total must not
+// exceed it.
 __global__ void __launch_bounds__(1024) fq_assign_offsets_kernel(int n_prob, int N, int n_fac, long long all_limit, int max_poly,
                                                                  long long n_cand, const int* __restrict__ poly_ofs,
-                                                                 int* __restrict__ cand_ofs)
+                                                                 int* __restrict__ cand_ofs, const int* __restrict__ n_fac_j = nullptr)
 {
   __shared__ long long s_run[1024];
   __shared__ long long s_total;
@@ -77,8 +92,9 @@ __global__ void __launch_bounds__(1024) fq_assign_offsets_kernel(int n_prob, int
   {
     const int P = poly_ofs[j + 1] - poly_ofs[j];
     const long long L = fqa::list_len(N, P, all_limit);
-    if (P < 0 || P > max_poly || L < 0) bad = true;
-    else sum += L * n_fac;
+    const int nf = n_fac_j ? n_fac_j[j] : n_fac;
+    if (P < 0 || P > max_poly || L < 0 || nf < 0 || nf > n_fac) bad = true;
+    else sum += L * nf;
   }
   if (bad) s_bad = 1;
   s_run[tid] = sum;
@@ -88,7 +104,7 @@ __global__ void __launch_bounds__(1024) fq_assign_offsets_kernel(int n_prob, int
     long long run = 0;
     for (int i = 0; i < T; i++) { const long long x = s_run[i]; s_run[i] = run; run += x; }
     s_total = run;
-    if (run != n_cand) s_bad = 1;
+    if (n_fac_j ? run > n_cand : run != n_cand) s_bad = 1;
   }
   __syncthreads();
   const bool empty = s_bad != 0;
@@ -96,18 +112,20 @@ __global__ void __launch_bounds__(1024) fq_assign_offsets_kernel(int n_prob, int
   for (int j = j0; j < j1; j++)
   {
     cand_ofs[j] = empty ? 0 : (int)run;
-    if (!empty) run += fqa::list_len(N, poly_ofs[j + 1] - poly_ofs[j], all_limit) * n_fac;
+    if (!empty) run += fqa::list_len(N, poly_ofs[j + 1] - poly_ofs[j], all_limit) * (n_fac_j ? n_fac_j[j] : n_fac);
   }
   if (tid == 0) cand_ofs[n_prob] = empty ? 0 : (int)s_total;
 }
 
 // candidates of corridor j = factors x L_j, factor-major: dt = factor * dt_base[j] (as fq_expand_grid_kernel), sigma =
 // the assignment's unranked index within L_j.  One CTA per corridor, grid-striding over its own candidates; the binomials
-// of the non-decreasing unranking sit in shared memory.
+// of the non-decreasing unranking sit in shared memory.  Per-corridor windows (n_fac_j != NULL): `factors` holds one row of
+// n_fac factors per corridor, of which corridor j uses the first n_fac_j[j].
 __global__ void __launch_bounds__(256) fq_expand_assign_kernel(int n_prob, int N, int n_fac, long long all_limit,
                                                                const double* __restrict__ factors, const double* __restrict__ dt_base,
                                                                const int* __restrict__ poly_ofs, const int* __restrict__ cand_ofs,
-                                                               double* __restrict__ dt, uint8_t* __restrict__ sigma)
+                                                               double* __restrict__ dt, uint8_t* __restrict__ sigma,
+                                                               const int* __restrict__ n_fac_j = nullptr)
 {
   __shared__ long long s_binom[48 * 17];
   for (int i = threadIdx.x; i < 48 * 17; i += blockDim.x) s_binom[i] = fqa::binom(i / 17, i % 17);
@@ -117,13 +135,15 @@ __global__ void __launch_bounds__(256) fq_expand_assign_kernel(int n_prob, int N
   const int c0 = cand_ofs[j], n = cand_ofs[j + 1] - c0;
   const int P = poly_ofs[j + 1] - poly_ofs[j];
   const long long L = fqa::list_len(N, P, all_limit);
-  if (n <= 0 || L <= 0 || (long long)n != L * n_fac) return;        // an emptied sweep (fq_assign_offsets_kernel)
+  const int nf = n_fac_j ? n_fac_j[j] : n_fac;
+  const double* fac = n_fac_j ? factors + (size_t)j * n_fac : factors;
+  if (n <= 0 || L <= 0 || (long long)n != L * nf) return;           // an emptied sweep (fq_assign_offsets_kernel)
   const bool all = fqa::use_all(N, P, all_limit);
   const double base = dt_base[j];
   for (int i = threadIdx.x; i < n; i += blockDim.x)
   {
     const int f = (int)(i / L);
-    dt[c0 + i] = FQ_MUL(factors[f], base);
+    dt[c0 + i] = FQ_MUL(fac[f], base);
     fqa::unrank(N, P, all, i - (long long)f * L, s_binom, sigma + (size_t)(c0 + i) * N);
   }
 }
@@ -229,13 +249,15 @@ __global__ void fq_pair_final_kernel(const FqPairFinalArgs a)
   if (j >= a.n_prob) return;
   fq_pair_result r;
   const int ww = a.win_idx_w[j], ws = a.win_idx_s[j];
-  // list lengths: shared (n_sig_*), or per corridor (its candidates / n_fac; a corridor without candidates has no winner)
-  const int lw = a.cand_ofs_w ? (a.cand_ofs_w[j + 1] - a.cand_ofs_w[j]) / a.n_fac_w : a.n_sig_w;
-  const int ls = a.cand_ofs_s ? (a.cand_ofs_s[j + 1] - a.cand_ofs_s[j]) / a.n_fac_s : a.n_sig_s;
-  r.whole_dt_index = ww >= 0 ? ww / lw : -1;
-  r.whole_sigma_index = ww >= 0 ? ww % lw : -1;
-  r.safe_dt_index = ws >= 0 ? ws / ls : -1;
-  r.safe_sigma_index = ws >= 0 ? ws % ls : -1;
+  // list lengths: shared (n_sig_*), or per corridor (its candidates / n_fac; a corridor without candidates has no winner).
+  // With per-corridor windows n_fac is the corridor's own |F_j|, which may be 0 (then so are its candidates).
+  const int nfw = a.n_fac_j_w ? a.n_fac_j_w[j] : a.n_fac_w, nfs = a.n_fac_j_s ? a.n_fac_j_s[j] : a.n_fac_s;
+  const int lw = a.cand_ofs_w ? (nfw > 0 ? (a.cand_ofs_w[j + 1] - a.cand_ofs_w[j]) / nfw : 0) : a.n_sig_w;
+  const int ls = a.cand_ofs_s ? (nfs > 0 ? (a.cand_ofs_s[j + 1] - a.cand_ofs_s[j]) / nfs : 0) : a.n_sig_s;
+  r.whole_dt_index = ww >= 0 && lw > 0 ? ww / lw : -1;
+  r.whole_sigma_index = ww >= 0 && lw > 0 ? ww % lw : -1;
+  r.safe_dt_index = ws >= 0 && ls > 0 ? ws / ls : -1;
+  r.safe_sigma_index = ws >= 0 && ls > 0 ? ws % ls : -1;
   if (a.sigma_out_w)
     for (int t = 0; t < a.N_w; t++) a.sigma_out_w[(size_t)j * a.N_w + t] = a.win_sig_w[(size_t)j * a.N_w + t];
   if (a.sigma_out_s)
@@ -246,5 +268,33 @@ __global__ void fq_pair_final_kernel(const FqPairFinalArgs a)
   r.n_samples_whole = a.n_samples[j]; r.k_safe = a.k_safe[j];
   for (int i = 0; i < 9; i++) r.R[i] = a.x0_safe[j * 9 + i];
   a.out[j] = r;
+}
+
+// factor_that_worked_, trials_ and the next windows of every corridor (fq_window.h), after fq_pair_final_kernel.  trials:
+// the winner's index in F_j + 1; |F_j| without a winner; 0 for a sweep that did not run (a safe sweep after a whole sweep
+// without winner, or a sweep the offsets kernel emptied).  Each thread reads its corridor's windows before it writes the
+// next ones, so those may alias.
+__global__ void fq_pair_window_kernel(const FqPairWindowArgs a)
+{
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= a.n_prob) return;
+  const double nan = __longlong_as_double(0x7ff8000000000000ll);
+  const int dw = a.rec[j].whole_dt_index, ds = a.rec[j].safe_dt_index;
+  const bool ran_w = a.cand_ofs_w[a.n_prob] > 0, ran_s = ran_w && dw >= 0 && a.cand_ofs_s[a.n_prob] > 0;
+  const double fw = dw >= 0 ? a.fac_w[(size_t)j * a.max_fac_w + dw] : nan;
+  const double fs = ds >= 0 ? a.fac_s[(size_t)j * a.max_fac_s + ds] : nan;
+  const double iw = a.init_w[j], ew = a.final_w[j], is = a.init_s[j], es = a.final_s[j];
+  if (a.factor_w) a.factor_w[j] = fw;
+  if (a.factor_s) a.factor_s[j] = fs;
+  if (a.trials_w) a.trials_w[j] = !ran_w ? 0 : (dw >= 0 ? dw + 1 : a.n_fac_w[j]);
+  if (a.trials_s) a.trials_s[j] = !ran_s ? 0 : (ds >= 0 ? ds + 1 : a.n_fac_s[j]);
+  const bool both = dw >= 0 && ds >= 0;
+  double ni, nf;
+  fqw::next_window(both, fw, a.gamma_w, a.gammap_w, iw, ew, &ni, &nf);
+  if (a.next_init_w) a.next_init_w[j] = ni;
+  if (a.next_final_w) a.next_final_w[j] = nf;
+  fqw::next_window(both, fs, a.gamma_s, a.gammap_s, is, es, &ni, &nf);
+  if (a.next_init_s) a.next_init_s[j] = ni;
+  if (a.next_final_s) a.next_final_s[j] = nf;
 }
 }  // namespace fqp

@@ -3,6 +3,7 @@
 // (safe).  Kernels: the batch solve (fq_kernels_t.cuh) and the small kernels of fq_pair.cuh.
 #include "fq_assign.h"
 #include "fq_ctx.h"
+#include "fq_window.h"
 
 #include <algorithm>
 #include <cmath>
@@ -16,6 +17,8 @@ struct Scratch
       *cost_w, *cost_s, *re_cost;
   uint8_t *sig_w, *sig_s, *win_sig_w, *win_sig_s, *feas_w, *feas_s, *re_feas;
   int *cand_ofs_w, *cand_ofs_s, *win_idx_w, *win_idx_s, *win_ofs, *n_samples, *k_safe;
+  double *fac_w, *fac_s;                // per-corridor windows: n_prob x max_fac factor rows
+  int *nf_w, *nf_s;                     // and |F_j| (-1: refused)
 };
 
 template <class T>
@@ -26,8 +29,9 @@ T* carve(char*& p, size_t count)
   return r;
 }
 
-// shared = false: per-corridor lists (fq_replan_pairs_assign*), whose candidate counts the callers check themselves
-int check_common(fq_ctx* ctx, const fq_pair_args* a, bool shared = true)
+// shared = false: per-corridor lists (fq_replan_pairs_assign*), whose candidate counts the callers check themselves;
+// windows = true (with shared = false): per-corridor windows (fq_replan_pairs_window*), no factor list in `a`
+int check_common(fq_ctx* ctx, const fq_pair_args* a, bool shared = true, bool windows = false)
 {
   if (!a) return fq_fail(ctx, FQ_E_ARG, "args is NULL");
   if (a->n_prob <= 0) return fq_fail(ctx, FQ_E_ARG, "n_prob <= 0");
@@ -35,7 +39,9 @@ int check_common(fq_ctx* ctx, const fq_pair_args* a, bool shared = true)
   if (!(a->DC > 0) || !(a->r_fraction >= 0 && a->r_fraction <= 1)) return fq_fail(ctx, FQ_E_ARG, "DC must be > 0 and r_fraction in [0, 1]");
   if (!shared)
   {
-    if (a->n_fac_whole <= 0 || a->n_fac_safe <= 0) return fq_fail(ctx, FQ_E_ARG, "empty factor grid");
+    if (windows && (a->factors_whole || a->factors_safe || a->n_fac_whole != 0 || a->n_fac_safe != 0))
+      return fq_fail(ctx, FQ_E_ARG, "per-corridor windows: factors_* must be NULL and n_fac_* 0");
+    if (!windows && (a->n_fac_whole <= 0 || a->n_fac_safe <= 0)) return fq_fail(ctx, FQ_E_ARG, "empty factor grid");
     if (a->sigmas_whole || a->sigmas_safe || a->n_sig_whole != 0 || a->n_sig_safe != 0)
       return fq_fail(ctx, FQ_E_ARG, "per-corridor assignment lists: sigmas_* must be NULL and n_sig_* 0");
   }
@@ -45,7 +51,7 @@ int check_common(fq_ctx* ctx, const fq_pair_args* a, bool shared = true)
       ((long long)a->n_prob * a->n_fac_whole * a->n_sig_whole > (1LL << 30) || (long long)a->n_prob * a->n_fac_safe * a->n_sig_safe > (1LL << 30)))
     return fq_fail(ctx, FQ_E_ARG, "too many candidates");
   if (!a->x0 || !a->xf_whole || !a->xf_safe || !a->lim || !a->poly_ofs_whole || !a->face_ofs_whole || !a->poly_ofs_safe ||
-      !a->face_ofs_safe || !a->factors_whole || !a->factors_safe || !a->results)
+      !a->face_ofs_safe || (!windows && (!a->factors_whole || !a->factors_safe)) || !a->results)
     return fq_fail(ctx, FQ_E_ARG, "NULL argument");
   return 0;
 }
@@ -58,6 +64,8 @@ struct Lists
   size_t ncw = 0, ncs = 0;              // candidates of the whole / safe sweep
   int mcw = 0, mcs = 0;                 // largest candidate count of one corridor
   int eew = 0, ees = 0;                 // candidates per time allocation (sizes an early-exit grid): the longest list
+  const fq_pair_window* win = nullptr;  // per-corridor windows (device pointers; needs `as`), or nullptr
+  int mfw = 0, mfs = 0;                 // with `win`: the factor rows' length (largest |F_j| allowed)
 };
 
 // largest |L(N, P, all_limit)| over P = 0 .. max_poly, or -1 when the list of max_poly polytopes is refused
@@ -66,6 +74,34 @@ long long longest_list(int N, int max_poly, long long all_limit)
   long long m = 0;
   for (int p = 0; p <= max_poly; p++) m = std::max(m, fqa::list_len(N, p, all_limit));
   return fqa::list_len(N, max_poly, all_limit) < 0 ? -1 : m;
+}
+
+// the hints of fq_pair_assign for the _dev entries -> the longest list of each sweep
+int check_assign_hints(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, long long* lw, long long* ls)
+{
+  if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
+  if (as->all_limit < 0) return fq_fail(ctx, FQ_E_ARG, "all_limit < 0");
+  if (as->max_poly_whole < 0 || as->max_poly_whole > FQ_MAX_POLY || as->max_poly_safe < 0 || as->max_poly_safe > FQ_MAX_POLY)
+    return fq_fail(ctx, FQ_E_ARG, "max_poly_* out of range (0..FQ_MAX_POLY)");
+  if (as->n_cand_whole < 0 || as->n_cand_whole > (1L << 30) || as->n_cand_safe < 0 || as->n_cand_safe > (1L << 30))
+    return fq_fail(ctx, FQ_E_ARG, "too many candidates (n_cand_* out of 0..2^30)");
+  *lw = longest_list(a->N_whole, as->max_poly_whole, as->all_limit);
+  *ls = longest_list(a->N_safe, as->max_poly_safe, as->all_limit);
+  if (*lw < 0 || *ls < 0) return fq_fail(ctx, FQ_E_ARG, "assignment list longer than 2^20");
+  if (((uintptr_t)a->Ab_whole & 15) || ((uintptr_t)a->Ab_safe & 15)) return fq_fail(ctx, FQ_E_ARG, "Ab must be 16-byte aligned");
+  return 0;
+}
+
+// the scalar parts of fq_pair_window, checked by every window entry
+const char* check_window_scalars(const fq_pair_window* w)
+{
+  if (!w) return "window is NULL";
+  if (!w->init_whole || !w->final_whole || !w->init_safe || !w->final_safe) return "window arrays must not be NULL";
+  if (!fqw::finite(w->inc_whole) || !(w->inc_whole > 0) || !fqw::finite(w->inc_safe) || !(w->inc_safe > 0))
+    return "inc_* must be finite and > 0";
+  if (!fqw::finite(w->gamma_whole) || !fqw::finite(w->gammap_whole) || !fqw::finite(w->gamma_safe) || !fqw::finite(w->gammap_safe))
+    return "gamma* must be finite";
+  return nullptr;
 }
 
 // the chain itself, every pointer a device pointer; `a` and the lists are checked
@@ -95,6 +131,8 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const Lists& l, fq_pair_result
       s.sig_w = carve<uint8_t>(p, ncw * Nw);   s.sig_s = carve<uint8_t>(p, ncs * Ns);
       s.win_sig_w = carve<uint8_t>(p, (size_t)P * Nw);  s.win_sig_s = carve<uint8_t>(p, (size_t)P * Ns);
       s.feas_w = carve<uint8_t>(p, ncw);       s.feas_s = carve<uint8_t>(p, ncs);   s.re_feas = carve<uint8_t>(p, P);
+      s.fac_w = carve<double>(p, l.win ? (size_t)P * l.mfw : 0);  s.fac_s = carve<double>(p, l.win ? (size_t)P * l.mfs : 0);
+      s.nf_w = carve<int>(p, l.win ? P : 0);   s.nf_s = carve<int>(p, l.win ? P : 0);
       return (size_t)(p - base);
     };
     need = layout(nullptr);
@@ -115,11 +153,25 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const Lists& l, fq_pair_result
     safe.N = Ns; safe.force_final = 0; safe.n_prob = P; safe.x0 = s.x0_safe; safe.xf = a->xf_safe; safe.lim = a->lim;
     safe.poly_ofs = a->poly_ofs_safe; safe.face_ofs = a->face_ofs_safe; safe.Ab = a->Ab_safe; safe.max_faces = a->max_faces_safe;
 
+    // ---- per-corridor windows: every window is read here, before anything is written (the outputs may alias them)
+    const fq_pair_window* win = l.win;
+    if (win)
+    {
+      FQ_CUDA(fq_launch_window_factors(P, l.mfw, win->init_whole, win->final_whole, win->inc_whole, s.fac_w, s.nf_w, st));
+      FQ_CUDA(fq_launch_window_factors(P, l.mfs, win->init_safe, win->final_safe, win->inc_safe, s.fac_s, s.nf_s, st));
+    }
     // ---- whole sweep (faster.cpp:406-418)
     FQ_CUDA(fq_launch_dtbase(P, Nw, a->DC, a->x0, a->xf_whole, a->lim, s.dt_base_w, st));
     if (!l.as)
       FQ_CUDA(fq_launch_expand_grid(P, Nw, a->n_fac_whole, a->n_sig_whole, a->factors_whole, a->sigmas_whole, s.dt_base_w, s.dt_w,
                                     s.sig_w, s.cand_ofs_w, st));
+    else if (win)
+    {
+      FQ_CUDA(fq_launch_window_offsets(P, Nw, l.mfw, l.as->all_limit, l.as->max_poly_whole, (long long)ncw, a->poly_ofs_whole, s.nf_w,
+                                       s.cand_ofs_w, st));
+      FQ_CUDA(fq_launch_expand_window(P, Nw, l.mfw, l.as->all_limit, s.fac_w, s.nf_w, s.dt_base_w, a->poly_ofs_whole, s.cand_ofs_w,
+                                      s.dt_w, s.sig_w, st));
+    }
     else
     {
       FQ_CUDA(fq_launch_assign_offsets(P, Nw, a->n_fac_whole, l.as->all_limit, l.as->max_poly_whole, (long long)ncw, a->poly_ofs_whole,
@@ -151,6 +203,13 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const Lists& l, fq_pair_result
     if (!l.as)
       FQ_CUDA(fq_launch_expand_grid(P, Ns, a->n_fac_safe, a->n_sig_safe, a->factors_safe, a->sigmas_safe, s.dt_base_s, s.dt_s,
                                     s.sig_s, s.cand_ofs_s, st));
+    else if (win)
+    {
+      FQ_CUDA(fq_launch_window_offsets(P, Ns, l.mfs, l.as->all_limit, l.as->max_poly_safe, (long long)ncs, a->poly_ofs_safe, s.nf_s,
+                                       s.cand_ofs_s, st));
+      FQ_CUDA(fq_launch_expand_window(P, Ns, l.mfs, l.as->all_limit, s.fac_s, s.nf_s, s.dt_base_s, a->poly_ofs_safe, s.cand_ofs_s,
+                                      s.dt_s, s.sig_s, st));
+    }
     else
     {
       FQ_CUDA(fq_launch_assign_offsets(P, Ns, a->n_fac_safe, l.as->all_limit, l.as->max_poly_safe, (long long)ncs, a->poly_ofs_safe,
@@ -184,12 +243,25 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const Lists& l, fq_pair_result
       f.cand_ofs_w = s.cand_ofs_w; f.cand_ofs_s = s.cand_ofs_s; f.n_fac_w = a->n_fac_whole; f.n_fac_s = a->n_fac_safe;
       f.N_w = Nw; f.N_s = Ns; f.win_sig_w = s.win_sig_w; f.win_sig_s = s.win_sig_s;
       f.sigma_out_w = l.as->sigma_whole; f.sigma_out_s = l.as->sigma_safe;
+      if (win) { f.n_fac_j_w = s.nf_w; f.n_fac_j_s = s.nf_s; }
       if (l.as->cand_ofs_whole)
         FQ_CUDA(cudaMemcpyAsync(l.as->cand_ofs_whole, s.cand_ofs_w, sizeof(int) * (size_t)(P + 1), cudaMemcpyDeviceToDevice, st));
       if (l.as->cand_ofs_safe)
         FQ_CUDA(cudaMemcpyAsync(l.as->cand_ofs_safe, s.cand_ofs_s, sizeof(int) * (size_t)(P + 1), cudaMemcpyDeviceToDevice, st));
     }
     FQ_CUDA(fq_launch_pair_final(f, st));
+    if (win)
+    {
+      FqPairWindowArgs wa;
+      wa.n_prob = P; wa.max_fac_w = l.mfw; wa.max_fac_s = l.mfs; wa.rec = a->results;
+      wa.cand_ofs_w = s.cand_ofs_w; wa.cand_ofs_s = s.cand_ofs_s; wa.n_fac_w = s.nf_w; wa.n_fac_s = s.nf_s; wa.fac_w = s.fac_w; wa.fac_s = s.fac_s;
+      wa.init_w = win->init_whole; wa.final_w = win->final_whole; wa.init_s = win->init_safe; wa.final_s = win->final_safe;
+      wa.gamma_w = win->gamma_whole; wa.gammap_w = win->gammap_whole; wa.gamma_s = win->gamma_safe; wa.gammap_s = win->gammap_safe;
+      wa.factor_w = win->factor_whole; wa.factor_s = win->factor_safe; wa.trials_w = win->trials_whole; wa.trials_s = win->trials_safe;
+      wa.next_init_w = win->next_init_whole; wa.next_final_w = win->next_final_whole;
+      wa.next_init_s = win->next_init_safe; wa.next_final_s = win->next_final_safe;
+      FQ_CUDA(fq_launch_pair_window(wa, st));
+    }
     // ---- the path's one exchange: every rank's result records to every rank (north_star: one all-gather, only when the
     //      batch is spread over several GPUs)
     if (results_all && ctx->comm)
@@ -225,17 +297,9 @@ extern "C" int fq_replan_pairs_assign_dev(fq_ctx* ctx, const fq_pair_args* a, co
 {
   if (!ctx) return FQ_E_ARG;
   if (int rc = check_common(ctx, a, false)) return rc;
-  if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
-  if (as->all_limit < 0) return fq_fail(ctx, FQ_E_ARG, "all_limit < 0");
-  if (as->max_poly_whole < 0 || as->max_poly_whole > FQ_MAX_POLY || as->max_poly_safe < 0 || as->max_poly_safe > FQ_MAX_POLY)
-    return fq_fail(ctx, FQ_E_ARG, "max_poly_* out of range (0..FQ_MAX_POLY)");
-  if (as->n_cand_whole < 0 || as->n_cand_whole > (1L << 30) || as->n_cand_safe < 0 || as->n_cand_safe > (1L << 30))
-    return fq_fail(ctx, FQ_E_ARG, "too many candidates (n_cand_* out of 0..2^30)");
-  const long long lw = longest_list(a->N_whole, as->max_poly_whole, as->all_limit);
-  const long long ls = longest_list(a->N_safe, as->max_poly_safe, as->all_limit);
-  if (lw < 0 || ls < 0) return fq_fail(ctx, FQ_E_ARG, "assignment list longer than 2^20");
+  long long lw = 0, ls = 0;
+  if (int rc = check_assign_hints(ctx, a, as, &lw, &ls)) return rc;
   if (lw * a->n_fac_whole > (1LL << 30) || ls * a->n_fac_safe > (1LL << 30)) return fq_fail(ctx, FQ_E_ARG, "too many candidates");
-  if (((uintptr_t)a->Ab_whole & 15) || ((uintptr_t)a->Ab_safe & 15)) return fq_fail(ctx, FQ_E_ARG, "Ab must be 16-byte aligned");
   FQ_CUDA(cudaSetDevice(ctx->device));
   cudaStream_t st = stream_v ? (cudaStream_t)stream_v : ctx->stream;
   Lists l;
@@ -246,12 +310,39 @@ extern "C" int fq_replan_pairs_assign_dev(fq_ctx* ctx, const fq_pair_args* a, co
   return run_chain(ctx, a, l, results_all, st);
 }
 
+// every pointer of `a`, `as` and `win` is a device pointer; the sweeps' sizes come from the hints of `as` (capacities) and
+// `win` (factor rows)
+extern "C" int fq_replan_pairs_window_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
+                                          fq_pair_result* results_all, void* stream_v)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (int rc = check_common(ctx, a, false, true)) return rc;
+  if (const char* why = check_window_scalars(win)) return fq_fail(ctx, FQ_E_ARG, why);
+  if (win->max_fac_whole < 0 || win->max_fac_whole > fqw::kMaxFactors || win->max_fac_safe < 0 || win->max_fac_safe > fqw::kMaxFactors)
+    return fq_fail(ctx, FQ_E_ARG, "max_fac_* out of range (0..4096)");
+  long long lw = 0, ls = 0;
+  if (int rc = check_assign_hints(ctx, a, as, &lw, &ls)) return rc;
+  if (lw * win->max_fac_whole > (1LL << 30) || ls * win->max_fac_safe > (1LL << 30)) return fq_fail(ctx, FQ_E_ARG, "too many candidates");
+  FQ_CUDA(cudaSetDevice(ctx->device));
+  cudaStream_t st = stream_v ? (cudaStream_t)stream_v : ctx->stream;
+  Lists l;
+  l.as = as; l.win = win;
+  l.ncw = (size_t)as->n_cand_whole; l.ncs = (size_t)as->n_cand_safe;
+  l.mfw = win->max_fac_whole; l.mfs = win->max_fac_safe;
+  l.mcw = (int)std::max(1LL, lw * l.mfw); l.mcs = (int)std::max(1LL, ls * l.mfs);
+  l.eew = (int)lw; l.ees = (int)ls;
+  return run_chain(ctx, a, l, results_all, st);
+}
+
 int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results,
-                            const fq_pair_assign* as)
+                            const fq_pair_assign* as, const fq_pair_window* win)
 {
   if (!ctx) return FQ_E_ARG;
   if (int rc = fq_settle(ctx)) return rc;
-  if (int rc = check_common(ctx, a, as == nullptr)) return rc;
+  if (win && !as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
+  if (int rc = check_common(ctx, a, as == nullptr, win != nullptr)) return rc;
+  if (win)
+    if (const char* why = check_window_scalars(win)) return fq_fail(ctx, FQ_E_ARG, why);
   const int P = a->n_prob, Nw = a->N_whole, Ns = a->N_safe;
   // ---- validate the two corridor descriptions
   auto check = [&](const int* po, const int* fo, const double* Ab, FqCorridorSizes* sizes) -> const char* {
@@ -275,6 +366,7 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
     if (a->factors_safe[i] < a->factors_safe[i - 1]) return fq_fail(ctx, FQ_E_ARG, "factors_safe must be ascending");
   size_t ncw = (size_t)P * a->n_fac_whole * a->n_sig_whole, ncs = (size_t)P * a->n_fac_safe * a->n_sig_safe;
   fq_pair_assign da{};                 // per-corridor lists: the device-side outputs and exact sizes
+  fq_pair_window dw{};                 // per-corridor windows: device copies and the longest factor lists
   if (as)
   {
     if (as->all_limit < 0) return fq_fail(ctx, FQ_E_ARG, "all_limit < 0");
@@ -285,7 +377,15 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
       const int pw = a->poly_ofs_whole[j + 1] - a->poly_ofs_whole[j], ps = a->poly_ofs_safe[j + 1] - a->poly_ofs_safe[j];
       const long long lw = fqa::list_len(Nw, pw, as->all_limit), ls = fqa::list_len(Ns, ps, as->all_limit);
       if (lw < 0 || ls < 0) return fq_fail(ctx, FQ_E_ARG, "assignment list of a corridor longer than 2^20");
-      tw += lw * a->n_fac_whole; ts += ls * a->n_fac_safe;
+      int nfw = a->n_fac_whole, nfs = a->n_fac_safe;
+      if (win)
+      {
+        nfw = fqw::factors(win->init_whole[j], win->final_whole[j], win->inc_whole, nullptr, 0);
+        nfs = fqw::factors(win->init_safe[j], win->final_safe[j], win->inc_safe, nullptr, 0);
+        if (nfw < 0 || nfs < 0) return fq_fail(ctx, FQ_E_ARG, "time-allocation window refused (not finite, init <= 0, more than 4096 factors or a stalled accumulation)");
+        dw.max_fac_whole = std::max(dw.max_fac_whole, nfw); dw.max_fac_safe = std::max(dw.max_fac_safe, nfs);
+      }
+      tw += lw * nfw; ts += ls * nfs;
       mpw = std::max(mpw, pw); mps = std::max(mps, ps);
     }
     if (tw > (1LL << 30) || ts > (1LL << 30)) return fq_fail(ctx, FQ_E_ARG, "too many candidates");
@@ -316,6 +416,7 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   const size_t opow = put(4 * (size_t)(P + 1)), ofow = put(4 * (size_t)(cw.n_poly + 1));
   const size_t opos = put(4 * (size_t)(P + 1)), ofos = put(4 * (size_t)(cs.n_poly + 1));
   const size_t osw = put((size_t)a->n_sig_whole * Nw), oss = put((size_t)a->n_sig_safe * Ns);
+  const size_t owin = win ? put(8 * 4 * (size_t)P) : 0;   // init_whole, final_whole, init_safe, final_safe
   const size_t in_bytes = o;
   o = 0;
   const size_t ores = put(sizeof(fq_pair_result) * (size_t)P);
@@ -323,6 +424,8 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   const size_t ocw = put(8 * ncw), ocs = put(8 * ncs), ofew = put(ncw), ofes = put(ncs);
   size_t ocaw = 0, ocas = 0, osgw = 0, osgs = 0;        // per-corridor lists: offsets and winners' assignments
   if (as) { ocaw = put(4 * (size_t)(P + 1)); ocas = put(4 * (size_t)(P + 1)); osgw = put((size_t)P * Nw); osgs = put((size_t)P * Ns); }
+  size_t ofac = 0, otri = 0, onext = 0;                 // windows: factor_* (2 P), trials_* (2 P), next_* (4 P)
+  if (win) { ofac = put(8 * 2 * (size_t)P); otri = put(4 * 2 * (size_t)P); onext = put(8 * 4 * (size_t)P); }
   const size_t out_bytes = o;
   FQ_CUDA(ctx->h_in.reserve(in_bytes));
   FQ_CUDA(ctx->d_pair_io.reserve(in_bytes + out_bytes));
@@ -333,8 +436,13 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   if (cs.n_face) std::memcpy(hi + oAbs, a->Ab_safe, 32 * (size_t)cs.n_face);
   std::memcpy(hi + ox0, a->x0, 72 * (size_t)P);      std::memcpy(hi + oxfw, a->xf_whole, 72 * (size_t)P);
   std::memcpy(hi + oxfs, a->xf_safe, 72 * (size_t)P); std::memcpy(hi + olim, a->lim, 24 * (size_t)P);
-  std::memcpy(hi + ofw, a->factors_whole, 8 * (size_t)a->n_fac_whole);
-  std::memcpy(hi + ofs, a->factors_safe, 8 * (size_t)a->n_fac_safe);
+  if (a->n_fac_whole) std::memcpy(hi + ofw, a->factors_whole, 8 * (size_t)a->n_fac_whole);
+  if (a->n_fac_safe) std::memcpy(hi + ofs, a->factors_safe, 8 * (size_t)a->n_fac_safe);
+  if (win)
+  {
+    const double* w4[4] = { win->init_whole, win->final_whole, win->init_safe, win->final_safe };
+    for (int i = 0; i < 4; i++) std::memcpy(hi + owin + 8 * (size_t)P * i, w4[i], 8 * (size_t)P);
+  }
   std::memcpy(hi + opow, a->poly_ofs_whole, 4 * (size_t)(P + 1)); std::memcpy(hi + ofow, a->face_ofs_whole, 4 * (size_t)(cw.n_poly + 1));
   std::memcpy(hi + opos, a->poly_ofs_safe, 4 * (size_t)(P + 1));  std::memcpy(hi + ofos, a->face_ofs_safe, 4 * (size_t)(cs.n_poly + 1));
   if (a->sigmas_whole) std::memcpy(hi + osw, a->sigmas_whole, (size_t)a->n_sig_whole * Nw);
@@ -346,7 +454,8 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   d.lim = (const double*)(din + olim);
   d.poly_ofs_whole = (const int*)(din + opow); d.face_ofs_whole = (const int*)(din + ofow); d.Ab_whole = (const double*)(din + oAbw);
   d.poly_ofs_safe = (const int*)(din + opos); d.face_ofs_safe = (const int*)(din + ofos); d.Ab_safe = (const double*)(din + oAbs);
-  d.factors_whole = (const double*)(din + ofw); d.factors_safe = (const double*)(din + ofs);
+  d.factors_whole = a->factors_whole ? (const double*)(din + ofw) : nullptr;
+  d.factors_safe = a->factors_safe ? (const double*)(din + ofs) : nullptr;
   d.sigmas_whole = a->sigmas_whole ? (const uint8_t*)(din + osw) : nullptr;
   d.sigmas_safe = a->sigmas_safe ? (const uint8_t*)(din + oss) : nullptr;
   d.feasible_whole = a->feasible_whole ? (uint8_t*)(dout + ofew) : nullptr; d.cost_whole = a->cost_whole ? (double*)(dout + ocw) : nullptr;
@@ -362,7 +471,22 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
     da.cand_ofs_whole = as->cand_ofs_whole ? (int*)(dout + ocaw) : nullptr; da.cand_ofs_safe = as->cand_ofs_safe ? (int*)(dout + ocas) : nullptr;
     da.sigma_whole = as->sigma_whole ? (uint8_t*)(dout + osgw) : nullptr;  da.sigma_safe = as->sigma_safe ? (uint8_t*)(dout + osgs) : nullptr;
   }
-  int rc = as ? fq_replan_pairs_assign_dev(ctx, &d, &da, nullptr, st) : fq_replan_pairs_dev(ctx, &d, nullptr, st);
+  if (win)
+  {
+    const double* wi = (const double*)(din + owin);
+    double* fo = (double*)(dout + ofac);
+    int* to = (int*)(dout + otri);
+    double* no = (double*)(dout + onext);
+    dw.init_whole = wi; dw.final_whole = wi + P; dw.init_safe = wi + 2 * (size_t)P; dw.final_safe = wi + 3 * (size_t)P;
+    dw.inc_whole = win->inc_whole; dw.inc_safe = win->inc_safe;
+    dw.gamma_whole = win->gamma_whole; dw.gammap_whole = win->gammap_whole; dw.gamma_safe = win->gamma_safe; dw.gammap_safe = win->gammap_safe;
+    dw.factor_whole = win->factor_whole ? fo : nullptr;               dw.factor_safe = win->factor_safe ? fo + P : nullptr;
+    dw.trials_whole = win->trials_whole ? to : nullptr;               dw.trials_safe = win->trials_safe ? to + P : nullptr;
+    dw.next_init_whole = win->next_init_whole ? no : nullptr;         dw.next_final_whole = win->next_final_whole ? no + P : nullptr;
+    dw.next_init_safe = win->next_init_safe ? no + 2 * (size_t)P : nullptr; dw.next_final_safe = win->next_final_safe ? no + 3 * (size_t)P : nullptr;
+  }
+  int rc = win ? fq_replan_pairs_window_dev(ctx, &d, &da, &dw, nullptr, st)
+         : as ? fq_replan_pairs_assign_dev(ctx, &d, &da, nullptr, st) : fq_replan_pairs_dev(ctx, &d, nullptr, st);
   if (rc) return rc;
   // ---- results straight into the caller's arrays (asynchronous when they are pinned)
   if (d_results) *d_results = (fq_pair_result*)(dout + ores);
@@ -385,6 +509,16 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
     if (as->cand_ofs_safe) FQ_CUDA(cudaMemcpyAsync(as->cand_ofs_safe, dout + ocas, 4 * (size_t)(P + 1), cudaMemcpyDeviceToHost, st));
     if (as->sigma_whole) FQ_CUDA(cudaMemcpyAsync(as->sigma_whole, dout + osgw, (size_t)P * Nw, cudaMemcpyDeviceToHost, st));
     if (as->sigma_safe) FQ_CUDA(cudaMemcpyAsync(as->sigma_safe, dout + osgs, (size_t)P * Ns, cudaMemcpyDeviceToHost, st));
+  }
+  if (win)
+  { // the caller's window arrays were copied into the upload above, so the next_* outputs may alias them
+    auto back = [&](void* host, const void* dev, size_t elem) {
+      return host ? cudaMemcpyAsync(host, dev, elem * (size_t)P, cudaMemcpyDeviceToHost, st) : cudaSuccess;
+    };
+    FQ_CUDA(back(win->factor_whole, dw.factor_whole, 8));   FQ_CUDA(back(win->factor_safe, dw.factor_safe, 8));
+    FQ_CUDA(back(win->trials_whole, dw.trials_whole, 4));   FQ_CUDA(back(win->trials_safe, dw.trials_safe, 4));
+    FQ_CUDA(back(win->next_init_whole, dw.next_init_whole, 8)); FQ_CUDA(back(win->next_final_whole, dw.next_final_whole, 8));
+    FQ_CUDA(back(win->next_init_safe, dw.next_init_safe, 8));   FQ_CUDA(back(win->next_final_safe, dw.next_final_safe, 8));
   }
   if (deferred) { ctx->pending = true; return 0; }
   FQ_CUDA(cudaStreamSynchronize(st));
@@ -415,4 +549,21 @@ extern "C" int fq_replan_pairs_assign_async(fq_ctx* ctx, const fq_pair_args* a, 
   if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
   if (ctx->is_group || ctx->comm) return fq_replan_pairs_sharded(ctx, a, true, as);
   return fq_replan_pairs_host_ex(ctx, a, true, nullptr, true, as);
+}
+
+extern "C" int fq_replan_pairs_window(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
+  if (!win) return fq_fail(ctx, FQ_E_ARG, "window is NULL");
+  if (ctx->is_group || ctx->comm) return fq_replan_pairs_sharded(ctx, a, false, as, win);
+  return fq_replan_pairs_host_ex(ctx, a, false, nullptr, true, as, win);
+}
+extern "C" int fq_replan_pairs_window_async(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
+  if (!win) return fq_fail(ctx, FQ_E_ARG, "window is NULL");
+  if (ctx->is_group || ctx->comm) return fq_replan_pairs_sharded(ctx, a, true, as, win);
+  return fq_replan_pairs_host_ex(ctx, a, true, nullptr, true, as, win);
 }

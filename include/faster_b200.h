@@ -47,7 +47,7 @@ typedef struct fq_ctx fq_ctx;     /* opaque: device, stream, plan tables, scratc
 
 int fq_abi_version(void);
 /* 1 if this build has the named feature: "sweep_early_exit", "replan_pairs", "multi_gpu", "row_tol", "certificates",
- * "replan_pairs_assign". */
+ * "replan_pairs_assign", "replan_pairs_window". */
 int fq_has_feature(const char* name);
 
 /* Threading: a context is used from one thread at a time, like a SolverGurobi instance in the reference (one replan
@@ -283,6 +283,59 @@ int fq_replan_pairs_assign_async(fq_ctx* ctx, const fq_pair_args* args, const fq
  * does not synchronise.  Refused up front (FQ_E_ARG): max_poly_* outside 0..FQ_MAX_POLY, n_cand_* outside 0..2^30. */
 int fq_replan_pairs_assign_dev(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, fq_pair_result* results_all,
                                void* stream);
+
+/* ---- chained replan with a per-corridor time-allocation window ------------------------------------------------------
+ *
+ * The one piece of solver state Faster::replan() carries from one replan to the next is each solver object's window of
+ * time-allocation factors: [1, 10] with step increment_* at start-up (setFactorInitialAndFinalAndIncrement, faster.cpp:57,
+ * :68), then, after every replan in which BOTH sweeps succeed, [max(f* - gamma, 1.0), f* + gammap] around the factor that
+ * worked (faster.cpp:582-588).  genNewTraj visits the factors `for (double i = fi; i <= ff; i = i + inc)`
+ * (solverGurobi.cpp:445-446).  The entry points below give corridor j its OWN window and list:
+ *   F_j = the factors that loop visits for (init_*[j], final_*[j], inc_*), accumulated as it does (never fi + k inc);
+ *         final < init gives no factor (no candidate, no winner).  Refused: a bound or inc not finite, init <= 0,
+ *         inc <= 0, more than 4096 factors (the drop-in class's cap), or an accumulation that stalls (i + inc == i).
+ *   candidates of corridor j: |F_j| x |L_j| (L_j: the per-corridor assignment list of fq_pair_assign), factor-major,
+ *         dt = F_j[f] * max(getDTInitial, 2 DC); *_dt_index of the result records indexes F_j.
+ *   factor_*[j]  factor_that_worked_ (NaN: no winner)
+ *   trials_*[j]  the winner's index in F_j + 1; |F_j| without a winner; 0 for a sweep that did not run (the safe sweep
+ *                after a whole sweep without winner; an emptied sweep of the _dev variant)
+ *   next_*[j]    the window of the next replan: if both sweeps won, max(f*_w - gamma_whole, 1.0) and f*_w + gammap_whole
+ *                (and likewise for safe); otherwise the input window unchanged, since replan() returns before its update
+ *                (faster.cpp:420-424, :529-533).  appendToPlan's early return (:548) is planner state and not modelled.
+ * fq_pair_args is used as for fq_replan_pairs_assign except that factors_* must be NULL and n_fac_* 0 (FQ_E_ARG otherwise);
+ * `assign` is required.  Feature "replan_pairs_window". */
+typedef struct fq_pair_window
+{
+  const double *init_whole, *final_whole, *init_safe, *final_safe;  /* n_prob each: setFactorInitialAndFinalAndIncrement */
+  double inc_whole, inc_safe;                                       /* par_.increment_*                                  */
+  double gamma_whole, gammap_whole, gamma_safe, gammap_safe;        /* par_.gamma*_, for the next window                */
+  int max_fac_whole, max_fac_safe;                                  /* _dev only: largest |F_j| (hint, checked)          */
+  double *factor_whole, *factor_safe;                               /* out n_prob, or NULL                               */
+  int *trials_whole, *trials_safe;                                  /* out n_prob, or NULL                               */
+  double *next_init_whole, *next_final_whole, *next_init_safe, *next_final_safe;  /* out n_prob, or NULL; MAY alias the inputs */
+} fq_pair_window;
+
+/* |F(fi, ff, inc)|, writing its first min(|F|, cap) factors to out (may be NULL); FQ_E_ARG when the window is refused.
+ * Pure host code, the same source as the device's. */
+long fq_pair_window_factors(double fi, double ff, double inc, double* out, long cap);
+/* HOST pointers everywhere (window arrays included); every window is validated here (FQ_E_ARG).  Blocks until every output
+ * is in the caller's arrays.  On a multi-GPU context the corridors are sharded by candidate count |F_j| x |L_j|, whole +
+ * safe, as fq_replan_pairs_assign does. */
+int fq_replan_pairs_window(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window);
+/* The same, returning once everything is enqueued; outputs are valid after fq_wait(ctx).  Arrays must stay alive. */
+int fq_replan_pairs_window_async(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window);
+/* DEVICE pointers everywhere (the three structs live on the host), as fq_replan_pairs_assign_dev, so that consecutive
+ * replans of a batch can pass each call's next_* arrays (or the same arrays: they may alias init_* / final_*) to the next
+ * call without a host round trip.  The library cannot read the windows, so for this call assign->n_cand_* is a CAPACITY
+ * (the per-candidate outputs hold that many; the sweep's total must not exceed it) and window->max_fac_* bounds |F_j|
+ * (the rows of factors kept on the device; for gamma = gammap = 20 and inc = 1 every window after the first has at most
+ * 41 factors).  cand_ofs_* report the layout used.  If a window of a sweep is refused, a corridor has more than max_fac_*
+ * factors or more than max_poly_* polytopes, or the total exceeds the capacity, that sweep gets NO candidates: every winner
+ * of it is "none", nothing is written to its per-candidate outputs, and every window is returned unchanged, so a closed
+ * loop's state is never corrupted.  The call still returns 0.  Refused up front (FQ_E_ARG): inc_* not finite or <= 0,
+ * max_fac_* outside 0..4096, and the hints fq_replan_pairs_assign_dev refuses. */
+int fq_replan_pairs_window_dev(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
+                               fq_pair_result* results_all, void* stream);
 
 /* ---- several GPUs behind the boundary (SURVEY.md 8b/8e) ---------------------------------------------------------
  *
