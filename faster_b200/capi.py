@@ -16,7 +16,8 @@ EXPORTS = ["fq_abi_version", "fq_create", "fq_destroy", "fq_last_error", "fq_set
            "fq_replan_pairs", "fq_replan_pairs_async", "fq_replan_pairs_dev", "fq_create_multi", "fq_comm_unique_id", "fq_comm_init",
            "fq_comm_info", "fq_allgather_dev", "fq_shard_range", "fq_solve_multi_sharded", "fq_solve_batch_cert", "fq_has_feature",
            "fq_pair_assign_count", "fq_replan_pairs_assign", "fq_replan_pairs_assign_async", "fq_replan_pairs_assign_dev",
-           "fq_pair_window_factors", "fq_replan_pairs_window", "fq_replan_pairs_window_async", "fq_replan_pairs_window_dev"]
+           "fq_pair_window_factors", "fq_replan_pairs_window", "fq_replan_pairs_window_async", "fq_replan_pairs_window_dev",
+           "fq_replan_pairs_exact", "fq_replan_pairs_exact_async", "fq_replan_pairs_exact_dev"]
 
 
 class FqError(RuntimeError):
@@ -70,6 +71,12 @@ class PairWindow(C.Structure):
                 ("next_final_safe", C.c_void_p)]
 
 
+class PairExact(C.Structure):
+    """fq_pair_exact of include/faster_b200.h: per-corridor outputs of the exact chain."""
+    _fields_ = [("exact_whole", C.c_void_p), ("exact_safe", C.c_void_p), ("nodes_whole", C.c_void_p), ("nodes_safe", C.c_void_p)]
+
+
+EXACT_KEYS = ["exact_whole", "exact_safe", "nodes_whole", "nodes_safe"]
 WINDOW_IN_KEYS = ["init_whole", "final_whole", "init_safe", "final_safe"]
 WINDOW_OUT_KEYS = ["factor_whole", "factor_safe", "trials_whole", "trials_safe", "next_init_whole", "next_final_whole",
                    "next_init_safe", "next_final_safe"]
@@ -125,6 +132,11 @@ def lib():
         L.fq_replan_pairs_window_async.argtypes = L.fq_replan_pairs_window.argtypes
         L.fq_replan_pairs_window_dev.argtypes = [C.c_void_p, C.POINTER(PairArgs), C.POINTER(PairAssign), C.POINTER(PairWindow),
                                                  C.c_void_p, C.c_void_p]
+        L.fq_replan_pairs_exact.argtypes = [C.c_void_p, C.POINTER(PairArgs), C.POINTER(PairAssign), C.POINTER(PairWindow),
+                                            C.POINTER(PairExact)]
+        L.fq_replan_pairs_exact_async.argtypes = L.fq_replan_pairs_exact.argtypes
+        L.fq_replan_pairs_exact_dev.argtypes = [C.c_void_p, C.POINTER(PairArgs), C.POINTER(PairAssign), C.POINTER(PairWindow),
+                                                C.POINTER(PairExact), C.c_void_p, C.c_void_p]
         L.fq_create_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_void_p]
         L.fq_comm_unique_id.argtypes = [C.c_void_p]
         L.fq_comm_init.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
@@ -225,6 +237,14 @@ def window_args(win, out_ptrs, inc=1.0, gamma=20.0, max_fac_whole=0, max_fac_saf
     s.gamma_whole, s.gammap_whole, s.gamma_safe, s.gammap_safe = (float(g) for g in gamma)
     s.max_fac_whole, s.max_fac_safe = int(max_fac_whole), int(max_fac_safe)
     for k in WINDOW_OUT_KEYS:
+        setattr(s, k, out_ptrs.get(k) or None)
+    return s
+
+
+def exact_args(out_ptrs):
+    """PairExact; out_ptrs: addresses of EXACT_KEYS (0/None/missing = NULL)."""
+    s = PairExact()
+    for k in EXACT_KEYS:
         setattr(s, k, out_ptrs.get(k) or None)
     return s
 
@@ -500,6 +520,54 @@ class Solver:
         fn = self._L.fq_replan_pairs_window_async if deferred else self._L.fq_replan_pairs_window
         self._check(fn(self._h, C.byref(a), C.byref(s), C.byref(wa)))
         return out
+
+    def replan_pairs_exact(self, w, all_limit=0, windows=None, inc=1.0, gamma=20.0, want_candidates=True, want_coeffs=True,
+                           deferred=False):
+        """fq_replan_pairs_exact on a make_pair_workload dict (host arrays; its sigmas_* are not used).  windows=None: the shared
+        factor lists factors_* of `w`, as replan_pairs_assign; otherwise per-corridor windows as replan_pairs_window.  -> the
+        dict of replan_pairs_assign (or _window) plus exact_whole, exact_safe (int32: 1 = the minimum over all assignments)
+        and nodes_whole, nodes_safe (int64: tree nodes evaluated).  deferred: valid after wait()."""
+        n = w["n_prob"]
+        if windows is None:
+            offs = {kind: assign_offsets(w["poly_ofs_" + kind], w["N_" + kind], len(w["factors_" + kind]), all_limit)
+                    for kind in ("whole", "safe")}
+        else:
+            wins = {k: np.ascontiguousarray(windows[k], np.float64) for k in WINDOW_IN_KEYS}
+            incs = (inc, inc) if np.isscalar(inc) else tuple(inc)
+            offs = {}
+            for kind, ik in (("whole", incs[0]), ("safe", incs[1])):
+                nf = [len(window_factors(a, b, ik)) for a, b in zip(wins["init_" + kind], wins["final_" + kind])]
+                offs[kind] = window_offsets(w["poly_ofs_" + kind], w["N_" + kind], nf, all_limit)
+        out = dict(results=np.zeros(n, PAIR_RESULT_DTYPE), cand_ofs_whole=np.zeros(n + 1, np.int32), cand_ofs_safe=np.zeros(n + 1, np.int32),
+                   sigma_whole=np.zeros((n, w["N_whole"]), np.uint8), sigma_safe=np.zeros((n, w["N_safe"]), np.uint8),
+                   exact_whole=np.zeros(n, np.int32), exact_safe=np.zeros(n, np.int32), nodes_whole=np.zeros(n, np.int64),
+                   nodes_safe=np.zeros(n, np.int64))
+        if windows is not None:
+            out.update({k: (np.zeros(n, np.int32) if k.startswith("trials") else np.zeros(n)) for k in WINDOW_OUT_KEYS})
+        if want_candidates:
+            ncw, ncs = int(offs["whole"][-1]), int(offs["safe"][-1])
+            out.update(feasible_whole=np.zeros(ncw, np.uint8), cost_whole=np.zeros(ncw), feasible_safe=np.zeros(ncs, np.uint8),
+                       cost_safe=np.zeros(ncs))
+        if want_coeffs:
+            out.update(coeffs_whole=np.zeros((n, w["N_whole"], 12)), coeffs_safe=np.zeros((n, w["N_safe"], 12)))
+        skip = ("sigmas_",) if windows is None else ("sigmas_", "factors_")
+        a = pair_args(w, lambda k: None if k.startswith(skip) else w[k].ctypes.data, {k: v.ctypes.data for k, v in out.items()})
+        a.n_sig_whole = a.n_sig_safe = 0
+        if windows is not None:
+            a.n_fac_whole = a.n_fac_safe = 0
+        s = assign_args(all_limit, {k: out[k].ctypes.data for k in ("cand_ofs_whole", "cand_ofs_safe", "sigma_whole", "sigma_safe")})
+        wa = None if windows is None else window_args(lambda k: wins[k].ctypes.data, {k: out[k].ctypes.data for k in WINDOW_OUT_KEYS},
+                                                       inc, gamma)
+        ex = exact_args({k: out[k].ctypes.data for k in EXACT_KEYS})
+        fn = self._L.fq_replan_pairs_exact_async if deferred else self._L.fq_replan_pairs_exact
+        self._check(fn(self._h, C.byref(a), C.byref(s), C.byref(wa) if wa is not None else None, C.byref(ex)))
+        return out
+
+    def replan_pairs_exact_dev(self, a, s, win, ex, results_all=0, stream=0):
+        """fq_replan_pairs_exact_dev: `a`, `s`, `win` (PairWindow or None) and `ex` (PairExact) hold device addresses and the
+        host hints of the _assign_dev / _window_dev entries."""
+        self._check(self._L.fq_replan_pairs_exact_dev(self._h, C.byref(a), C.byref(s), C.byref(win) if win is not None else None,
+                                                      C.byref(ex), results_all or None, stream or None))
 
     def replan_pairs_window_dev(self, a, s, win, results_all=0, stream=0):
         """fq_replan_pairs_window_dev: `a` (PairArgs), `s` (PairAssign) and `win` (PairWindow) hold device addresses and the

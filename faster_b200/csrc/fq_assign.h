@@ -85,4 +85,34 @@ FQ_HD void unrank(int N, int P, bool all, long long idx, const long long* binom_
     out[t] = (uint8_t)v;
   }
 }
+
+// the index of s[0 .. N-1] in L(N, P, all_limit) (the inverse of unrank), or -1 when s is not in the list
+FQ_HD long long rank(int N, int P, bool all, const uint8_t* s)
+{
+  long long idx = 0;
+  if (P <= 0)
+  {
+    for (int t = 0; t < N; t++)
+      if (s[t] != 0) return -1;
+    return 0;
+  }
+  if (all)
+  {
+    for (int t = 0; t < N; t++)
+    {
+      if (s[t] >= P) return -1;
+      idx = idx * P + s[t];
+    }
+    return idx;
+  }
+  int v = 0;
+  for (int t = 0; t < N; t++)
+  {
+    if (s[t] < v || s[t] >= P) return -1;
+    const int m = N - t - 1;
+    for (int c = v; c < s[t]; c++) idx += binom(m + (P - c) - 1, m);
+    v = s[t];
+  }
+  return idx;
+}
 }  // namespace fqa

@@ -1,5 +1,6 @@
 // C ABI of faster_b200 (see include/faster_b200.h): context, plan cache, host<->device staging, launches.
 #include "fq_ctx.h"
+#include "fq_presolve.h"
 
 #include <algorithm>
 #include <chrono>
@@ -143,7 +144,7 @@ extern "C" int fq_has_feature(const char* name)
   if (!name) return 0;
   const std::string n(name);
   if (n == "sweep_early_exit" || n == "replan_pairs" || n == "multi_gpu" || n == "row_tol" || n == "certificates" ||
-      n == "replan_pairs_assign" || n == "replan_pairs_window")
+      n == "replan_pairs_assign" || n == "replan_pairs_window" || n == "replan_pairs_exact")
     return 1;
   return 0;
 }
@@ -805,7 +806,7 @@ extern "C" int fq_gen_new_traj_exact(fq_ctx* ctx, int N, int force_final, const 
     const size_t opo = o;    o += sizeof(int) * 2;
     const size_t ofo = o;    o += sizeof(int) * (size_t)(P + 1);
     const size_t oroot = o;  o += sizeof(int) * (size_t)n_dt;
-    const size_t ocnt = o;   o = fq_align16(o + sizeof(int) * 8);   // [0] n_children [1] n_leaves [2..3] flags
+    const size_t ocnt = o;   o = fq_align16(o + sizeof(int) * 8);   // [0..1] parents of even / odd levels [2] n_leaves [3..4] flags
     const size_t head = o;
     const size_t oleaf = o;  o = fq_align16(o + 32 * (size_t)leaf_cap);
     const size_t opoolA = o; o = fq_align16(o + nb * (size_t)cap);
@@ -821,19 +822,7 @@ extern "C" int fq_gen_new_traj_exact(fq_ctx* ctx, int N, int force_final, const 
     std::memcpy(hi + oxf, xf, sizeof(double) * 9);
     std::memcpy(hi + olim, lim, sizeof(double) * 3);
     std::memcpy(hi + odts, dts, sizeof(double) * (size_t)n_dt);
-    // presolve on the constant control points: segment 0 starts with cp0, cp1, cp2 fixed by (x0, dt) and, with the final
-    // position pinned, the last control point is xf -- a time allocation for which no polytope holds them is infeasible
-    // for EVERY assignment and needs no tree (otherwise such corridors make the tree explore all prefixes)
-    auto inside_any = [&](const double* pt) {
-      for (int p = 0; p < P; p++)
-      {
-        bool in = true;
-        for (int f = face_ofs[p]; f < face_ofs[p + 1] && in; f++)
-          in = Ab[4 * f] * pt[0] + Ab[4 * f + 1] * pt[1] + Ab[4 * f + 2] * pt[2] - Ab[4 * f + 3] <= ctx->row_tol;
-        if (in) return true;
-      }
-      return false;
-    };
+    // presolve (fq_presolve.h): time allocations at which no assignment can be feasible get no root
     int n_roots = 0;
     for (int d = 0; d < n_dt; d++)
     {
@@ -842,28 +831,10 @@ extern "C" int fq_gen_new_traj_exact(fq_ctx* ctx, int N, int force_final, const 
       std::memcpy(&bits, &c, 8);
       ((unsigned long long*)(hi + oinc))[d] = bits;              // +inf orders above every finite cost
       if (d >= n_search) continue;
-      bool possible = true;
-      if (force_final) possible = inside_any(xf);
-      if (possible)
-      { // all three constant points of segment 0 must share one polytope
-        possible = false;
-        const double t = dts[d];
-        for (int p = 0; p < P && !possible; p++)
-        {
-          bool in = true;
-          for (int kk = 0; kk < 3 && in; kk++)
-          {
-            double pt[3];
-            for (int ax = 0; ax < 3; ax++)
-              pt[ax] = x0[ax] + (kk >= 1 ? x0[3 + ax] * t * (kk == 1 ? 1.0 / 3.0 : 2.0 / 3.0) : 0.0) + (kk == 2 ? x0[6 + ax] * t * t / 6.0 : 0.0);
-            for (int f = face_ofs[p]; f < face_ofs[p + 1] && in; f++)
-              in = Ab[4 * f] * pt[0] + Ab[4 * f + 1] * pt[1] + Ab[4 * f + 2] * pt[2] - Ab[4 * f + 3] <= ctx->row_tol;
-          }
-          possible = in;
-        }
-      }
+      const bool possible = fqs::root_possible(P, face_ofs, Ab, x0, xf, force_final, dts[d], ctx->row_tol);
       if (possible) ((int*)(hi + oroot))[n_roots++] = d;
     }
+    ((int*)(hi + ocnt))[0] = n_roots;
     ((int*)(hi + opo))[0] = 0; ((int*)(hi + opo))[1] = P;
     for (int p = 0; p <= P; p++) ((int*)(hi + ofo))[p] = face_ofs[p];
     cudaStream_t st = ctx->stream;
@@ -876,16 +847,19 @@ extern "C" int fq_gen_new_traj_exact(fq_ctx* ctx, int N, int force_final, const 
     L.k.n_prob = 1; L.k.x0 = (const double*)(db + ox0); L.k.xf = (const double*)(db + oxf); L.k.lim = (const double*)(db + olim);
     L.k.poly_ofs = (const int*)(db + opo); L.k.face_ofs = (const int*)(db + ofo); L.k.Ab = (const double*)(db + oAb);
     L.k.max_faces = n_face; L.k.item_cap = N * cs.max_poly_faces; L.k.row_tol = ctx->row_tol;
-    L.n_dt = n_dt; L.P = P; L.dts = (const double*)(db + odts); L.roots = (const int*)(db + oroot);
-    L.incumbent = (unsigned long long*)(db + oinc); L.leaves = db + oleaf; L.n_leaves = (int*)(db + ocnt) + 1;
-    L.leaf_cap = leaf_cap; L.flags = (int*)(db + ocnt) + 2; L.n_children = (int*)(db + ocnt); L.cap = cap;
+    L.n_dt = n_dt; L.dts = (const double*)(db + odts); L.roots = (const int*)(db + oroot);
+    L.incumbent = (unsigned long long*)(db + oinc); L.leaves = db + oleaf; L.n_leaves = (int*)(db + ocnt) + 2;
+    L.leaf_cap = leaf_cap; L.flags = (int*)(db + ocnt) + 3; L.cap = cap; L.nodes = nullptr; L.keep_ties = 0;
     int n_par = n_roots;
     long nodes = 0;
     unsigned char* pools[2] = { (unsigned char*)(db + opoolA), (unsigned char*)(db + opoolB) };
-    int cnt[4] = { 0, 0, 0, 0 };
+    int cnt[5] = { 0, 0, 0, 0, 0 };
+    // one corridor, one warp per child.  The levels are driven from the host: it sizes each launch to the level's
+    // children and stops at the first cut, which keeps this sweep's node counts and costs as they were
     for (int depth = 0; depth < N && n_par > 0; depth++)
     {
-      L.depth = depth; L.n_parents = n_par;
+      L.depth = depth; L.cpc = (int)(((long long)n_par * P + FQ_WARPS_PER_CTA - 1) / FQ_WARPS_PER_CTA);
+      L.n_parents = (int*)(db + ocnt) + (depth & 1); L.n_children = (int*)(db + ocnt) + ((depth + 1) & 1);
       L.parents = pools[depth & 1]; L.children = pools[(depth + 1) & 1];
       FQ_CUDA(cudaMemsetAsync(L.n_children, 0, sizeof(int), st));
       cudaError_t e = fq_launch_bnb_level(L, st);
@@ -894,15 +868,15 @@ extern "C" int fq_gen_new_traj_exact(fq_ctx* ctx, int N, int force_final, const 
       FQ_CUDA(cudaMemcpyAsync(cnt, db + ocnt, sizeof(cnt), cudaMemcpyDeviceToHost, st));
       FQ_CUDA(cudaStreamSynchronize(st));
       nodes += (long)n_par * P;
-      if (cnt[2]) { exact = false; break; }                      // pool overflow: the tree was cut
-      if (cnt[3]) { exact = false; break; }                      // a node hit the iteration cap / a NaN and its subtree was
+      if (cnt[3]) { exact = false; break; }                      // pool overflow: the tree was cut
+      if (cnt[4]) { exact = false; break; }                      // a node hit the iteration cap / a NaN and its subtree was
                                                                  // dropped: the optimum may hide there, so not exact
-      n_par = cnt[0];
+      n_par = cnt[(depth + 1) & 1];
     }
     if (nodes_out) *nodes_out = nodes;
     if (exact)
     {
-      const int n_leaves = std::min(cnt[1], leaf_cap);
+      const int n_leaves = std::min(cnt[2], leaf_cap);
       struct Leaf { int dt_idx, pad; double cost; unsigned char sigma[16]; };
       std::vector<Leaf> leaves((size_t)std::max(n_leaves, 1));
       std::vector<unsigned long long> inc(n_dt);

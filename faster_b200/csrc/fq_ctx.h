@@ -117,9 +117,10 @@ int fq_solve_multi_host_ex(fq_ctx* ctx, int N, int force_final, int n_prob, cons
 // fq_pair_capi.cu.  d_results (may be NULL): receives the device address of the result records; copy_results = false
 // leaves the caller's `results` array untouched (the multi-GPU path reads the all-gathered table instead).  as != NULL:
 // per-corridor assignment lists (fq_replan_pairs_assign*, host pointers); win != NULL (with as): per-corridor windows
-// (fq_replan_pairs_window*, host pointers)
+// (fq_replan_pairs_window*, host pointers); ex != NULL (with as): the exact stage (fq_replan_pairs_exact*, host pointers)
 int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results,
-                            const fq_pair_assign* as = nullptr, const fq_pair_window* win = nullptr);
+                            const fq_pair_assign* as = nullptr, const fq_pair_window* win = nullptr,
+                            const fq_pair_exact* ex = nullptr);
 // fq_multi.cu
 void fq_comm_release(fq_ctx* ctx);
 // all-gather on one context's communicator (one process per GPU): `bytes` from every rank, rank order

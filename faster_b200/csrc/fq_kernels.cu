@@ -617,13 +617,25 @@ size_t fq_bnb_node_bytes(int N, int force_final)
 #undef FQ_CASE
 }
 
+size_t fq_bnb_level_smem(int N, int force_final, int max_faces, int item_cap)
+{
+#define FQ_CASE(NN) case NN: return force_final ? fqb::level_smem<NN, true>(max_faces, item_cap) : fqb::level_smem<NN, false>(max_faces, item_cap);
+  switch (N)
+  {
+    FQ_CASE(4) FQ_CASE(5) FQ_CASE(6) FQ_CASE(7) FQ_CASE(8) FQ_CASE(9) FQ_CASE(10) FQ_CASE(11) FQ_CASE(12)
+    FQ_CASE(13) FQ_CASE(14) FQ_CASE(15) FQ_CASE(16)
+    default: return 0;
+  }
+#undef FQ_CASE
+}
+
 cudaError_t fq_launch_bnb_level(const FqBnbLevel& l, cudaStream_t stream)
 {
   fqb::BnbArgs b;
-  b.k = l.k; b.n_dt = l.n_dt; b.P = l.P; b.dts = l.dts; b.depth = l.depth; b.n_parents = l.n_parents;
+  b.k = l.k; b.n_dt = l.n_dt; b.dts = l.dts; b.depth = l.depth; b.cpc = l.cpc; b.n_parents = l.n_parents;
   b.parents = l.parents; b.roots = l.roots; b.children = l.children; b.n_children = l.n_children; b.cap = l.cap;
   b.incumbent = l.incumbent; b.leaves = (fqb::LeafRec*)l.leaves; b.n_leaves = l.n_leaves; b.leaf_cap = l.leaf_cap;
-  b.flags = l.flags;
+  b.flags = l.flags; b.nodes = l.nodes; b.keep_ties = l.keep_ties; b.lbound = l.lbound; b.closed = l.closed;
 #define FQ_CASE(NN) case NN: return l.k.force_final ? fqb::launch_level<NN, true>(b, stream) : fqb::launch_level<NN, false>(b, stream);
   switch (l.k.N)
   {
@@ -632,6 +644,41 @@ cudaError_t fq_launch_bnb_level(const FqBnbLevel& l, cudaStream_t stream)
     default: return cudaErrorInvalidConfiguration;
   }
 #undef FQ_CASE
+}
+
+cudaError_t fq_launch_bnb_roots(const FqBnbChainArgs& a, cudaStream_t stream)
+{
+  if (a.n_prob <= 0) return cudaSuccess;
+  fqb::fq_bnb_roots_kernel<<<(a.n_prob + 63) / 64, 64, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+
+cudaError_t fq_launch_bnb_certify(const FqBnbChainArgs& a, cudaStream_t stream)
+{
+  if (a.n_prob <= 0) return cudaSuccess;
+  fqb::fq_bnb_certify_kernel<<<(a.n_prob + 63) / 64, 64, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+
+cudaError_t fq_launch_bnb_resolve(const FqBnbChainArgs& a, cudaStream_t stream)
+{
+  if (a.n_prob <= 0) return cudaSuccess;
+  fqb::fq_bnb_resolve_kernel<<<(a.n_prob + 63) / 64, 64, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+
+cudaError_t fq_launch_bnb_fallback(const FqBnbChainArgs& a, const uint8_t* feasible, double* redo_dt, cudaStream_t stream)
+{
+  if (a.n_prob <= 0) return cudaSuccess;
+  fqb::fq_bnb_fallback_kernel<<<(a.n_prob + 63) / 64, 64, 0, stream>>>(a, feasible, redo_dt);
+  return cudaGetLastError();
+}
+
+cudaError_t fq_launch_bnb_adopt(int n_prob, int N, const double* redo_dt, const double* redo_coeffs, double* coeffs, cudaStream_t stream)
+{
+  if (n_prob <= 0) return cudaSuccess;
+  fqb::fq_bnb_adopt_kernel<<<n_prob, 128, 0, stream>>>(n_prob, N, redo_dt, redo_coeffs, coeffs);
+  return cudaGetLastError();
 }
 
 cudaError_t fq_launch_dtbase(int n_prob, int N, double DC, const double* x0, const double* xf, const double* lim,

@@ -98,26 +98,79 @@ cudaError_t fq_launch_solve(const FqKernelArgs& a, int max_cand_per_prob, cudaSt
 bool fq_has_specialised(int N, int force_final, int max_faces);
 cudaError_t fq_launch_select(const FqSelectArgs& a, cudaStream_t stream);
 
-// ---- branch-and-bound over assignments (fq_bnb.cuh)
+// ---- branch-and-bound over assignments (fq_bnb.cuh): corridor c of a level is problem c of k, with slices of its own
 struct FqBnbLevel
 {
-  FqKernelArgs k;                  // plan + ONE problem
-  int n_dt, P;
-  const double* dts;               // device
-  int depth, n_parents;
+  FqKernelArgs k;                  // plan + the corridors (k.n_prob)
+  int n_dt;                        // row length of dts / roots / incumbent
+  const double* dts;               // device, n_prob x n_dt
+  int depth, cpc;                  // cpc: CTAs per corridor
+  const int* n_parents;            // device, n_prob
   const unsigned char* parents;
   const int* roots;
   unsigned char* children;
-  int* n_children;
-  int cap;
+  int* n_children;                 // device, n_prob
+  int cap;                         // nodes per corridor
   unsigned long long* incumbent;
-  void* leaves;                    // fqb::LeafRec[leaf_cap]: {int dt_idx, pad; double cost; uchar sigma[16]}
+  void* leaves;                    // fqb::LeafRec[n_prob x leaf_cap]: {int dt_idx, corridor; double cost; uchar sigma[16]}
   int* n_leaves;
   int leaf_cap;
-  int* flags;
+  int* flags;                      // n_prob x 2
+  long long* nodes;                // n_prob, or nullptr
+  int keep_ties;
+  unsigned long long* lbound;      // keep_ties: n_prob x n_dt each (fq_bnb.cuh), or nullptr
+  unsigned char* closed;
 };
 size_t fq_bnb_node_bytes(int N, int force_final);     // 0 if unsupported
+// shared memory of a level launch for max_faces staged rows and item_cap rows per warp (0 if N is unsupported)
+size_t fq_bnb_level_smem(int N, int force_final, int max_faces, int item_cap);
 cudaError_t fq_launch_bnb_level(const FqBnbLevel& l, cudaStream_t stream);
+
+// the chained replan's exact stage (fq_replan_pairs_exact*): roots before the levels, resolve after them
+struct FqBnbChainArgs
+{
+  int n_prob, N, force_final, stride;   // stride: row length of dts / roots / incumbent (largest factor count)
+  int max_faces;                        // rows the level kernel stages (corridors with more get status 2)
+  int tree_ok;                          // 0: the level kernel has no instance for N (every tree corridor gets status 2)
+  long long all_limit;
+  const int *poly_ofs, *face_ofs;
+  const double *Ab, *x0, *xf;
+  double row_tol;
+  const int* cand_ofs;                  // the sweep's candidates: factor-major, |L_c| per factor
+  const double* cand_dt;
+  int n_fac;                            // factors per corridor, or per corridor n_fac_j[c]
+  const int* n_fac_j;
+  int* win_idx;                         // the list winners (fq_select_multi_kernel); resolve overwrites them
+  double *win_cost, *win_dt;
+  uint8_t* win_sig;
+  // tree state (ctx->d_bnb)
+  double* dts;
+  unsigned long long *incumbent, *lbound;
+  uint8_t* closed;
+  int* roots;
+  int* n_par;                           // 2 x n_prob: parent counts of even / odd levels
+  int* n_leaves;
+  int* flags;
+  long long* nodes;
+  const void* leaves;
+  int leaf_cap;
+  uint8_t* status;
+  uint8_t* changed;                     // out: the winner is the tree's
+  // the list winners, saved by the resolve before it overwrites win_* (restored where the tree's winner does not re-solve)
+  int* keep_idx;
+  double *keep_cost, *keep_dt;
+  uint8_t* keep_sig;
+  int* exact_out;                       // out, or nullptr
+  long long* nodes_out;                 // out, or nullptr
+};
+cudaError_t fq_launch_bnb_roots(const FqBnbChainArgs& a, cudaStream_t stream);
+cudaError_t fq_launch_bnb_certify(const FqBnbChainArgs& a, cudaStream_t stream);
+cudaError_t fq_launch_bnb_resolve(const FqBnbChainArgs& a, cudaStream_t stream);
+// after the winners' coefficient solve (feasible = its flags): a tree winner the solve did not confirm is replaced by the
+// list winner, whose dt goes to redo_dt (NaN elsewhere) for a second coefficient solve into redo_coeffs; adopt copies
+// those coefficients (n_prob x N x 12) where redo_dt is set
+cudaError_t fq_launch_bnb_fallback(const FqBnbChainArgs& a, const uint8_t* feasible, double* redo_dt, cudaStream_t stream);
+cudaError_t fq_launch_bnb_adopt(int n_prob, int N, const double* redo_dt, const double* redo_coeffs, double* coeffs, cudaStream_t stream);
 
 // ---- chained replan (fq_pair.cuh): the small kernels between the whole and the safe sweep
 struct FqSelectMultiArgs
@@ -166,6 +219,13 @@ struct FqPairFinalArgs
   // per-corridor windows (fq_replan_pairs_window*): corridor j's factor count, which then replaces n_fac_* in the split
   const int* n_fac_j_w = nullptr;
   const int* n_fac_j_s = nullptr;
+  // exact stage (fq_replan_pairs_exact*): corridors whose winner came from the tree get *_sigma_index = the rank of the
+  // winning assignment in L_j, or -1 when it is not in L_j
+  const uint8_t* changed_w = nullptr;
+  const uint8_t* changed_s = nullptr;
+  const int* poly_ofs_w = nullptr;
+  const int* poly_ofs_s = nullptr;
+  long long all_limit = 0;
 };
 
 // factor_*, trials_* and the next windows of fq_replan_pairs_window* (fq_window.h), from the result records

@@ -258,6 +258,16 @@ __global__ void fq_pair_final_kernel(const FqPairFinalArgs a)
   r.whole_sigma_index = ww >= 0 && lw > 0 ? ww % lw : -1;
   r.safe_dt_index = ws >= 0 && ls > 0 ? ws / ls : -1;
   r.safe_sigma_index = ws >= 0 && ls > 0 ? ws % ls : -1;
+  if (a.changed_w && a.changed_w[j])
+  {
+    const int P = a.poly_ofs_w[j + 1] - a.poly_ofs_w[j];
+    r.whole_sigma_index = (int)fqa::rank(a.N_w, P, fqa::use_all(a.N_w, P, a.all_limit), a.win_sig_w + (size_t)j * a.N_w);
+  }
+  if (a.changed_s && a.changed_s[j])
+  {
+    const int P = a.poly_ofs_s[j + 1] - a.poly_ofs_s[j];
+    r.safe_sigma_index = (int)fqa::rank(a.N_s, P, fqa::use_all(a.N_s, P, a.all_limit), a.win_sig_s + (size_t)j * a.N_s);
+  }
   if (a.sigma_out_w)
     for (int t = 0; t < a.N_w; t++) a.sigma_out_w[(size_t)j * a.N_w + t] = a.win_sig_w[(size_t)j * a.N_w + t];
   if (a.sigma_out_s)

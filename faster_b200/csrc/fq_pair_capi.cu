@@ -66,7 +66,89 @@ struct Lists
   int eew = 0, ees = 0;                 // candidates per time allocation (sizes an early-exit grid): the longest list
   const fq_pair_window* win = nullptr;  // per-corridor windows (device pointers; needs `as`), or nullptr
   int mfw = 0, mfs = 0;                 // with `win`: the factor rows' length (largest |F_j| allowed)
+  const fq_pair_exact* ex = nullptr;    // exact stage after each sweep's selection (device pointers; needs `as`), or nullptr
 };
+
+// Exact stage (fq_replan_pairs_exact*): node pools, leaves and per-corridor tree state, carved from ctx->d_bnb.  Corridor c
+// owns a slice of kTreeCap(n_prob) nodes in each of the two level pools (parents / children) and of kLeafCap leaves, so a
+// cut tree never takes room from another corridor.
+const int kLeafCap = 4096;
+inline int tree_cap(int n_prob) { return std::max(64, 65536 / std::max(n_prob, 1)); }
+struct Tree
+{
+  double* dts;
+  unsigned long long *incumbent, *lbound;
+  int *roots, *n_par, *n_leaves, *flags;
+  long long* nodes;
+  uint8_t *status, *changed_w, *changed_s, *closed;
+  int* keep_idx;                       // the list winners of the sweep in progress (fq_bnb_resolve_kernel)
+  double *keep_cost, *keep_dt, *redo_dt, *redo_coeffs;
+  uint8_t* keep_sig;
+  void* leaves;
+  unsigned char *pool0, *pool1;
+};
+
+size_t tree_layout(char* base, int n_prob, int stride, int max_N, size_t nb, Tree* t)
+{
+  char* p = base;
+  const size_t np = (size_t)n_prob, cells = np * (size_t)std::max(stride, 1);
+  t->dts = carve<double>(p, cells);  t->incumbent = carve<unsigned long long>(p, cells);  t->roots = carve<int>(p, cells);
+  t->lbound = carve<unsigned long long>(p, cells);  t->closed = carve<uint8_t>(p, cells);
+  t->keep_idx = carve<int>(p, np);  t->keep_cost = carve<double>(p, np);  t->keep_dt = carve<double>(p, np);
+  t->keep_sig = carve<uint8_t>(p, np * max_N);  t->redo_dt = carve<double>(p, np);  t->redo_coeffs = carve<double>(p, np * 12 * max_N);
+  t->n_par = carve<int>(p, 2 * np);  t->n_leaves = carve<int>(p, np);  t->flags = carve<int>(p, 2 * np);
+  t->nodes = carve<long long>(p, np);
+  t->status = carve<uint8_t>(p, np); t->changed_w = carve<uint8_t>(p, np);  t->changed_s = carve<uint8_t>(p, np);
+  t->leaves = carve<char>(p, np * kLeafCap * 32);
+  t->pool0 = carve<unsigned char>(p, np * tree_cap(n_prob) * nb);
+  t->pool1 = carve<unsigned char>(p, np * tree_cap(n_prob) * nb);
+  return (size_t)(p - base);
+}
+
+// One sweep's exact stage, enqueued on `st` after its selection: roots, N level launches (parent counts stay on the
+// device) and the resolve.  `k` holds the sweep's corridors, `c` its candidates and list winners.
+int exact_stage(fq_ctx* ctx, const Tree& t, FqKernelArgs k, FqBnbChainArgs& c, int max_poly_faces, uint8_t* changed,
+                cudaStream_t st)
+{
+  const int N = k.N, ff = k.force_final, n = k.n_prob;
+  c.n_prob = n; c.N = N; c.force_final = ff; c.poly_ofs = k.poly_ofs; c.face_ofs = k.face_ofs; c.Ab = k.Ab; c.x0 = k.x0;
+  c.xf = k.xf; c.row_tol = ctx->row_tol;
+  c.dts = t.dts; c.incumbent = t.incumbent; c.lbound = t.lbound; c.closed = t.closed;
+  c.keep_idx = t.keep_idx; c.keep_cost = t.keep_cost; c.keep_dt = t.keep_dt; c.keep_sig = t.keep_sig; c.roots = t.roots; c.n_par = t.n_par; c.n_leaves = t.n_leaves; c.flags = t.flags;
+  c.nodes = t.nodes; c.leaves = t.leaves; c.leaf_cap = kLeafCap; c.status = t.status; c.changed = changed;
+  // rows the level kernel stages: at most 2047 (the item encoding), shrunk until one CTA-wide copy fits in shared memory
+  int F = std::min(std::max(k.max_faces, 1), 2047);
+  auto items = [&](int f) { return N * std::min(max_poly_faces > 0 ? max_poly_faces : f, f); };
+  while (F > 1 && fq_bnb_level_smem(N, ff, F, items(F)) > 227 * 1024) F = F * 15 / 16;
+  c.tree_ok = fq_bnb_node_bytes(N, ff) != 0 && fq_bnb_level_smem(N, ff, F, items(F)) <= 227 * 1024;
+  c.max_faces = F;
+  FQ_CUDA(fq_launch_bnb_roots(c, st));
+  if (c.tree_ok)
+  {
+    FqPlanDev* pd = nullptr;
+    if (int rc = fq_get_plan(ctx, N, ff, &pd)) return rc;
+    FqBnbLevel L{};
+    L.k = k;
+    fq_fill_plan_args(*pd, &L.k);
+    L.k.max_faces = F; L.k.item_cap = items(F); L.k.row_tol = ctx->row_tol;
+    L.n_dt = c.stride; L.dts = t.dts; L.roots = t.roots; L.cap = tree_cap(n); L.incumbent = t.incumbent; L.leaves = t.leaves;
+    L.n_leaves = t.n_leaves; L.leaf_cap = kLeafCap; L.flags = t.flags; L.nodes = t.nodes; L.keep_ties = 1;
+    L.lbound = t.lbound; L.closed = t.closed;
+    L.cpc = std::max(1, (16 * std::max(ctx->sm_count, 1) + n - 1) / n);
+    unsigned char* pools[2] = { t.pool0, t.pool1 };
+    for (int depth = 0; depth < N; depth++)
+    {
+      L.depth = depth;
+      L.n_parents = t.n_par + (size_t)n * (depth & 1); L.n_children = t.n_par + (size_t)n * ((depth + 1) & 1);
+      L.parents = pools[depth & 1]; L.children = pools[(depth + 1) & 1];
+      FQ_CUDA(cudaMemsetAsync(L.n_children, 0, sizeof(int) * (size_t)n, st));
+      FQ_CUDA(fq_launch_bnb_level(L, st));
+      if (depth == 0) FQ_CUDA(fq_launch_bnb_certify(c, st));
+    }
+  }
+  FQ_CUDA(fq_launch_bnb_resolve(c, st));
+  return 0;
+}
 
 // largest |L(N, P, all_limit)| over P = 0 .. max_poly, or -1 when the list of max_poly polytopes is refused
 long long longest_list(int N, int max_poly, long long all_limit)
@@ -138,6 +220,14 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const Lists& l, fq_pair_result
     need = layout(nullptr);
     FQ_CUDA(ctx->d_pair.reserve(need));       // grows only on the first call / a larger batch (synchronous cudaMalloc)
     layout((char*)ctx->d_pair.p);
+    Tree tree{};
+    const int stride = std::max(l.win ? std::max(l.mfw, l.mfs) : std::max(a->n_fac_whole, a->n_fac_safe), 1);
+    if (l.ex)
+    { // the whole tree is done before the safe one starts: one pool serves both
+      const size_t nb = std::max(fq_bnb_node_bytes(Nw, 1), fq_bnb_node_bytes(Ns, 0));
+      FQ_CUDA(ctx->d_bnb.reserve(tree_layout(nullptr, P, stride, std::max(Nw, Ns), nb, &tree)));
+      tree_layout((char*)ctx->d_bnb.p, P, stride, std::max(Nw, Ns), nb, &tree);
+    }
 
     uint8_t* feas_w = a->feasible_whole ? a->feasible_whole : s.feas_w;
     uint8_t* feas_s = a->feasible_safe ? a->feasible_safe : s.feas_s;
@@ -189,11 +279,32 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const Lists& l, fq_pair_result
     sw.feasible = feas_w; sw.cost = cost_w; sw.win_idx = s.win_idx_w; sw.win_cost = s.win_cost_w; sw.win_dt = s.win_dt_w;
     sw.win_sigma = s.win_sig_w; sw.win_ofs = s.win_ofs;
     FQ_CUDA(fq_launch_select_multi(sw, st));
+    FqBnbChainArgs cx{};                                   // the exact stage's view of a sweep
+    // after a sweep's coefficient solve: tree winners it did not confirm go back to their list winners, whose
+    // coefficients a second solve of those corridors provides
+    auto confirm = [&](const FqKernelArgs& sweep, double* coeffs, int mpf) -> int {
+      FQ_CUDA(fq_launch_bnb_fallback(cx, s.re_feas, tree.redo_dt, st));
+      FqKernelArgs r = sweep;
+      r.cand_ofs = s.win_ofs; r.dt = tree.redo_dt; r.sigma = cx.win_sig; r.feasible = s.re_feas; r.cost = s.re_cost; r.coeffs = tree.redo_coeffs;
+      if (int e = fq_launch_solve_ctx(ctx, r, 1, mpf, st)) return e;
+      FQ_CUDA(fq_launch_bnb_adopt(P, sweep.N, tree.redo_dt, tree.redo_coeffs, coeffs, st));
+      return 0;
+    };
+    if (l.ex)
+    {
+      cx.stride = stride; cx.all_limit = l.as->all_limit; cx.cand_ofs = s.cand_ofs_w; cx.cand_dt = s.dt_w;
+      cx.n_fac = a->n_fac_whole; cx.n_fac_j = win ? s.nf_w : nullptr;
+      cx.win_idx = s.win_idx_w; cx.win_cost = s.win_cost_w; cx.win_dt = s.win_dt_w; cx.win_sig = s.win_sig_w;
+      cx.exact_out = l.ex->exact_whole; cx.nodes_out = l.ex->nodes_whole;
+      rc = exact_stage(ctx, tree, whole, cx, a->max_poly_faces_whole, tree.changed_w, st);
+      if (rc) return rc;
+    }
     // coefficients of the winners: one candidate per corridor through the same kernel (losers' dt is NaN -> "not solved")
     k = whole;
     k.cand_ofs = s.win_ofs; k.dt = s.win_dt_w; k.sigma = s.win_sig_w; k.feasible = s.re_feas; k.cost = s.re_cost; k.coeffs = coeffs_w;
     rc = fq_launch_solve_ctx(ctx, k, 1, a->max_poly_faces_whole, st);
     if (rc) return rc;
+    if (l.ex && (rc = confirm(whole, coeffs_w, a->max_poly_faces_whole))) return rc;
     // ---- R (faster.cpp:474-475) and the safe sweep from it (faster.cpp:521-527)
     FqPairMidArgs m;
     m.n_prob = P; m.N = Nw; m.DC = a->DC; m.r_fraction = a->r_fraction; m.coeffs = coeffs_w; m.win_dt = s.win_dt_w;
@@ -226,12 +337,21 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const Lists& l, fq_pair_result
     ss.N = Ns; ss.n_sig = a->n_sig_safe; ss.cand_ofs = s.cand_ofs_s; ss.dt = s.dt_s; ss.sigma = s.sig_s; ss.feasible = feas_s;
     ss.cost = cost_s; ss.win_idx = s.win_idx_s; ss.win_cost = s.win_cost_s; ss.win_dt = s.win_dt_s; ss.win_sigma = s.win_sig_s;
     FQ_CUDA(fq_launch_select_multi(ss, st));
-    if (a->coeffs_safe)
+    if (l.ex)
+    {
+      cx.cand_ofs = s.cand_ofs_s; cx.cand_dt = s.dt_s; cx.n_fac = a->n_fac_safe; cx.n_fac_j = win ? s.nf_s : nullptr;
+      cx.win_idx = s.win_idx_s; cx.win_cost = s.win_cost_s; cx.win_dt = s.win_dt_s; cx.win_sig = s.win_sig_s;
+      cx.exact_out = l.ex->exact_safe; cx.nodes_out = l.ex->nodes_safe;
+      rc = exact_stage(ctx, tree, safe, cx, a->max_poly_faces_safe, tree.changed_s, st);
+      if (rc) return rc;
+    }
+    if (a->coeffs_safe || l.ex)           // the exact stage re-solves its winners to confirm them, wanted or not
     {
       k = safe;
       k.cand_ofs = s.win_ofs; k.dt = s.win_dt_s; k.sigma = s.win_sig_s; k.feasible = s.re_feas; k.cost = s.re_cost; k.coeffs = coeffs_s;
       rc = fq_launch_solve_ctx(ctx, k, 1, a->max_poly_faces_safe, st);
       if (rc) return rc;
+      if (l.ex && (rc = confirm(safe, coeffs_s, a->max_poly_faces_safe))) return rc;
     }
     FqPairFinalArgs f;
     f.n_prob = P; f.n_sig_w = a->n_sig_whole; f.n_sig_s = a->n_sig_safe; f.win_idx_w = s.win_idx_w; f.win_idx_s = s.win_idx_s;
@@ -244,6 +364,11 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const Lists& l, fq_pair_result
       f.N_w = Nw; f.N_s = Ns; f.win_sig_w = s.win_sig_w; f.win_sig_s = s.win_sig_s;
       f.sigma_out_w = l.as->sigma_whole; f.sigma_out_s = l.as->sigma_safe;
       if (win) { f.n_fac_j_w = s.nf_w; f.n_fac_j_s = s.nf_s; }
+      if (l.ex)
+      {
+        f.changed_w = tree.changed_w; f.changed_s = tree.changed_s; f.poly_ofs_w = a->poly_ofs_whole; f.poly_ofs_s = a->poly_ofs_safe;
+        f.all_limit = l.as->all_limit;
+      }
       if (l.as->cand_ofs_whole)
         FQ_CUDA(cudaMemcpyAsync(l.as->cand_ofs_whole, s.cand_ofs_w, sizeof(int) * (size_t)(P + 1), cudaMemcpyDeviceToDevice, st));
       if (l.as->cand_ofs_safe)
@@ -291,9 +416,11 @@ extern "C" int fq_replan_pairs_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_r
   return run_chain(ctx, a, l, results_all, st);
 }
 
-// every pointer of `a` and of `as` is a device pointer; the sweeps' sizes come from the hints of `as`
-extern "C" int fq_replan_pairs_assign_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, fq_pair_result* results_all,
-                                          void* stream_v)
+namespace
+{
+// every pointer of `a` and of `as` (and `ex`) is a device pointer; the sweeps' sizes come from the hints of `as`
+int assign_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_exact* ex, fq_pair_result* results_all,
+               void* stream_v)
 {
   if (!ctx) return FQ_E_ARG;
   if (int rc = check_common(ctx, a, false)) return rc;
@@ -307,13 +434,14 @@ extern "C" int fq_replan_pairs_assign_dev(fq_ctx* ctx, const fq_pair_args* a, co
   l.ncw = (size_t)as->n_cand_whole; l.ncs = (size_t)as->n_cand_safe;
   l.mcw = (int)(lw * a->n_fac_whole); l.mcs = (int)(ls * a->n_fac_safe);
   l.eew = (int)lw; l.ees = (int)ls;
+  l.ex = ex;
   return run_chain(ctx, a, l, results_all, st);
 }
 
-// every pointer of `a`, `as` and `win` is a device pointer; the sweeps' sizes come from the hints of `as` (capacities) and
-// `win` (factor rows)
-extern "C" int fq_replan_pairs_window_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
-                                          fq_pair_result* results_all, void* stream_v)
+// every pointer of `a`, `as` and `win` (and `ex`) is a device pointer; the sweeps' sizes come from the hints of `as`
+// (capacities) and `win` (factor rows)
+int window_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex,
+               fq_pair_result* results_all, void* stream_v)
 {
   if (!ctx) return FQ_E_ARG;
   if (int rc = check_common(ctx, a, false, true)) return rc;
@@ -331,11 +459,34 @@ extern "C" int fq_replan_pairs_window_dev(fq_ctx* ctx, const fq_pair_args* a, co
   l.mfw = win->max_fac_whole; l.mfs = win->max_fac_safe;
   l.mcw = (int)std::max(1LL, lw * l.mfw); l.mcs = (int)std::max(1LL, ls * l.mfs);
   l.eew = (int)lw; l.ees = (int)ls;
+  l.ex = ex;
   return run_chain(ctx, a, l, results_all, st);
+}
+}  // namespace
+
+extern "C" int fq_replan_pairs_assign_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, fq_pair_result* results_all,
+                                          void* stream_v)
+{
+  return assign_dev(ctx, a, as, nullptr, results_all, stream_v);
+}
+
+extern "C" int fq_replan_pairs_window_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
+                                          fq_pair_result* results_all, void* stream_v)
+{
+  return window_dev(ctx, a, as, win, nullptr, results_all, stream_v);
+}
+
+extern "C" int fq_replan_pairs_exact_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
+                                         const fq_pair_exact* ex, fq_pair_result* results_all, void* stream_v)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (!ex) return fq_fail(ctx, FQ_E_ARG, "exact is NULL");
+  if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
+  return win ? window_dev(ctx, a, as, win, ex, results_all, stream_v) : assign_dev(ctx, a, as, ex, results_all, stream_v);
 }
 
 int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results,
-                            const fq_pair_assign* as, const fq_pair_window* win)
+                            const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex)
 {
   if (!ctx) return FQ_E_ARG;
   if (int rc = fq_settle(ctx)) return rc;
@@ -426,6 +577,8 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   if (as) { ocaw = put(4 * (size_t)(P + 1)); ocas = put(4 * (size_t)(P + 1)); osgw = put((size_t)P * Nw); osgs = put((size_t)P * Ns); }
   size_t ofac = 0, otri = 0, onext = 0;                 // windows: factor_* (2 P), trials_* (2 P), next_* (4 P)
   if (win) { ofac = put(8 * 2 * (size_t)P); otri = put(4 * 2 * (size_t)P); onext = put(8 * 4 * (size_t)P); }
+  size_t oex = 0, ond = 0;                              // exact stage: exact_* (2 P ints), nodes_* (2 P)
+  if (ex) { oex = put(4 * 2 * (size_t)P); ond = put(8 * 2 * (size_t)P); }
   const size_t out_bytes = o;
   FQ_CUDA(ctx->h_in.reserve(in_bytes));
   FQ_CUDA(ctx->d_pair_io.reserve(in_bytes + out_bytes));
@@ -485,7 +638,16 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
     dw.next_init_whole = win->next_init_whole ? no : nullptr;         dw.next_final_whole = win->next_final_whole ? no + P : nullptr;
     dw.next_init_safe = win->next_init_safe ? no + 2 * (size_t)P : nullptr; dw.next_final_safe = win->next_final_safe ? no + 3 * (size_t)P : nullptr;
   }
-  int rc = win ? fq_replan_pairs_window_dev(ctx, &d, &da, &dw, nullptr, st)
+  fq_pair_exact dx{};
+  if (ex)
+  {
+    int* eo = (int*)(dout + oex);
+    long long* no = (long long*)(dout + ond);
+    dx.exact_whole = ex->exact_whole ? eo : nullptr;  dx.exact_safe = ex->exact_safe ? eo + P : nullptr;
+    dx.nodes_whole = ex->nodes_whole ? no : nullptr;  dx.nodes_safe = ex->nodes_safe ? no + P : nullptr;
+  }
+  int rc = ex ? fq_replan_pairs_exact_dev(ctx, &d, &da, win ? &dw : nullptr, &dx, nullptr, st)
+         : win ? fq_replan_pairs_window_dev(ctx, &d, &da, &dw, nullptr, st)
          : as ? fq_replan_pairs_assign_dev(ctx, &d, &da, nullptr, st) : fq_replan_pairs_dev(ctx, &d, nullptr, st);
   if (rc) return rc;
   // ---- results straight into the caller's arrays (asynchronous when they are pinned)
@@ -519,6 +681,13 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
     FQ_CUDA(back(win->trials_whole, dw.trials_whole, 4));   FQ_CUDA(back(win->trials_safe, dw.trials_safe, 4));
     FQ_CUDA(back(win->next_init_whole, dw.next_init_whole, 8)); FQ_CUDA(back(win->next_final_whole, dw.next_final_whole, 8));
     FQ_CUDA(back(win->next_init_safe, dw.next_init_safe, 8));   FQ_CUDA(back(win->next_final_safe, dw.next_final_safe, 8));
+  }
+  if (ex)
+  {
+    if (ex->exact_whole) FQ_CUDA(cudaMemcpyAsync(ex->exact_whole, dx.exact_whole, 4 * (size_t)P, cudaMemcpyDeviceToHost, st));
+    if (ex->exact_safe) FQ_CUDA(cudaMemcpyAsync(ex->exact_safe, dx.exact_safe, 4 * (size_t)P, cudaMemcpyDeviceToHost, st));
+    if (ex->nodes_whole) FQ_CUDA(cudaMemcpyAsync(ex->nodes_whole, dx.nodes_whole, 8 * (size_t)P, cudaMemcpyDeviceToHost, st));
+    if (ex->nodes_safe) FQ_CUDA(cudaMemcpyAsync(ex->nodes_safe, dx.nodes_safe, 8 * (size_t)P, cudaMemcpyDeviceToHost, st));
   }
   if (deferred) { ctx->pending = true; return 0; }
   FQ_CUDA(cudaStreamSynchronize(st));
@@ -566,4 +735,30 @@ extern "C" int fq_replan_pairs_window_async(fq_ctx* ctx, const fq_pair_args* a, 
   if (!win) return fq_fail(ctx, FQ_E_ARG, "window is NULL");
   if (ctx->is_group || ctx->comm) return fq_replan_pairs_sharded(ctx, a, true, as, win);
   return fq_replan_pairs_host_ex(ctx, a, true, nullptr, true, as, win);
+}
+
+// host variants of the exact chain: one context on one GPU.  Gathering the per-corridor exact / nodes arrays of a
+// multi-GPU context would need a second exchange besides the records', so those contexts are refused.
+namespace
+{
+int exact_host(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex,
+               bool deferred)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (!ex) return fq_fail(ctx, FQ_E_ARG, "exact is NULL");
+  if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
+  if (ctx->is_group || ctx->comm) return fq_fail(ctx, FQ_E_ARG, "fq_replan_pairs_exact: multi-GPU contexts are not supported (use _exact_dev)");
+  return fq_replan_pairs_host_ex(ctx, a, deferred, nullptr, true, as, win, ex);
+}
+}  // namespace
+
+extern "C" int fq_replan_pairs_exact(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
+                                     const fq_pair_exact* ex)
+{
+  return exact_host(ctx, a, as, win, ex, false);
+}
+extern "C" int fq_replan_pairs_exact_async(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
+                                           const fq_pair_exact* ex)
+{
+  return exact_host(ctx, a, as, win, ex, true);
 }

@@ -337,6 +337,56 @@ int fq_replan_pairs_window_async(fq_ctx* ctx, const fq_pair_args* args, const fq
 int fq_replan_pairs_window_dev(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
                                fq_pair_result* results_all, void* stream);
 
+/* ---- chained replan with the exact MIQP optimum of every corridor ------------------------------------------------------
+ *
+ * SolverGurobi solves an MIQP over every binary b[t][p] (solverGurobi.cpp:217-246): at the first factor where ANY of the
+ * P^N assignments of segments to polytopes is feasible, the cheapest one.  The entry points below return that answer for
+ * every corridor of a batch, by branch-and-bound over all assignments on the device (fq_bnb.cuh), with no host round trip.
+ * `assign` is required and used as in fq_replan_pairs_assign; window == NULL takes the shared ascending factor lists of
+ * fq_pair_args (as _assign), a window the per-corridor windows of fq_replan_pairs_window (factor_*, trials_*, next_*
+ * included).  Feature "replan_pairs_exact".
+ *
+ * For corridor j and each sweep, with F_j its factors, L_j its list (all_limit still chooses it: the list is the pre-sweep
+ * whose winner seeds the tree) and f* the first factor at which L_j has a feasible candidate:
+ *   - the winner is at the first factor f <= f* at which ANY assignment is feasible (every factor of F_j without f*);
+ *   - at that factor it is the minimum-cost assignment.  The list winner is kept unless some assignment is cheaper by more
+ *     than a relative 1e-9, and then the records are byte for byte those of _assign / _window.  Otherwise the winner is
+ *     the lexicographically smallest assignment (base-P_j digits, segment 0 most significant) within a relative 1e-9 of the
+ *     minimum, so that exact ties of overlapping polytopes never depend on the order in which warps finish (whether a
+ *     slice near its capacity overflows can: DESIGN.md 3.2); its cost is the tree's evaluation of that assignment;
+ *   - corridors whose list already holds every assignment (P_j <= 1 or P_j^N <= all_limit) run no tree: exact 1, nodes 0;
+ *   - *_sigma_index is the winner's index in L_j, or -1 when it is not in L_j (then *_dt_index >= 0 tells it from "no
+ *     winner"); assign->sigma_* always holds the winning assignment;
+ *   - feasible_* / cost_* stay the list pre-sweep's per-candidate outputs;
+ *   - R, the safe sweep, the window update and the records follow the exact whole winner;
+ *   - exact_*[j] = 0: the corridor's tree was cut (its node or leaf slice filled up, or a node gave up at the iteration
+ *     cap), its faces exceed what the level kernel stages (2047, or less where shared memory runs out; DESIGN.md 3.4), or
+ *     the sweep's N has no tree kernel (N < 4), or the winners' coefficient solve rejected the tree's winner (a cold
+ *     solve can hit the iteration cap where the warm-started tree did not).  The corridor then gets its list winner,
+ *     byte-identical to _assign; the other corridors of the batch are unaffected.
+ * Each corridor owns max(64, 65536 / n_prob) nodes of each of two level pools and 4096 leaves in the context's device
+ * memory, which the context keeps until it is destroyed (at N = 10 and up to 1024 corridors about 1.3 GB with the
+ * arena's headroom; DESIGN.md 3.2). */
+typedef struct fq_pair_exact
+{
+  int *exact_whole, *exact_safe;        /* out n_prob, or NULL: 1 = the minimum over all P_j^N assignments, 0 = list winner kept (above) */
+  long long *nodes_whole, *nodes_safe;  /* out n_prob, or NULL: tree nodes the levels considered for the corridor   */
+} fq_pair_exact;
+
+/* HOST pointers everywhere; blocks until every output is in the caller's arrays.  FQ_E_ARG: exact or assign NULL, the
+ * refusals of _assign / _window, and multi-GPU contexts (gathering exact_* / nodes_* would need a second exchange). */
+int fq_replan_pairs_exact(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
+                          const fq_pair_exact* exact);
+/* The same, returning once everything is enqueued; outputs are valid after fq_wait(ctx).  Arrays must stay alive. */
+int fq_replan_pairs_exact_async(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
+                                const fq_pair_exact* exact);
+/* DEVICE pointers everywhere (the structs live on the host), with the hint and capacity rules of _assign_dev /
+ * _window_dev: a broken hint empties that sweep (exact 1, nodes 0, every winner "none"), nothing is written past the
+ * caller's arrays.  Never synchronises: the N level launches of a sweep read their parent counts on the device.  On a
+ * rank context the records are all-gathered into results_all as fq_replan_pairs_dev does. */
+int fq_replan_pairs_exact_dev(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
+                              const fq_pair_exact* exact, fq_pair_result* results_all, void* stream);
+
 /* ---- several GPUs behind the boundary (SURVEY.md 8b/8e) ---------------------------------------------------------
  *
  * Candidates of different corridors are independent, so a batch is sharded BY CORRIDOR: contiguous blocks of problems
