@@ -17,7 +17,8 @@ EXPORTS = ["fq_abi_version", "fq_create", "fq_destroy", "fq_last_error", "fq_set
            "fq_comm_info", "fq_allgather_dev", "fq_shard_range", "fq_solve_multi_sharded", "fq_solve_batch_cert", "fq_has_feature",
            "fq_pair_assign_count", "fq_replan_pairs_assign", "fq_replan_pairs_assign_async", "fq_replan_pairs_assign_dev",
            "fq_pair_window_factors", "fq_replan_pairs_window", "fq_replan_pairs_window_async", "fq_replan_pairs_window_dev",
-           "fq_replan_pairs_exact", "fq_replan_pairs_exact_async", "fq_replan_pairs_exact_dev"]
+           "fq_replan_pairs_exact", "fq_replan_pairs_exact_async", "fq_replan_pairs_exact_dev", "fq_replan_pairs_decomp",
+           "fq_replan_pairs_decomp_async", "fq_replan_pairs_decomp_dev"]
 
 
 class FqError(RuntimeError):
@@ -76,6 +77,18 @@ class PairExact(C.Structure):
     _fields_ = [("exact_whole", C.c_void_p), ("exact_safe", C.c_void_p), ("nodes_whole", C.c_void_p), ("nodes_safe", C.c_void_p)]
 
 
+class PairDecomp(C.Structure):
+    """fq_pair_decomp of include/faster_b200.h: paths and clouds in, the device-built corridors out."""
+    _fields_ = [("path_whole", C.c_void_p), ("path_safe", C.c_void_p), ("obs_ofs_whole", C.c_void_p), ("obs_ofs_safe", C.c_void_p),
+                ("obs_whole", C.c_void_p), ("obs_safe", C.c_void_p), ("goal", C.c_void_p), ("bbox", C.c_double * 3),
+                ("inflate", C.c_double), ("z_ground", C.c_double), ("max_obs_whole", C.c_int), ("max_obs_safe", C.c_int),
+                ("face_ofs_whole", C.c_void_p), ("face_ofs_safe", C.c_void_p), ("Ab_whole", C.c_void_p), ("Ab_safe", C.c_void_p),
+                ("E", C.c_void_p), ("M", C.c_void_p), ("status_whole", C.c_void_p), ("status_safe", C.c_void_p)]
+
+
+DECOMP_IN_KEYS = ["path_whole", "path_safe", "obs_ofs_whole", "obs_ofs_safe", "obs_whole", "obs_safe", "goal"]
+DECOMP_OUT_KEYS = ["face_ofs_whole", "face_ofs_safe", "Ab_whole", "Ab_safe", "E", "M", "status_whole", "status_safe"]
+DECOMP_STATUS = dict(ok=0, poly_faces=1, corridor_faces=2, cloud=3, zero_segment=4, not_run=5)   # FQ_DECOMP_*
 EXACT_KEYS = ["exact_whole", "exact_safe", "nodes_whole", "nodes_safe"]
 WINDOW_IN_KEYS = ["init_whole", "final_whole", "init_safe", "final_safe"]
 WINDOW_OUT_KEYS = ["factor_whole", "factor_safe", "trials_whole", "trials_safe", "next_init_whole", "next_final_whole",
@@ -137,6 +150,11 @@ def lib():
         L.fq_replan_pairs_exact_async.argtypes = L.fq_replan_pairs_exact.argtypes
         L.fq_replan_pairs_exact_dev.argtypes = [C.c_void_p, C.POINTER(PairArgs), C.POINTER(PairAssign), C.POINTER(PairWindow),
                                                 C.POINTER(PairExact), C.c_void_p, C.c_void_p]
+        L.fq_replan_pairs_decomp.argtypes = [C.c_void_p, C.POINTER(PairArgs), C.POINTER(PairAssign), C.POINTER(PairWindow),
+                                             C.POINTER(PairExact), C.POINTER(PairDecomp)]
+        L.fq_replan_pairs_decomp_async.argtypes = L.fq_replan_pairs_decomp.argtypes
+        L.fq_replan_pairs_decomp_dev.argtypes = [C.c_void_p, C.POINTER(PairArgs), C.POINTER(PairAssign), C.POINTER(PairWindow),
+                                                 C.POINTER(PairExact), C.POINTER(PairDecomp), C.c_void_p, C.c_void_p]
         L.fq_create_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_void_p]
         L.fq_comm_unique_id.argtypes = [C.c_void_p]
         L.fq_comm_init.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
@@ -247,6 +265,42 @@ def exact_args(out_ptrs):
     for k in EXACT_KEYS:
         setattr(s, k, out_ptrs.get(k) or None)
     return s
+
+
+def decomp_args(ptr, out_ptrs, bbox=(2.0, 2.0, 1.0), inflate=0.42, z_ground=0.0, max_obs_whole=0, max_obs_safe=0):
+    """PairDecomp; ptr(key) -> address of the input `key` (DECOMP_IN_KEYS; None = NULL), out_ptrs: addresses of
+    DECOMP_OUT_KEYS (0/None/missing = NULL).  The max_obs_* hints matter for the _dev entry only."""
+    s = PairDecomp()
+    for k in DECOMP_IN_KEYS:
+        setattr(s, k, ptr(k))
+    s.bbox = (C.c_double * 3)(*[float(x) for x in bbox])
+    s.inflate, s.z_ground = float(inflate), float(z_ground)
+    s.max_obs_whole, s.max_obs_safe = int(max_obs_whole), int(max_obs_safe)
+    for k in DECOMP_OUT_KEYS:
+        setattr(s, k, out_ptrs.get(k) or None)
+    return s
+
+
+def make_decomp_workload(pairs, max_faces=400, max_poly_faces=64):
+    """Packs corridor.forest_pair_paths dicts (one per corridor) into the host arrays of fq_pair_args (face_ofs_*, Ab_* and
+    xf_* absent: the chain makes them) and of fq_pair_decomp.  max_faces / max_poly_faces are the caps of both sweeps.
+    -> dict as make_pair_workload plus path_*, obs_ofs_*, obs_* (one cloud per corridor, the same arrays for both sweeps)
+    and goal."""
+    n = len(pairs)
+    out = dict(n_prob=n, N_whole=pairs[0]["N"], N_safe=pairs[0]["N"], DC=float(pairs[0]["DC"]), r_fraction=0.6,
+               x0=np.ascontiguousarray([p["x0"] for p in pairs], np.float64),
+               lim=np.ascontiguousarray([p["lim"] for p in pairs], np.float64),
+               goal=np.ascontiguousarray([p["goal"] for p in pairs], np.float64))
+    for kind in ("whole", "safe"):
+        paths = [np.asarray(p["path_" + kind], np.float64) for p in pairs]
+        out["poly_ofs_" + kind] = np.concatenate([[0], np.cumsum([len(x) - 1 for x in paths])]).astype(np.int32)
+        out["path_" + kind] = np.ascontiguousarray(np.vstack(paths))
+        out["max_faces_" + kind], out["max_poly_faces_" + kind] = int(max_faces), int(max_poly_faces)
+    obs = [np.asarray(p["obs"], np.float64).reshape(-1, 3) for p in pairs]
+    ofs = np.concatenate([[0], np.cumsum([len(o) for o in obs])]).astype(np.int32)
+    cloud = np.ascontiguousarray(np.vstack(obs)) if ofs[-1] else np.zeros((1, 3))
+    out.update(obs_ofs_whole=ofs, obs_ofs_safe=ofs, obs_whole=cloud, obs_safe=cloud)
+    return out
 
 
 def ellipsoid_decomp(path, obs, bbox=(2.0, 2.0, 1.0), inflate=0.42, z_ground=0.0, cap_rows=4096):
@@ -562,6 +616,68 @@ class Solver:
         fn = self._L.fq_replan_pairs_exact_async if deferred else self._L.fq_replan_pairs_exact
         self._check(fn(self._h, C.byref(a), C.byref(s), C.byref(wa) if wa is not None else None, C.byref(ex)))
         return out
+
+    def replan_pairs_decomp(self, w, all_limit=0, windows=None, inc=1.0, gamma=20.0, exact=False, bbox=(2.0, 2.0, 1.0),
+                            inflate=0.42, z_ground=0.0, use_goal=True, want_candidates=False, want_coeffs=True, deferred=False):
+        """fq_replan_pairs_decomp on a make_decomp_workload dict (host arrays) with its factors_whole / factors_safe (shared
+        factor lists) or `windows` (per-corridor windows, as replan_pairs_window); exact=True adds the exact stage.  -> the
+        dict of replan_pairs_assign (plus the window / exact outputs when asked for) and the corridors the sweeps used:
+        face_ofs_* / Ab_* (CSR), E, M (n_prob x 3) and status_whole / status_safe (FQ_DECOMP_*).  deferred: valid after wait()."""
+        n, Nw, Ns = w["n_prob"], w["N_whole"], w["N_safe"]
+        if windows is None:
+            offs = {kind: assign_offsets(w["poly_ofs_" + kind], w["N_" + kind], len(w["factors_" + kind]), all_limit)
+                    for kind in ("whole", "safe")}
+        else:
+            wins = {k: np.ascontiguousarray(windows[k], np.float64) for k in WINDOW_IN_KEYS}
+            incs = (inc, inc) if np.isscalar(inc) else tuple(inc)
+            offs = {}
+            for kind, ik in (("whole", incs[0]), ("safe", incs[1])):
+                nf = [len(window_factors(a, b, ik)) for a, b in zip(wins["init_" + kind], wins["final_" + kind])]
+                offs[kind] = window_offsets(w["poly_ofs_" + kind], w["N_" + kind], nf, all_limit)
+        out = dict(results=np.zeros(n, PAIR_RESULT_DTYPE), cand_ofs_whole=np.zeros(n + 1, np.int32), cand_ofs_safe=np.zeros(n + 1, np.int32),
+                   sigma_whole=np.zeros((n, Nw), np.uint8), sigma_safe=np.zeros((n, Ns), np.uint8),
+                   face_ofs_whole=np.zeros(int(w["poly_ofs_whole"][-1]) + 1, np.int32), face_ofs_safe=np.zeros(int(w["poly_ofs_safe"][-1]) + 1, np.int32),
+                   Ab_whole=np.zeros((n * w["max_faces_whole"], 4)), Ab_safe=np.zeros((n * w["max_faces_safe"], 4)),
+                   E=np.zeros((n, 3)), M=np.zeros((n, 3)), status_whole=np.zeros(n, np.int32), status_safe=np.zeros(n, np.int32))
+        if windows is not None:
+            out.update({k: (np.zeros(n, np.int32) if k.startswith("trials") else np.zeros(n)) for k in WINDOW_OUT_KEYS})
+        if exact:
+            out.update(exact_whole=np.zeros(n, np.int32), exact_safe=np.zeros(n, np.int32), nodes_whole=np.zeros(n, np.int64),
+                       nodes_safe=np.zeros(n, np.int64))
+        if want_candidates:
+            ncw, ncs = int(offs["whole"][-1]), int(offs["safe"][-1])
+            out.update(feasible_whole=np.zeros(ncw, np.uint8), cost_whole=np.zeros(ncw), feasible_safe=np.zeros(ncs, np.uint8),
+                       cost_safe=np.zeros(ncs))
+        if want_coeffs:
+            out.update(coeffs_whole=np.zeros((n, Nw, 12)), coeffs_safe=np.zeros((n, Ns, 12)))
+        a = PairArgs()
+        a.n_prob, a.N_whole, a.N_safe, a.DC, a.r_fraction = n, Nw, Ns, w["DC"], w["r_fraction"]
+        for k in ("x0", "lim", "poly_ofs_whole", "poly_ofs_safe"):
+            setattr(a, k, w[k].ctypes.data)
+        if windows is None:
+            a.factors_whole, a.factors_safe = w["factors_whole"].ctypes.data, w["factors_safe"].ctypes.data
+            a.n_fac_whole, a.n_fac_safe = len(w["factors_whole"]), len(w["factors_safe"])
+        for k in ("feasible_whole", "cost_whole", "feasible_safe", "cost_safe", "coeffs_whole", "coeffs_safe", "results"):
+            setattr(a, k, out[k].ctypes.data if k in out else None)
+        for k in ("max_faces_whole", "max_poly_faces_whole", "max_faces_safe", "max_poly_faces_safe"):
+            setattr(a, k, int(w[k]))
+        s = assign_args(all_limit, {k: out[k].ctypes.data for k in ("cand_ofs_whole", "cand_ofs_safe", "sigma_whole", "sigma_safe")})
+        wa = None if windows is None else window_args(lambda k: wins[k].ctypes.data, {k: out[k].ctypes.data for k in WINDOW_OUT_KEYS},
+                                                       inc, gamma)
+        ex = exact_args({k: out[k].ctypes.data for k in EXACT_KEYS}) if exact else None
+        dc = decomp_args(lambda k: None if (k == "goal" and not use_goal) else w[k].ctypes.data,
+                         {k: out[k].ctypes.data for k in DECOMP_OUT_KEYS}, bbox, inflate, z_ground)
+        fn = self._L.fq_replan_pairs_decomp_async if deferred else self._L.fq_replan_pairs_decomp
+        self._check(fn(self._h, C.byref(a), C.byref(s), C.byref(wa) if wa is not None else None, C.byref(ex) if ex is not None else None,
+                       C.byref(dc)))
+        return out
+
+    def replan_pairs_decomp_dev(self, a, s, win, ex, dc, results_all=0, stream=0):
+        """fq_replan_pairs_decomp_dev: `a`, `s`, `win` (PairWindow or None), `ex` (PairExact or None) and `dc` (PairDecomp)
+        hold device addresses and the host hints of the _assign_dev / _window_dev entries and dc.max_obs_*."""
+        self._check(self._L.fq_replan_pairs_decomp_dev(self._h, C.byref(a), C.byref(s), C.byref(win) if win is not None else None,
+                                                       C.byref(ex) if ex is not None else None, C.byref(dc), results_all or None,
+                                                       stream or None))
 
     def replan_pairs_exact_dev(self, a, s, win, ex, results_all=0, stream=0):
         """fq_replan_pairs_exact_dev: `a`, `s`, `win` (PairWindow or None) and `ex` (PairExact) hold device addresses and the

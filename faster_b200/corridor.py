@@ -341,6 +341,26 @@ def make_forest_pair_mixed(seed, N=10, max_poly_whole=3, max_poly_safe=4, Ra=4.0
     fewer too.  Nothing is padded.  -> (whole, safe) dicts as make_forest_pair_whole / make_forest_pair_safe."""
     from . import capi
     prof = UAV
+    p = forest_pair_paths(seed, N, max_poly_whole, max_poly_safe, Ra, r_fraction, n_trees, query, DC)
+    verts, spath, obs = p["path_whole"], p["path_safe"], p["obs"]
+    polys_w = capi.ellipsoid_decomp(verts, obs, prof["bbox"], prof["drone_radius"], prof["z_ground"], cap_rows=8192)
+    whole = dict(N=N, P=len(polys_w), x0=p["x0"], xf=p["xf_whole"], lim=p["lim"], polys=polys_w, force_final=True, DC=DC, verts=verts,
+                 verts_all=p["path_all"], obs=obs, seed=seed, profile="uav")
+    polys_s = capi.ellipsoid_decomp(spath, obs, prof["bbox"], prof["drone_radius"], prof["z_ground"], cap_rows=8192)
+    safe = dict(N=N, P=len(polys_s), x0=p["R_estimate"], xf=p["xf_safe"], lim=p["lim"].copy(), polys=polys_s, force_final=False, DC=DC,
+                verts=spath, seed=seed, profile="uav")
+    return whole, safe
+
+
+def forest_pair_paths(seed, N=10, max_poly_whole=3, max_poly_safe=4, Ra=4.0, r_fraction=0.6, n_trees=60, query=(0.6, 7.0), DC=0.01):
+    """The inputs of one replan of make_forest_pair_mixed before any decomposition, for the chain that decomposes on the
+    device (fq_replan_pairs_decomp*): the whole and safe paths, already trimmed by deleteVertexes; the occupied cells' centres
+    (one cloud serves both sweeps: the synthetic forest has no unknown space); the goal G (the JPS query's end); x0 and lim.
+    Vertex 0 of path_safe is the estimate of R that make_forest_pair_mixed cuts the safe corridor around (R_estimate, 9
+    doubles); the device replaces it with its own R.  xf_whole / xf_safe put E and M at the paths' last vertices, as
+    make_forest_pair_mixed does.  -> dict."""
+    from . import capi
+    prof = UAV
     rng = np.random.default_rng(seed)
     _, centres, radii = make_forest(seed, n_trees=n_trees)
     grid_jps, origin, res = voxelise_forest(centres, radii, inflation=0.47)
@@ -360,7 +380,6 @@ def make_forest_pair_mixed(seed, N=10, max_poly_whole=3, max_poly_safe=4, Ra=4.0
     path_all = split_long_segments(path, 1.5)
     verts = split_long_segments(clip_path_to_sphere(path, path[0], Ra), 1.5)[:max_poly_whole + 1]
     obs = (np.argwhere(grid > 0)[:, ::-1] + 0.5) * res + origin
-    polys_w = capi.ellipsoid_decomp(verts, obs, prof["bbox"], prof["drone_radius"], prof["z_ground"], cap_rows=8192)
     d0 = verts[1] - verts[0]
     d0 /= np.linalg.norm(d0)
     x0 = np.zeros(9)
@@ -369,8 +388,6 @@ def make_forest_pair_mixed(seed, N=10, max_poly_whole=3, max_poly_safe=4, Ra=4.0
     xf = np.zeros(9)
     xf[:3] = verts[-1]
     lim = np.array(prof["lim"])
-    whole = dict(N=N, P=len(polys_w), x0=x0, xf=xf, lim=lim, polys=polys_w, force_final=True, DC=DC, verts=verts,
-                 verts_all=path_all, obs=obs, seed=seed, profile="uav")
     # R estimate: r_fraction of the whole path's length; the safe path continues along the full path from there
     seg = np.linalg.norm(np.diff(verts, axis=0), axis=1)
     at = r_fraction * seg.sum()
@@ -382,14 +399,12 @@ def make_forest_pair_mixed(seed, N=10, max_poly_whole=3, max_poly_safe=4, Ra=4.0
     if len(rest) < 2:
         rest = [R, verts[-1] if np.linalg.norm(verts[-1] - R) > 1e-3 else R + 0.5 * d0]
     spath = split_long_segments(clip_path_to_sphere(np.array(rest), R, Ra), 1.5)[:max_poly_safe + 1]
-    polys_s = capi.ellipsoid_decomp(spath, obs, prof["bbox"], prof["drone_radius"], prof["z_ground"], cap_rows=8192)
     R9 = np.zeros(9)
     R9[:3] = R
     xfs = np.zeros(9)
     xfs[:3] = spath[-1]
-    safe = dict(N=N, P=len(polys_s), x0=R9, xf=xfs, lim=lim.copy(), polys=polys_s, force_final=False, DC=DC, verts=spath,
-                seed=seed, profile="uav")
-    return whole, safe
+    return dict(N=N, DC=DC, path_whole=np.asarray(verts, float), path_safe=np.asarray(spath, float), path_all=path_all, obs=obs,
+                goal=np.asarray(t, float), x0=x0, xf_whole=xf, xf_safe=xfs, lim=lim, R_estimate=R9, seed=seed, profile="uav")
 
 
 # ------------------------------------------------------------------------------------------------------------------

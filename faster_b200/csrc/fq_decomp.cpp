@@ -2,89 +2,19 @@
 // SolverGurobi::setPolytopes in the reference (JPS_Manager::cvxEllipsoidDecomp, faster/src/jps_manager.cpp:80-127, over
 // DecompUtil's EllipsoidDecomp3D: decomp_util/ellipsoid_decomp.h:96-123, line_segment.h:33-38,57-98,156-252,
 // decomp_base.h:39-46,83-115, decomp_geometry/ellipsoid.h:24-73, polyhedron.h:13-92,131-152).
-// Eigen-free restatement; it stays on the host (BASELINE north_star: "JPS3D and convex decomposition stay on host as
-// input generators").  The ellipsoid is kept as (Rf, axes) so that C^-1 = Rf diag(1/axes) Rf' is exact by construction.
+// Eigen-free restatement.  The ellipsoid is kept as (Rf, axes) so that C^-1 = Rf diag(1/axes) Rf' is exact by construction.
+// The arithmetic is fq_decomp.h, shared with the device kernel of the chained replan (fq_decomp.cuh); the loops, the
+// pre-filter and the vectorised distance pass below are the host's own.
 #include "../../include/faster_b200.h"
+
+#include "fq_decomp.h"
 
 #include <cmath>
 #include <vector>
 
 namespace
 {
-constexpr double kEps = 1e-10;   // decomp_basis/data_type.h:129
-
-struct V3
-{
-  double x, y, z;
-};
-inline V3 operator+(V3 a, V3 b) { return { a.x + b.x, a.y + b.y, a.z + b.z }; }
-inline V3 operator-(V3 a, V3 b) { return { a.x - b.x, a.y - b.y, a.z - b.z }; }
-inline V3 operator*(V3 a, double s) { return { a.x * s, a.y * s, a.z * s }; }
-inline double dot(V3 a, V3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
-inline double norm(V3 a) { return std::sqrt(dot(a, a)); }
-
-struct M3
-{
-  double m[3][3];
-};
-inline V3 mul(const M3& R, V3 v)
-{
-  return { R.m[0][0] * v.x + R.m[0][1] * v.y + R.m[0][2] * v.z, R.m[1][0] * v.x + R.m[1][1] * v.y + R.m[1][2] * v.z,
-           R.m[2][0] * v.x + R.m[2][1] * v.y + R.m[2][2] * v.z };
-}
-inline V3 mulT(const M3& R, V3 v)
-{
-  return { R.m[0][0] * v.x + R.m[1][0] * v.y + R.m[2][0] * v.z, R.m[0][1] * v.x + R.m[1][1] * v.y + R.m[2][1] * v.z,
-           R.m[0][2] * v.x + R.m[1][2] * v.y + R.m[2][2] * v.z };
-}
-inline M3 matmul(const M3& A, const M3& B)
-{
-  M3 C;
-  for (int i = 0; i < 3; i++)
-    for (int j = 0; j < 3; j++) C.m[i][j] = A.m[i][0] * B.m[0][j] + A.m[i][1] * B.m[1][j] + A.m[i][2] * B.m[2][j];
-  return C;
-}
-inline M3 rotx(double a)
-{
-  const double c = std::cos(a), s = std::sin(a);
-  return { { { 1, 0, 0 }, { 0, c, -s }, { 0, s, c } } };
-}
-inline M3 roty(double a)
-{
-  const double c = std::cos(a), s = std::sin(a);
-  return { { { c, 0, s }, { 0, 1, 0 }, { -s, 0, c } } };
-}
-inline M3 rotz(double a)
-{
-  const double c = std::cos(a), s = std::sin(a);
-  return { { { c, -s, 0 }, { s, c, 0 }, { 0, 0, 1 } } };
-}
-// geometric_utils.h:27-35: zero roll, R = Rz(yaw) Ry(pitch)
-inline M3 vec3_to_rotation(V3 v)
-{
-  const double pitch = std::atan2(-v.z, std::hypot(v.x, v.y)), yaw = std::atan2(v.y, v.x);
-  return matmul(rotz(yaw), roty(pitch));
-}
-inline double sgn(double v) { return (0.0 < v) - (v < 0.0); }
-
-struct Plane
-{
-  V3 p, n;
-};
-
-struct Ellip
-{
-  M3 Rf;
-  double ax[3];
-  V3 d;
-  // |C^-1 (pt - d)| with C = Rf diag(ax) Rf'   (ellipsoid.h:24-27)
-  double dist(V3 pt) const
-  {
-    const V3 q = mulT(Rf, pt - d);
-    const double a = q.x / ax[0], b = q.y / ax[1], c = q.z / ax[2];
-    return std::sqrt(a * a + b * b + c * c);
-  }
-};
+using namespace fqd;
 
 // E.dist for n points given as separate coordinate arrays: the same operations in the same order as Ellip::dist (packed
 // IEEE divisions and square roots round like the scalar ones; the avx2 clone has no FMA), four points per instruction
@@ -117,38 +47,6 @@ int closest(const Ellip& E, const std::vector<V3>& pts, const std::vector<int>& 
   return best;
 }
 
-void local_bbox(V3 p1, V3 p2, const double* bbox, Plane out[6])
-{ // line_segment.h:57-98
-  const V3 d = p2 - p1;
-  const V3 dir = d * (1.0 / norm(d));
-  V3 dir_h = { dir.y, -dir.x, 0.0 };
-  if (norm(dir_h) == 0) dir_h = { -1.0, 0.0, 0.0 };
-  dir_h = dir_h * (1.0 / norm(dir_h));
-  const V3 dir_v = { dir.y * dir_h.z - dir.z * dir_h.y, dir.z * dir_h.x - dir.x * dir_h.z, dir.x * dir_h.y - dir.y * dir_h.x };
-  out[0] = { p1 + dir_h * bbox[1], dir_h };
-  out[1] = { p1 - dir_h * bbox[1], dir_h * -1.0 };
-  out[2] = { p2 + dir * bbox[0], dir };
-  out[3] = { p1 - dir * bbox[0], dir * -1.0 };
-  out[4] = { p1 + dir_v * bbox[2], dir_v };
-  out[5] = { p1 - dir_v * bbox[2], dir_v * -1.0 };
-}
-
-// axis-aligned hull of the oriented box bb[0..5] of local_bbox (padded by 1e-6, far beyond the 1e-10 of the exact test)
-void bbox_aabb(V3 p1, const Plane bb[6], double lo[3], double hi[3])
-{
-  for (int k = 0; k < 3; k++) { lo[k] = 1e300; hi[k] = -1e300; }
-  for (int c = 0; c < 8; c++)
-  { // a corner adds to p1 the displacement of one face point of each opposite pair (the three axes are orthogonal)
-    const Plane& fh = bb[(c & 1) ? 0 : 1];
-    const Plane& fd = bb[(c & 2) ? 2 : 3];
-    const Plane& fv = bb[(c & 4) ? 4 : 5];
-    const V3 corner = p1 + (fh.p - p1) + (fd.p - p1) + (fv.p - p1);
-    const double cc[3] = { corner.x, corner.y, corner.z };
-    for (int k = 0; k < 3; k++) { lo[k] = std::fmin(lo[k], cc[k]); hi[k] = std::fmax(hi[k], cc[k]); }
-  }
-  for (int k = 0; k < 3; k++) { lo[k] -= 1e-6; hi[k] += 1e-6; }
-}
-
 void decompose_segment(V3 p1, V3 p2, const double* obs, int n_obs, const double* bbox, double inflate, std::vector<Plane>* planes)
 {
   Plane bb[6];
@@ -162,23 +60,16 @@ void decompose_segment(V3 p1, V3 p2, const double* obs, int n_obs, const double*
   for (int i = 0; i < n_obs; i++)
   {
     const double x = obs[3 * i], y = obs[3 * i + 1], z = obs[3 * i + 2];
-    if (x < lo[0] || x > hi[0] || y < lo[1] || y > hi[1] || z < lo[2] || z > hi[2]) continue;
+    if (outside_aabb(lo, hi, x, y, z)) continue;
     const V3 pt = { x, y, z };
-    bool in = true;
-    for (int k = 0; k < 6 && in; k++) in = !(dot(bb[k].n, pt - bb[k].p) > kEps);
-    if (in) O.push_back(pt);
+    if (inside_bbox(bb, pt)) O.push_back(pt);
   }
   // find_ellipsoid(0)  (line_segment.h:156-252)
-  const double f = norm(p1 - p2) / 2;
-  const M3 Ri = vec3_to_rotation(p2 - p1);
+  double f;
+  M3 Ri;
   Ellip E;
-  E.Rf = Ri; E.ax[0] = E.ax[1] = E.ax[2] = f; E.d = (p1 + p2) * 0.5;
-  for (V3& it : O)
-  { // obstacle inflation in the ellipsoid frame (:178-190), in place: the polyhedron below sees the inflated points
-    V3 p = mulT(Ri, it - E.d);
-    p = { p.x - sgn(p.x) * inflate, p.y - sgn(p.y) * inflate, p.z - sgn(p.z) * inflate };
-    it = mul(Ri, p) + E.d;
-  }
+  ellipsoid_start(p1, p2, &E, &Ri, &f);
+  for (V3& it : O) it = inflate_point(Ri, E.d, it, inflate);   // in place: the polyhedron below sees the inflated points
   // coordinate arrays of the (inflated) points for the two passes that evaluate the distance of EVERY point
   const int nO = (int)O.size();
   std::vector<double> soa((size_t)4 * nO);
@@ -191,16 +82,10 @@ void decompose_segment(V3 p1, V3 p2, const double* obs, int n_obs, const double*
   cur = inside0;
   while (!cur.empty())
   { // shrink the two short axes together (:195-217)
-    const V3 pw = O[closest(E, O, cur)];
-    V3 p = mulT(Ri, pw - E.d);
-    const double roll = std::atan2(p.z, p.y);
-    E.Rf = matmul(Ri, rotx(roll));
-    p = mulT(E.Rf, pw - E.d);
-    if (p.x < E.ax[0]) E.ax[1] = std::fabs(p.y) / std::sqrt(1 - (p.x / E.ax[0]) * (p.x / E.ax[0]));
-    E.ax[2] = E.ax[1];
+    shrink_short_axes(&E, Ri, O[closest(E, O, cur)]);
     std::vector<int> nxt;
     for (int i : cur)
-      if (1 - E.dist(O[i]) > kEps) nxt.push_back(i);
+      if (still_inside(E, O[i])) nxt.push_back(i);
     cur.swap(nxt);
   }
   E.ax[2] = f;   // reset with the old axes(2) (:219-224)
@@ -209,13 +94,10 @@ void decompose_segment(V3 p1, V3 p2, const double* obs, int n_obs, const double*
     if (E.dist(O[i]) <= 1) cur.push_back(i);
   while (!cur.empty())
   { // shrink the third axis (:226-247)
-    const V3 pw = O[closest(E, O, cur)];
-    const V3 p = mulT(E.Rf, pw - E.d);
-    const double dd = 1 - (p.x / E.ax[0]) * (p.x / E.ax[0]) - (p.y / E.ax[1]) * (p.y / E.ax[1]);
-    if (dd > kEps) E.ax[2] = std::fabs(p.z) / std::sqrt(dd);
+    shrink_third_axis(&E, O[closest(E, O, cur)]);
     std::vector<int> nxt;
     for (int i : cur)
-      if (1 - E.dist(O[i]) > kEps) nxt.push_back(i);
+      if (still_inside(E, O[i])) nxt.push_back(i);
     cur.swap(nxt);
   }
   // find_polyhedron (decomp_base.h:83-115): tangent half-spaces at successive closest points
@@ -231,15 +113,11 @@ void decompose_segment(V3 p1, V3 p2, const double* obs, int n_obs, const double*
     for (int i : remain)
       if (dist_of[i] < bd) { bd = dist_of[i]; best = i; }     // first strict minimum, as closest()
     const V3 cp = O[best];
-    // n = C^-1 C^-T (cp - d) = Rf diag(1/ax^2) Rf' (cp - d), normalised  (ellipsoid.h:65-73)
-    V3 q = mulT(E.Rf, cp - E.d);
-    q = { q.x / (E.ax[0] * E.ax[0]), q.y / (E.ax[1] * E.ax[1]), q.z / (E.ax[2] * E.ax[2]) };
-    V3 n = mul(E.Rf, q);
-    n = n * (1.0 / norm(n));
+    const V3 n = tangent_normal(E, cp);
     planes->push_back({ cp, n });
     std::vector<int> nxt;
     for (int i : remain)
-      if (dot(n, O[i] - cp) < 0) nxt.push_back(i);
+      if (before_plane(n, cp, O[i])) nxt.push_back(i);
     remain.swap(nxt);
   }
   for (int k = 0; k < 6; k++) planes->push_back(bb[k]);   // add_local_bbox (line_segment.h:33-38)
@@ -261,7 +139,7 @@ extern "C" int fq_ellipsoid_decomp(const double* path, int n_seg, const double* 
     for (int s = 0; s < n_seg; s++)
     {
       const V3 p1 = { path[3 * s], path[3 * s + 1], path[3 * s + 2] }, p2 = { path[3 * s + 3], path[3 * s + 4], path[3 * s + 5] };
-      if (norm(p2 - p1) == 0) return FQ_E_ARG;
+      if (norm(sub(p2, p1)) == 0) return FQ_E_ARG;
       Plane bb[6];
       double lo[3], hi[3];
       local_bbox(p1, p2, bbox, bb);
@@ -272,7 +150,7 @@ extern "C" int fq_ellipsoid_decomp(const double* path, int n_seg, const double* 
     for (int i = 0; i < n_obs; i++)
     {
       const double x = obs[3 * i], y = obs[3 * i + 1], z = obs[3 * i + 2];
-      if (x < ulo[0] || x > uhi[0] || y < ulo[1] || y > uhi[1] || z < ulo[2] || z > uhi[2]) continue;
+      if (outside_aabb(ulo, uhi, x, y, z)) continue;
       near_pts.push_back(x); near_pts.push_back(y); near_pts.push_back(z);      // order preserved
     }
     obs = near_pts.data();
@@ -282,21 +160,13 @@ extern "C" int fq_ellipsoid_decomp(const double* path, int n_seg, const double* 
   for (int s = 0; s < n_seg; s++)
   {
     const V3 p1 = { path[3 * s], path[3 * s + 1], path[3 * s + 2] }, p2 = { path[3 * s + 3], path[3 * s + 4], path[3 * s + 5] };
-    if (norm(p2 - p1) == 0) return FQ_E_ARG;
+    if (norm(sub(p2, p1)) == 0) return FQ_E_ARG;
     planes.clear();
     decompose_segment(p1, p2, obs, n_obs, bbox, inflate, &planes);
     if (rows + (int)planes.size() + 1 > cap_rows) return FQ_E_NOMEM;
-    const V3 mid = (p1 + p2) * 0.5;
-    for (const Plane& pl : planes)
-    { // LinearConstraint3D(pt_inside, hyperplanes): A x <= b with the segment midpoint inside (polyhedron.h:131-152)
-      V3 n = pl.n;
-      double c = dot(pl.p, n);
-      if (dot(n, mid) - c > 0) { n = n * -1.0; c = -c; }
-      double* r = Ab + (size_t)4 * rows++;
-      r[0] = n.x; r[1] = n.y; r[2] = n.z; r[3] = c;
-    }
-    double* g = Ab + (size_t)4 * rows++;                  // ground face (jps_manager.cpp:118-122)
-    g[0] = 0; g[1] = 0; g[2] = -1; g[3] = -z_ground;
+    const V3 mid = scale(add(p1, p2), 0.5);
+    for (const Plane& pl : planes) oriented_row(pl, mid, Ab + (size_t)4 * rows++);
+    ground_row(z_ground, Ab + (size_t)4 * rows++);
     face_ofs[s + 1] = rows;
   }
   return rows;

@@ -539,6 +539,7 @@ __global__ void __launch_bounds__(256) fq_fill_kernel(const FqFillArgs a)
 #include "fq_kernels_t.cuh"
 #include "fq_bnb.cuh"
 #include "fq_pair.cuh"
+#include "fq_decomp.cuh"
 
 size_t fq_solve_smem_bytes(const FqKernelArgs& a)
 {
@@ -769,5 +770,15 @@ cudaError_t fq_launch_pair_final(const FqPairFinalArgs& a, cudaStream_t stream)
 {
   if (a.n_prob <= 0) return cudaSuccess;
   fqp::fq_pair_final_kernel<<<(a.n_prob + 127) / 128, 128, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+
+size_t fq_decomp_spill_n(int max_obs) { return max_obs > fqd::kFitPts ? (size_t)(max_obs - fqd::kFitPts) : 0; }
+
+cudaError_t fq_launch_decomp(const FqDecompArgs& a, cudaStream_t stream)
+{
+  if (a.n_prob <= 0) return cudaSuccess;
+  if (a.max_poly > 0) fqd::fq_decomp_kernel<<<a.n_prob * a.max_poly, fqd::kThreads, 0, stream>>>(a);
+  fqd::fq_decomp_csr_kernel<<<1, 1024, 0, stream>>>(a);
   return cudaGetLastError();
 }

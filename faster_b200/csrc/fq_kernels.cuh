@@ -243,6 +243,37 @@ struct FqPairWindowArgs
   double *next_init_w, *next_final_w, *next_init_s, *next_final_s;   // out, or NULL; may alias init_* / final_*
 };
 
+// the device decomposition of one sweep's corridors (fq_decomp.cuh): fq_decomp_kernel stages every polytope's rows in a slot
+// of cap_pf rows (slot j * max_poly + s), fq_decomp_csr_kernel packs them into the sweep's CSR and sets the final states
+struct FqDecompArgs
+{
+  int n_prob, max_poly;
+  const int* poly_ofs;                  // n_prob + 1: P_j
+  const double* path;                   // corridor j: rows poly_ofs[j] + j .. poly_ofs[j+1] + j
+  const double* first;                  // NULL, or n_prob x 9: vertex 0 of corridor j is first[9 j .. 9 j + 2] (R; NaN: not run)
+  const int* obs_ofs;                   // n_prob + 1
+  const double* obs;
+  int max_obs;                          // clouds above it are refused; sizes the spill slices
+  double bbox[3], inflate, z_ground;
+  int cap_pf;                           // staged rows per polytope: the max_poly_faces cap
+  int max_faces;                        // the corridor cap
+  double* stage;                        // n_prob x max_poly x cap_pf x 4
+  int* stage_n;                         // n_prob x max_poly: rows, or -FQ_DECOMP_* status
+  double* spill;                        // n_prob x max_poly x spill_n x 4 (x, y, z, dist of survivors kFitPts and beyond)
+  uint8_t* spill_flag;                  // n_prob x max_poly x spill_n
+  int spill_n;                          // max(max_obs - kFitPts, 0)
+  // fq_decomp_csr_kernel
+  const double* goal;                   // n_prob x 3, or NULL
+  int face_cap;                         // face_ofs has face_cap + 1 entries (n_prob x max_poly)
+  int* face_ofs;                        // out: absolute CSR over poly_ofs
+  double* Ab;                           // out: n_prob x max_faces rows of 4
+  double* xf;                           // out: n_prob x 9 final states (NaN rows for failed corridors)
+  double* pos_out;                      // out n_prob x 3, or NULL
+  int* status;                          // out n_prob, or NULL
+};
+size_t fq_decomp_spill_n(int max_obs);
+cudaError_t fq_launch_decomp(const FqDecompArgs& a, cudaStream_t stream);
+
 cudaError_t fq_launch_dtbase(int n_prob, int N, double DC, const double* x0, const double* xf, const double* lim,
                              double* dt_base, cudaStream_t stream);
 cudaError_t fq_launch_expand_grid(int n_prob, int N, int n_fac, int n_sig, const double* factors, const uint8_t* sig_list,

@@ -19,6 +19,10 @@ struct Scratch
   int *cand_ofs_w, *cand_ofs_s, *win_idx_w, *win_idx_s, *win_ofs, *n_samples, *k_safe;
   double *fac_w, *fac_s;                // per-corridor windows: n_prob x max_fac factor rows
   int *nf_w, *nf_s;                     // and |F_j| (-1: refused)
+  // decomposing chain: both sweeps' staging and spill (used one sweep after the other), the corridors, the final states
+  double *dc_stage, *dc_spill, *dc_Ab_w, *dc_Ab_s, *dc_xf_w, *dc_xf_s;
+  int *dc_stage_n, *dc_face_w, *dc_face_s;
+  uint8_t* dc_spill_flag;
 };
 
 template <class T>
@@ -30,8 +34,9 @@ T* carve(char*& p, size_t count)
 }
 
 // shared = false: per-corridor lists (fq_replan_pairs_assign*), whose candidate counts the callers check themselves;
-// windows = true (with shared = false): per-corridor windows (fq_replan_pairs_window*), no factor list in `a`
-int check_common(fq_ctx* ctx, const fq_pair_args* a, bool shared = true, bool windows = false)
+// windows = true (with shared = false): per-corridor windows (fq_replan_pairs_window*), no factor list in `a`;
+// decomp = true: the chain decomposes the corridors (fq_replan_pairs_decomp*), so `a` has no faces and no final states
+int check_common(fq_ctx* ctx, const fq_pair_args* a, bool shared = true, bool windows = false, bool decomp = false)
 {
   if (!a) return fq_fail(ctx, FQ_E_ARG, "args is NULL");
   if (a->n_prob <= 0) return fq_fail(ctx, FQ_E_ARG, "n_prob <= 0");
@@ -50,8 +55,12 @@ int check_common(fq_ctx* ctx, const fq_pair_args* a, bool shared = true, bool wi
   if (shared &&
       ((long long)a->n_prob * a->n_fac_whole * a->n_sig_whole > (1LL << 30) || (long long)a->n_prob * a->n_fac_safe * a->n_sig_safe > (1LL << 30)))
     return fq_fail(ctx, FQ_E_ARG, "too many candidates");
-  if (!a->x0 || !a->xf_whole || !a->xf_safe || !a->lim || !a->poly_ofs_whole || !a->face_ofs_whole || !a->poly_ofs_safe ||
-      !a->face_ofs_safe || (!windows && (!a->factors_whole || !a->factors_safe)) || !a->results)
+  if (decomp && (a->face_ofs_whole || a->face_ofs_safe || a->Ab_whole || a->Ab_safe || a->xf_whole || a->xf_safe))
+    return fq_fail(ctx, FQ_E_ARG, "decomposing chain: face_ofs_*, Ab_* and xf_* must be NULL (the chain makes them)");
+  if (decomp && (a->max_faces_whole <= 0 || a->max_faces_safe <= 0 || a->max_poly_faces_whole <= 0 || a->max_poly_faces_safe <= 0))
+    return fq_fail(ctx, FQ_E_ARG, "decomposing chain: max_faces_* and max_poly_faces_* are caps and must be > 0");
+  if (!a->x0 || (!decomp && (!a->xf_whole || !a->xf_safe || !a->face_ofs_whole || !a->face_ofs_safe)) || !a->lim || !a->poly_ofs_whole ||
+      !a->poly_ofs_safe || (!windows && (!a->factors_whole || !a->factors_safe)) || !a->results)
     return fq_fail(ctx, FQ_E_ARG, "NULL argument");
   return 0;
 }
@@ -67,7 +76,21 @@ struct Lists
   const fq_pair_window* win = nullptr;  // per-corridor windows (device pointers; needs `as`), or nullptr
   int mfw = 0, mfs = 0;                 // with `win`: the factor rows' length (largest |F_j| allowed)
   const fq_pair_exact* ex = nullptr;    // exact stage after each sweep's selection (device pointers; needs `as`), or nullptr
+  const fq_pair_decomp* dc = nullptr;   // the chain decomposes the corridors (device pointers; needs `as`), or nullptr
 };
+
+// the checks of fq_pair_decomp that need no device memory
+const char* check_decomp_scalars(const fq_pair_decomp* d)
+{
+  if (!d) return "decomp is NULL";
+  if (!d->path_whole || !d->path_safe || !d->obs_ofs_whole || !d->obs_ofs_safe || !d->obs_whole || !d->obs_safe)
+    return "decomp: path_* / obs_ofs_* / obs_* must not be NULL";
+  for (int k = 0; k < 3; k++)
+    if (!std::isfinite(d->bbox[k]) || !(d->bbox[k] > 0)) return "decomp: bbox must be finite and > 0";
+  if (!std::isfinite(d->inflate) || d->inflate < 0 || !std::isfinite(d->z_ground)) return "decomp: inflate must be finite and >= 0, z_ground finite";
+  if (((uintptr_t)d->Ab_whole & 15) || ((uintptr_t)d->Ab_safe & 15)) return "decomp: Ab_* must be 16-byte aligned";
+  return nullptr;
+}
 
 // Exact stage (fq_replan_pairs_exact*): node pools, leaves and per-corridor tree state, carved from ctx->d_bnb.  Corridor c
 // owns a slice of kTreeCap(n_prob) nodes in each of the two level pools (parents / children) and of kLeafCap leaves, so a
@@ -193,6 +216,14 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const Lists& l, fq_pair_result
   const size_t ncw = l.ncw, ncs = l.ncs;
   // ---- scratch
   size_t need = 0;
+  // decomposing chain: staging slots of both sweeps (the larger), rows per slot, spilled survivors per slot
+  size_t dslots = 0, dcap = 0, dspill = 0;
+  if (l.dc)
+  {
+    dslots = (size_t)P * std::max(l.as->max_poly_whole, l.as->max_poly_safe);
+    dcap = (size_t)std::max(a->max_poly_faces_whole, a->max_poly_faces_safe);
+    dspill = fq_decomp_spill_n(std::max(l.dc->max_obs_whole, l.dc->max_obs_safe));
+  }
   {
     char* p = nullptr;
     Scratch s;
@@ -215,6 +246,13 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const Lists& l, fq_pair_result
       s.feas_w = carve<uint8_t>(p, ncw);       s.feas_s = carve<uint8_t>(p, ncs);   s.re_feas = carve<uint8_t>(p, P);
       s.fac_w = carve<double>(p, l.win ? (size_t)P * l.mfw : 0);  s.fac_s = carve<double>(p, l.win ? (size_t)P * l.mfs : 0);
       s.nf_w = carve<int>(p, l.win ? P : 0);   s.nf_s = carve<int>(p, l.win ? P : 0);
+      s.dc_stage = carve<double>(p, dslots * dcap * 4);     s.dc_stage_n = carve<int>(p, dslots);
+      s.dc_spill = carve<double>(p, dslots * dspill * 4);   s.dc_spill_flag = carve<uint8_t>(p, dslots * dspill);
+      s.dc_Ab_w = carve<double>(p, l.dc && !l.dc->Ab_whole ? (size_t)P * a->max_faces_whole * 4 : 0);
+      s.dc_Ab_s = carve<double>(p, l.dc && !l.dc->Ab_safe ? (size_t)P * a->max_faces_safe * 4 : 0);
+      s.dc_face_w = carve<int>(p, l.dc && !l.dc->face_ofs_whole ? (size_t)P * l.as->max_poly_whole + 1 : 0);
+      s.dc_face_s = carve<int>(p, l.dc && !l.dc->face_ofs_safe ? (size_t)P * l.as->max_poly_safe + 1 : 0);
+      s.dc_xf_w = carve<double>(p, l.dc ? (size_t)9 * P : 0);  s.dc_xf_s = carve<double>(p, l.dc ? (size_t)9 * P : 0);
       return (size_t)(p - base);
     };
     need = layout(nullptr);
@@ -242,6 +280,31 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const Lists& l, fq_pair_result
     whole.poly_ofs = a->poly_ofs_whole; whole.face_ofs = a->face_ofs_whole; whole.Ab = a->Ab_whole; whole.max_faces = a->max_faces_whole;
     safe.N = Ns; safe.force_final = 0; safe.n_prob = P; safe.x0 = s.x0_safe; safe.xf = a->xf_safe; safe.lim = a->lim;
     safe.poly_ofs = a->poly_ofs_safe; safe.face_ofs = a->face_ofs_safe; safe.Ab = a->Ab_safe; safe.max_faces = a->max_faces_safe;
+    // decomposing chain (faster.cpp:393-403 whole, :485-504 safe): one sweep's corridors from its paths and clouds, into
+    // the caller's outputs or the scratch; the final states go to the scratch
+    auto decompose = [&](bool is_whole, FqKernelArgs* sweep) -> cudaError_t {
+      const fq_pair_decomp* d = l.dc;
+      FqDecompArgs x{};
+      x.n_prob = P; x.max_poly = is_whole ? l.as->max_poly_whole : l.as->max_poly_safe;
+      x.poly_ofs = is_whole ? a->poly_ofs_whole : a->poly_ofs_safe;
+      x.path = is_whole ? d->path_whole : d->path_safe;
+      x.first = is_whole ? nullptr : s.x0_safe;
+      x.obs_ofs = is_whole ? d->obs_ofs_whole : d->obs_ofs_safe; x.obs = is_whole ? d->obs_whole : d->obs_safe;
+      x.max_obs = is_whole ? d->max_obs_whole : d->max_obs_safe;
+      for (int k = 0; k < 3; k++) x.bbox[k] = d->bbox[k];
+      x.inflate = d->inflate; x.z_ground = d->z_ground;
+      x.cap_pf = is_whole ? a->max_poly_faces_whole : a->max_poly_faces_safe;
+      x.max_faces = is_whole ? a->max_faces_whole : a->max_faces_safe;
+      x.stage = s.dc_stage; x.stage_n = s.dc_stage_n; x.spill = s.dc_spill; x.spill_flag = s.dc_spill_flag; x.spill_n = (int)dspill;
+      x.goal = d->goal; x.face_cap = P * x.max_poly;
+      x.face_ofs = is_whole ? (d->face_ofs_whole ? d->face_ofs_whole : s.dc_face_w) : (d->face_ofs_safe ? d->face_ofs_safe : s.dc_face_s);
+      x.Ab = is_whole ? (d->Ab_whole ? d->Ab_whole : s.dc_Ab_w) : (d->Ab_safe ? d->Ab_safe : s.dc_Ab_s);
+      x.xf = is_whole ? s.dc_xf_w : s.dc_xf_s;
+      x.pos_out = is_whole ? d->E : d->M;
+      x.status = is_whole ? d->status_whole : d->status_safe;
+      sweep->face_ofs = x.face_ofs; sweep->Ab = x.Ab; sweep->xf = x.xf;
+      return fq_launch_decomp(x, st);
+    };
 
     // ---- per-corridor windows: every window is read here, before anything is written (the outputs may alias them)
     const fq_pair_window* win = l.win;
@@ -250,8 +313,9 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const Lists& l, fq_pair_result
       FQ_CUDA(fq_launch_window_factors(P, l.mfw, win->init_whole, win->final_whole, win->inc_whole, s.fac_w, s.nf_w, st));
       FQ_CUDA(fq_launch_window_factors(P, l.mfs, win->init_safe, win->final_safe, win->inc_safe, s.fac_s, s.nf_s, st));
     }
-    // ---- whole sweep (faster.cpp:406-418)
-    FQ_CUDA(fq_launch_dtbase(P, Nw, a->DC, a->x0, a->xf_whole, a->lim, s.dt_base_w, st));
+    // ---- whole sweep (faster.cpp:406-418); a decomposing chain first makes its corridors and E (which getDTInitial reads)
+    if (l.dc) FQ_CUDA(decompose(true, &whole));
+    FQ_CUDA(fq_launch_dtbase(P, Nw, a->DC, a->x0, whole.xf, a->lim, s.dt_base_w, st));
     if (!l.as)
       FQ_CUDA(fq_launch_expand_grid(P, Nw, a->n_fac_whole, a->n_sig_whole, a->factors_whole, a->sigmas_whole, s.dt_base_w, s.dt_w,
                                     s.sig_w, s.cand_ofs_w, st));
@@ -310,7 +374,8 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const Lists& l, fq_pair_result
     m.n_prob = P; m.N = Nw; m.DC = a->DC; m.r_fraction = a->r_fraction; m.coeffs = coeffs_w; m.win_dt = s.win_dt_w;
     m.win_idx = s.win_idx_w; m.x0_safe = s.x0_safe; m.n_samples = s.n_samples; m.k_safe = s.k_safe;
     FQ_CUDA(fq_launch_pair_mid(m, st));
-    FQ_CUDA(fq_launch_dtbase(P, Ns, a->DC, s.x0_safe, a->xf_safe, a->lim, s.dt_base_s, st));
+    if (l.dc) FQ_CUDA(decompose(false, &safe));            // the safe corridors around R, and M
+    FQ_CUDA(fq_launch_dtbase(P, Ns, a->DC, s.x0_safe, safe.xf, a->lim, s.dt_base_s, st));
     if (!l.as)
       FQ_CUDA(fq_launch_expand_grid(P, Ns, a->n_fac_safe, a->n_sig_safe, a->factors_safe, a->sigmas_safe, s.dt_base_s, s.dt_s,
                                     s.sig_s, s.cand_ofs_s, st));
@@ -420,10 +485,10 @@ namespace
 {
 // every pointer of `a` and of `as` (and `ex`) is a device pointer; the sweeps' sizes come from the hints of `as`
 int assign_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_exact* ex, fq_pair_result* results_all,
-               void* stream_v)
+               void* stream_v, const fq_pair_decomp* dc = nullptr)
 {
   if (!ctx) return FQ_E_ARG;
-  if (int rc = check_common(ctx, a, false)) return rc;
+  if (int rc = check_common(ctx, a, false, false, dc != nullptr)) return rc;
   long long lw = 0, ls = 0;
   if (int rc = check_assign_hints(ctx, a, as, &lw, &ls)) return rc;
   if (lw * a->n_fac_whole > (1LL << 30) || ls * a->n_fac_safe > (1LL << 30)) return fq_fail(ctx, FQ_E_ARG, "too many candidates");
@@ -434,17 +499,17 @@ int assign_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, con
   l.ncw = (size_t)as->n_cand_whole; l.ncs = (size_t)as->n_cand_safe;
   l.mcw = (int)(lw * a->n_fac_whole); l.mcs = (int)(ls * a->n_fac_safe);
   l.eew = (int)lw; l.ees = (int)ls;
-  l.ex = ex;
+  l.ex = ex; l.dc = dc;
   return run_chain(ctx, a, l, results_all, st);
 }
 
 // every pointer of `a`, `as` and `win` (and `ex`) is a device pointer; the sweeps' sizes come from the hints of `as`
 // (capacities) and `win` (factor rows)
 int window_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex,
-               fq_pair_result* results_all, void* stream_v)
+               fq_pair_result* results_all, void* stream_v, const fq_pair_decomp* dc = nullptr)
 {
   if (!ctx) return FQ_E_ARG;
-  if (int rc = check_common(ctx, a, false, true)) return rc;
+  if (int rc = check_common(ctx, a, false, true, dc != nullptr)) return rc;
   if (const char* why = check_window_scalars(win)) return fq_fail(ctx, FQ_E_ARG, why);
   if (win->max_fac_whole < 0 || win->max_fac_whole > fqw::kMaxFactors || win->max_fac_safe < 0 || win->max_fac_safe > fqw::kMaxFactors)
     return fq_fail(ctx, FQ_E_ARG, "max_fac_* out of range (0..4096)");
@@ -459,7 +524,7 @@ int window_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, con
   l.mfw = win->max_fac_whole; l.mfs = win->max_fac_safe;
   l.mcw = (int)std::max(1LL, lw * l.mfw); l.mcs = (int)std::max(1LL, ls * l.mfs);
   l.eew = (int)lw; l.ees = (int)ls;
-  l.ex = ex;
+  l.ex = ex; l.dc = dc;
   return run_chain(ctx, a, l, results_all, st);
 }
 }  // namespace
@@ -485,13 +550,25 @@ extern "C" int fq_replan_pairs_exact_dev(fq_ctx* ctx, const fq_pair_args* a, con
   return win ? window_dev(ctx, a, as, win, ex, results_all, stream_v) : assign_dev(ctx, a, as, ex, results_all, stream_v);
 }
 
+extern "C" int fq_replan_pairs_decomp_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
+                                          const fq_pair_exact* ex, const fq_pair_decomp* dc, fq_pair_result* results_all, void* stream_v)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
+  if (const char* why = check_decomp_scalars(dc)) return fq_fail(ctx, FQ_E_ARG, why);
+  if (dc->max_obs_whole < 0 || dc->max_obs_safe < 0) return fq_fail(ctx, FQ_E_ARG, "decomp: max_obs_* < 0");
+  return win ? window_dev(ctx, a, as, win, ex, results_all, stream_v, dc) : assign_dev(ctx, a, as, ex, results_all, stream_v, dc);
+}
+
 int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results,
-                            const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex)
+                            const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex, const fq_pair_decomp* dc)
 {
   if (!ctx) return FQ_E_ARG;
   if (int rc = fq_settle(ctx)) return rc;
-  if (win && !as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
-  if (int rc = check_common(ctx, a, as == nullptr, win != nullptr)) return rc;
+  if ((win || dc) && !as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
+  if (int rc = check_common(ctx, a, as == nullptr, win != nullptr, dc != nullptr)) return rc;
+  if (dc)
+    if (const char* why = check_decomp_scalars(dc)) return fq_fail(ctx, FQ_E_ARG, why);
   if (win)
     if (const char* why = check_window_scalars(win)) return fq_fail(ctx, FQ_E_ARG, why);
   const int P = a->n_prob, Nw = a->N_whole, Ns = a->N_safe;
@@ -504,9 +581,37 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
     return nullptr;
   };
   FqCorridorSizes cw, cs;
-  if (const char* why = check(a->poly_ofs_whole, a->face_ofs_whole, a->Ab_whole, &cw)) return fq_fail(ctx, FQ_E_ARG, why);
-  if (const char* why = check(a->poly_ofs_safe, a->face_ofs_safe, a->Ab_safe, &cs)) return fq_fail(ctx, FQ_E_ARG, why);
-  if (!fq_scan_all_finite(a->x0, 9 * (size_t)P) || !fq_scan_all_finite(a->xf_whole, 9 * (size_t)P) || !fq_scan_all_finite(a->xf_safe, 9 * (size_t)P))
+  int n_obs_w = 0, n_obs_s = 0, max_obs_w = 0, max_obs_s = 0;   // decomposing chain: the clouds
+  if (!dc)
+  {
+    if (const char* why = check(a->poly_ofs_whole, a->face_ofs_whole, a->Ab_whole, &cw)) return fq_fail(ctx, FQ_E_ARG, why);
+    if (const char* why = check(a->poly_ofs_safe, a->face_ofs_safe, a->Ab_safe, &cs)) return fq_fail(ctx, FQ_E_ARG, why);
+  }
+  else
+  { // polytope counts, paths, clouds and the goal
+    auto ofs = [&](const int* o, int max_step, int* total, int* largest) -> bool {
+      if (o[0] != 0) return false;
+      for (int j = 0; j < P; j++)
+      {
+        const int d = o[j + 1] - o[j];
+        if (d < 0 || d > max_step) return false;
+        *largest = std::max(*largest, d);
+      }
+      *total = o[P];
+      return true;
+    };
+    int mp = 0;
+    if (!ofs(a->poly_ofs_whole, FQ_MAX_POLY, &cw.n_poly, &mp) || !ofs(a->poly_ofs_safe, FQ_MAX_POLY, &cs.n_poly, &mp))
+      return fq_fail(ctx, FQ_E_ARG, "poly_ofs_* must start at 0 and step by 0..FQ_MAX_POLY");
+    if (!ofs(dc->obs_ofs_whole, 1 << 30, &n_obs_w, &max_obs_w) || !ofs(dc->obs_ofs_safe, 1 << 30, &n_obs_s, &max_obs_s))
+      return fq_fail(ctx, FQ_E_ARG, "decomp: obs_ofs_* must start at 0 and be non-decreasing");
+    if (!fq_scan_all_finite(dc->path_whole, 3 * (size_t)(cw.n_poly + P)) || !fq_scan_all_finite(dc->path_safe, 3 * (size_t)(cs.n_poly + P)) ||
+        !fq_scan_all_finite(dc->obs_whole, 3 * (size_t)n_obs_w) || !fq_scan_all_finite(dc->obs_safe, 3 * (size_t)n_obs_s) ||
+        (dc->goal && !fq_scan_all_finite(dc->goal, 3 * (size_t)P)))
+      return fq_fail(ctx, FQ_E_ARG, "decomp: non-finite value in a path, a cloud or the goal");
+  }
+  if (!fq_scan_all_finite(a->x0, 9 * (size_t)P) ||
+      (!dc && (!fq_scan_all_finite(a->xf_whole, 9 * (size_t)P) || !fq_scan_all_finite(a->xf_safe, 9 * (size_t)P))))
     return fq_fail(ctx, FQ_E_ARG, "non-finite value in x0/xf");
   if (!fq_scan_all_positive_finite(a->lim, 3 * (size_t)P) || !fq_scan_all_positive_finite(a->factors_whole, (size_t)a->n_fac_whole) ||
       !fq_scan_all_positive_finite(a->factors_safe, (size_t)a->n_fac_safe))
@@ -568,6 +673,13 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   const size_t opos = put(4 * (size_t)(P + 1)), ofos = put(4 * (size_t)(cs.n_poly + 1));
   const size_t osw = put((size_t)a->n_sig_whole * Nw), oss = put((size_t)a->n_sig_safe * Ns);
   const size_t owin = win ? put(8 * 4 * (size_t)P) : 0;   // init_whole, final_whole, init_safe, final_safe
+  size_t opaw = 0, opas = 0, ooow = 0, ooos = 0, oobw = 0, oobs = 0, ogoal = 0;   // decomposing chain: paths, clouds, goal
+  if (dc)
+  {
+    opaw = put(24 * (size_t)(cw.n_poly + P)); opas = put(24 * (size_t)(cs.n_poly + P));
+    ooow = put(4 * (size_t)(P + 1)); ooos = put(4 * (size_t)(P + 1));
+    oobw = put(24 * (size_t)n_obs_w); oobs = put(24 * (size_t)n_obs_s); ogoal = put(24 * (size_t)P);
+  }
   const size_t in_bytes = o;
   o = 0;
   const size_t ores = put(sizeof(fq_pair_result) * (size_t)P);
@@ -579,6 +691,13 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   if (win) { ofac = put(8 * 2 * (size_t)P); otri = put(4 * 2 * (size_t)P); onext = put(8 * 4 * (size_t)P); }
   size_t oex = 0, ond = 0;                              // exact stage: exact_* (2 P ints), nodes_* (2 P)
   if (ex) { oex = put(4 * 2 * (size_t)P); ond = put(8 * 2 * (size_t)P); }
+  size_t odfw = 0, odfs = 0, odaw = 0, odas = 0, oE = 0, oM = 0, ostw = 0, osts = 0;   // decomposing chain: its outputs
+  if (dc)
+  {
+    odfw = put(4 * (size_t)(cw.n_poly + 1)); odfs = put(4 * (size_t)(cs.n_poly + 1));
+    odaw = put(32 * (size_t)P * a->max_faces_whole); odas = put(32 * (size_t)P * a->max_faces_safe);
+    oE = put(24 * (size_t)P); oM = put(24 * (size_t)P); ostw = put(4 * (size_t)P); osts = put(4 * (size_t)P);
+  }
   const size_t out_bytes = o;
   FQ_CUDA(ctx->h_in.reserve(in_bytes));
   FQ_CUDA(ctx->d_pair_io.reserve(in_bytes + out_bytes));
@@ -587,8 +706,16 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   char* dout = din + in_bytes;
   if (cw.n_face) std::memcpy(hi + oAbw, a->Ab_whole, 32 * (size_t)cw.n_face);
   if (cs.n_face) std::memcpy(hi + oAbs, a->Ab_safe, 32 * (size_t)cs.n_face);
-  std::memcpy(hi + ox0, a->x0, 72 * (size_t)P);      std::memcpy(hi + oxfw, a->xf_whole, 72 * (size_t)P);
-  std::memcpy(hi + oxfs, a->xf_safe, 72 * (size_t)P); std::memcpy(hi + olim, a->lim, 24 * (size_t)P);
+  std::memcpy(hi + ox0, a->x0, 72 * (size_t)P);      std::memcpy(hi + olim, a->lim, 24 * (size_t)P);
+  if (!dc) { std::memcpy(hi + oxfw, a->xf_whole, 72 * (size_t)P); std::memcpy(hi + oxfs, a->xf_safe, 72 * (size_t)P); }
+  else
+  {
+    std::memcpy(hi + opaw, dc->path_whole, 24 * (size_t)(cw.n_poly + P)); std::memcpy(hi + opas, dc->path_safe, 24 * (size_t)(cs.n_poly + P));
+    std::memcpy(hi + ooow, dc->obs_ofs_whole, 4 * (size_t)(P + 1));       std::memcpy(hi + ooos, dc->obs_ofs_safe, 4 * (size_t)(P + 1));
+    if (n_obs_w) std::memcpy(hi + oobw, dc->obs_whole, 24 * (size_t)n_obs_w);
+    if (n_obs_s) std::memcpy(hi + oobs, dc->obs_safe, 24 * (size_t)n_obs_s);
+    if (dc->goal) std::memcpy(hi + ogoal, dc->goal, 24 * (size_t)P);
+  }
   if (a->n_fac_whole) std::memcpy(hi + ofw, a->factors_whole, 8 * (size_t)a->n_fac_whole);
   if (a->n_fac_safe) std::memcpy(hi + ofs, a->factors_safe, 8 * (size_t)a->n_fac_safe);
   if (win)
@@ -596,8 +723,11 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
     const double* w4[4] = { win->init_whole, win->final_whole, win->init_safe, win->final_safe };
     for (int i = 0; i < 4; i++) std::memcpy(hi + owin + 8 * (size_t)P * i, w4[i], 8 * (size_t)P);
   }
-  std::memcpy(hi + opow, a->poly_ofs_whole, 4 * (size_t)(P + 1)); std::memcpy(hi + ofow, a->face_ofs_whole, 4 * (size_t)(cw.n_poly + 1));
-  std::memcpy(hi + opos, a->poly_ofs_safe, 4 * (size_t)(P + 1));  std::memcpy(hi + ofos, a->face_ofs_safe, 4 * (size_t)(cs.n_poly + 1));
+  std::memcpy(hi + opow, a->poly_ofs_whole, 4 * (size_t)(P + 1)); std::memcpy(hi + opos, a->poly_ofs_safe, 4 * (size_t)(P + 1));
+  if (!dc)
+  {
+    std::memcpy(hi + ofow, a->face_ofs_whole, 4 * (size_t)(cw.n_poly + 1)); std::memcpy(hi + ofos, a->face_ofs_safe, 4 * (size_t)(cs.n_poly + 1));
+  }
   if (a->sigmas_whole) std::memcpy(hi + osw, a->sigmas_whole, (size_t)a->n_sig_whole * Nw);
   if (a->sigmas_safe) std::memcpy(hi + oss, a->sigmas_safe, (size_t)a->n_sig_safe * Ns);
   cudaStream_t st = ctx->stream;
@@ -615,7 +745,14 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   d.feasible_safe = a->feasible_safe ? (uint8_t*)(dout + ofes) : nullptr;   d.cost_safe = a->cost_safe ? (double*)(dout + ocs) : nullptr;
   d.coeffs_whole = a->coeffs_whole ? (double*)(dout + ocow) : nullptr;       d.coeffs_safe = a->coeffs_safe ? (double*)(dout + ocos) : nullptr;
   d.results = (fq_pair_result*)(dout + ores);
-  d.max_faces_whole = std::max(cw.max_faces, 1); d.max_poly_faces_whole = cw.max_poly_faces; d.max_faces_safe = std::max(cs.max_faces, 1); d.max_poly_faces_safe = cs.max_poly_faces;
+  if (!dc)
+  {
+    d.max_faces_whole = std::max(cw.max_faces, 1); d.max_poly_faces_whole = cw.max_poly_faces; d.max_faces_safe = std::max(cs.max_faces, 1); d.max_poly_faces_safe = cs.max_poly_faces;
+  }
+  else
+  { // the chain makes the corridors and final states; max_*faces_* stay the caller's caps
+    d.xf_whole = d.xf_safe = nullptr; d.face_ofs_whole = d.face_ofs_safe = nullptr; d.Ab_whole = d.Ab_safe = nullptr;
+  }
   // a NULL cost/flag output still needs a device array of its own kind: the chain allocates it in its scratch
   if ((d.feasible_whole == nullptr) != (d.cost_whole == nullptr) || (d.feasible_safe == nullptr) != (d.cost_safe == nullptr))
     return fq_fail(ctx, FQ_E_ARG, "feasible_* and cost_* must be given (or omitted) together");
@@ -646,7 +783,21 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
     dx.exact_whole = ex->exact_whole ? eo : nullptr;  dx.exact_safe = ex->exact_safe ? eo + P : nullptr;
     dx.nodes_whole = ex->nodes_whole ? no : nullptr;  dx.nodes_safe = ex->nodes_safe ? no + P : nullptr;
   }
-  int rc = ex ? fq_replan_pairs_exact_dev(ctx, &d, &da, win ? &dw : nullptr, &dx, nullptr, st)
+  fq_pair_decomp dd{};
+  if (dc)
+  {
+    dd = *dc;
+    dd.path_whole = (const double*)(din + opaw); dd.path_safe = (const double*)(din + opas);
+    dd.obs_ofs_whole = (const int*)(din + ooow); dd.obs_ofs_safe = (const int*)(din + ooos);
+    dd.obs_whole = (const double*)(din + oobw); dd.obs_safe = (const double*)(din + oobs);
+    dd.goal = dc->goal ? (const double*)(din + ogoal) : nullptr;
+    dd.max_obs_whole = max_obs_w; dd.max_obs_safe = max_obs_s;
+    dd.face_ofs_whole = (int*)(dout + odfw); dd.face_ofs_safe = (int*)(dout + odfs);
+    dd.Ab_whole = (double*)(dout + odaw); dd.Ab_safe = (double*)(dout + odas);
+    dd.E = (double*)(dout + oE); dd.M = (double*)(dout + oM); dd.status_whole = (int*)(dout + ostw); dd.status_safe = (int*)(dout + osts);
+  }
+  int rc = dc ? fq_replan_pairs_decomp_dev(ctx, &d, &da, win ? &dw : nullptr, ex ? &dx : nullptr, &dd, nullptr, st)
+         : ex ? fq_replan_pairs_exact_dev(ctx, &d, &da, win ? &dw : nullptr, &dx, nullptr, st)
          : win ? fq_replan_pairs_window_dev(ctx, &d, &da, &dw, nullptr, st)
          : as ? fq_replan_pairs_assign_dev(ctx, &d, &da, nullptr, st) : fq_replan_pairs_dev(ctx, &d, nullptr, st);
   if (rc) return rc;
@@ -688,6 +839,16 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
     if (ex->exact_safe) FQ_CUDA(cudaMemcpyAsync(ex->exact_safe, dx.exact_safe, 4 * (size_t)P, cudaMemcpyDeviceToHost, st));
     if (ex->nodes_whole) FQ_CUDA(cudaMemcpyAsync(ex->nodes_whole, dx.nodes_whole, 8 * (size_t)P, cudaMemcpyDeviceToHost, st));
     if (ex->nodes_safe) FQ_CUDA(cudaMemcpyAsync(ex->nodes_safe, dx.nodes_safe, 8 * (size_t)P, cudaMemcpyDeviceToHost, st));
+  }
+  if (dc)
+  {
+    auto back = [&](void* host, const void* dev, size_t bytes) { return host ? cudaMemcpyAsync(host, dev, bytes, cudaMemcpyDeviceToHost, st) : cudaSuccess; };
+    FQ_CUDA(back(dc->face_ofs_whole, dd.face_ofs_whole, 4 * (size_t)(cw.n_poly + 1)));
+    FQ_CUDA(back(dc->face_ofs_safe, dd.face_ofs_safe, 4 * (size_t)(cs.n_poly + 1)));
+    FQ_CUDA(back(dc->Ab_whole, dd.Ab_whole, 32 * (size_t)P * a->max_faces_whole));
+    FQ_CUDA(back(dc->Ab_safe, dd.Ab_safe, 32 * (size_t)P * a->max_faces_safe));
+    FQ_CUDA(back(dc->E, dd.E, 24 * (size_t)P));                   FQ_CUDA(back(dc->M, dd.M, 24 * (size_t)P));
+    FQ_CUDA(back(dc->status_whole, dd.status_whole, 4 * (size_t)P)); FQ_CUDA(back(dc->status_safe, dd.status_safe, 4 * (size_t)P));
   }
   if (deferred) { ctx->pending = true; return 0; }
   FQ_CUDA(cudaStreamSynchronize(st));
@@ -761,4 +922,29 @@ extern "C" int fq_replan_pairs_exact_async(fq_ctx* ctx, const fq_pair_args* a, c
                                            const fq_pair_exact* ex)
 {
   return exact_host(ctx, a, as, win, ex, true);
+}
+
+// host variants of the decomposing chain: one context on one GPU, as the exact chain's
+namespace
+{
+int decomp_host(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex,
+                const fq_pair_decomp* dc, bool deferred)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (!dc) return fq_fail(ctx, FQ_E_ARG, "decomp is NULL");
+  if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
+  if (ctx->is_group || ctx->comm) return fq_fail(ctx, FQ_E_ARG, "fq_replan_pairs_decomp: multi-GPU contexts are not supported (use _decomp_dev)");
+  return fq_replan_pairs_host_ex(ctx, a, deferred, nullptr, true, as, win, ex, dc);
+}
+}  // namespace
+
+extern "C" int fq_replan_pairs_decomp(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
+                                      const fq_pair_exact* ex, const fq_pair_decomp* dc)
+{
+  return decomp_host(ctx, a, as, win, ex, dc, false);
+}
+extern "C" int fq_replan_pairs_decomp_async(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
+                                            const fq_pair_exact* ex, const fq_pair_decomp* dc)
+{
+  return decomp_host(ctx, a, as, win, ex, dc, true);
 }

@@ -387,6 +387,71 @@ int fq_replan_pairs_exact_async(fq_ctx* ctx, const fq_pair_args* args, const fq_
 int fq_replan_pairs_exact_dev(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
                               const fq_pair_exact* exact, fq_pair_result* results_all, void* stream);
 
+/* ---- chained replan that decomposes its own corridors on the device ----------------------------------------------------
+ *
+ * Faster::replan cuts the safe corridor around R (faster.cpp:474-475 R, :485 JPS_safe[0] = R.pos, :495-496 deleteVertexes
+ * and M, :499 cvxEllipsoidDecomp over unknown and occupied space, :503-504 M = G when the last safe polytope contains G;
+ * the whole corridor likewise at :393-403).  R only exists on the device, so the entry points below take the paths and
+ * obstacle clouds instead of polytopes and run fq_ellipsoid_decomp's decomposition on the device: the whole corridors
+ * before the whole sweep, the safe corridors around the device's R between the sweeps.  Feature "replan_pairs_decomp".
+ *
+ * `assign` is required (per-corridor lists, as _assign); window == NULL takes the shared factor lists of fq_pair_args (as
+ * _assign), a window the per-corridor windows (as _window); exact == NULL returns the list winners, an fq_pair_exact the
+ * exact optimum (as _exact).  In fq_pair_args, poly_ofs_* give the polytope counts P_j (one per path segment),
+ * face_ofs_*, Ab_* and xf_* must be NULL (FQ_E_ARG otherwise: the chain makes them), and max_faces_* / max_poly_faces_* are
+ * CAPS on a corridor's and a polytope's faces (they also size the solve kernels, as always).
+ *
+ * Per corridor and sweep the decomposition gives, bit for bit up to the atan2/hypot/sin/cos of the device (a few ulp;
+ * DESIGN.md 3.2), the rows fq_ellipsoid_decomp gives for the same path and cloud, and the final state E (whole) / M (safe):
+ * the goal when goal != NULL and the last polytope's rows all satisfy a.x - b <= 0 (LinearConstraint::inside), the path's
+ * last vertex otherwise; velocity and acceleration 0.  A corridor whose decomposition fails (status != 0) gets no winner for
+ * that sweep, and after a failed whole sweep no safe sweep; every other corridor of the batch is unaffected. */
+#define FQ_DECOMP_OK 0
+#define FQ_DECOMP_POLY_FACES 1      /* a polytope has more than max_poly_faces_* faces                               */
+#define FQ_DECOMP_CORRIDOR_FACES 2  /* the corridor has more than max_faces_* faces                                  */
+#define FQ_DECOMP_CLOUD 3           /* the corridor's cloud has more than max_obs_* points (_dev)                    */
+#define FQ_DECOMP_ZERO_SEGMENT 4    /* two consecutive path vertices coincide (for safe: also R.pos and vertex 1)    */
+#define FQ_DECOMP_NOT_RUN 5         /* safe: no whole winner, so no R; either: more than max_poly_* polytopes (_dev)  */
+
+typedef struct fq_pair_decomp
+{
+  /* inputs, per corridor: corridor j's path has P_j + 1 vertices (x, y, z) at rows poly_ofs_*[j] + j .. poly_ofs_*[j+1] + j,
+   * already trimmed by deleteVertexes; vertex 0 of the safe path is replaced by R.pos.  Clouds are CSR: corridor j's
+   * points are rows obs_ofs_*[j] .. obs_ofs_*[j+1] of obs_* (occupied space for whole, unknown and occupied for safe; the
+   * two may be the same arrays). */
+  const double *path_whole, *path_safe;
+  const int *obs_ofs_whole, *obs_ofs_safe;
+  const double *obs_whole, *obs_safe;
+  /* inputs, shared */
+  const double* goal;                   /* n_prob x 3, or NULL (then E / M are the last vertices)                    */
+  double bbox[3];                       /* local bounding box half sizes (jps_manager.cpp:100: 2, 2, 1)                 */
+  double inflate;                       /* obstacle inflation, the drone radius                                          */
+  double z_ground;                      /* ground face -z <= -z_ground                                                  */
+  int max_obs_whole, max_obs_safe;      /* _dev only: the largest cloud of one corridor (checked: FQ_DECOMP_CLOUD)     */
+  /* outputs, each optional (NULL): the corridors the sweeps used (the reference's poly_*_out), as an ordinary gap-free
+   * CSR -- face_ofs_* (poly_ofs_*[n_prob] + 1, absolute) and Ab_* (16-byte aligned, room for n_prob x max_faces_* rows);
+   * a failed corridor's polytopes are empty -- the E / M positions (n_prob x 3, NaN for a failed corridor), and the status
+   * of every corridor's decomposition (n_prob, FQ_DECOMP_*). */
+  int *face_ofs_whole, *face_ofs_safe;
+  double *Ab_whole, *Ab_safe;
+  double *E, *M;
+  int *status_whole, *status_safe;
+} fq_pair_decomp;
+
+/* HOST pointers everywhere; blocks until every output is in the caller's arrays.  FQ_E_ARG: decomp or assign NULL, the
+ * fq_pair_args rules above, the refusals of _assign / _window / _exact, a path, cloud or goal value that is not finite,
+ * bbox <= 0, inflate < 0, and multi-GPU contexts. */
+int fq_replan_pairs_decomp(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
+                           const fq_pair_exact* exact, const fq_pair_decomp* decomp);
+/* The same, returning once everything is enqueued; outputs are valid after fq_wait(ctx).  Arrays must stay alive. */
+int fq_replan_pairs_decomp_async(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
+                                 const fq_pair_exact* exact, const fq_pair_decomp* decomp);
+/* DEVICE pointers everywhere (the structs live on the host), with the hint rules of _assign_dev / _window_dev / _exact_dev
+ * and decomp->max_obs_*.  Never synchronises (a CUDA graph can capture it).  On a rank context the records are all-gathered
+ * into results_all as fq_replan_pairs_dev does. */
+int fq_replan_pairs_decomp_dev(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
+                               const fq_pair_exact* exact, const fq_pair_decomp* decomp, fq_pair_result* results_all, void* stream);
+
 /* ---- several GPUs behind the boundary (SURVEY.md 8b/8e) ---------------------------------------------------------
  *
  * Candidates of different corridors are independent, so a batch is sharded BY CORRIDOR: contiguous blocks of problems
