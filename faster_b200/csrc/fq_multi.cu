@@ -276,6 +276,8 @@ int fq_replan_pairs_sharded(fq_ctx* g, const fq_pair_args* a, bool deferred, con
 {
   fq_ctx* ctx = g;
   if (!a || a->n_prob <= 0 || !a->results) return fq_fail(g, FQ_E_ARG, "bad arguments");
+  // the members' own check of N (fq_pair_capi.cu), here before the list lengths below use N and the offsets are written
+  if (a->N_whole < 3 || a->N_whole > FQ_MAX_N || a->N_safe < 2 || a->N_safe > FQ_MAX_N) return fq_fail(g, FQ_E_ARG, "N out of range");
   // the shards' corridor descriptions are rebased on the host before the per-member validation runs: the arrays read
   // here must exist (everything else is checked by the member's own call)
   if (!a->x0 || !a->xf_whole || !a->xf_safe || !a->lim || !a->poly_ofs_whole || !a->face_ofs_whole || !a->poly_ofs_safe ||
@@ -299,8 +301,7 @@ int fq_replan_pairs_sharded(fq_ctx* g, const fq_pair_args* a, bool deferred, con
   std::vector<int> ofb;
   if (as)
   {
-    if (a->N_whole < 1 || a->N_whole > FQ_MAX_N || a->N_safe < 1 || a->N_safe > FQ_MAX_N || as->all_limit < 0)
-      return fq_fail(g, FQ_E_ARG, "N out of range or all_limit < 0");
+    if (as->all_limit < 0) return fq_fail(g, FQ_E_ARG, "all_limit < 0");
     ofw.assign(P + 1, 0); ofs.assign(P + 1, 0); ofb.assign(P + 1, 0);
     for (int j = 0; j < P; j++)
     {
