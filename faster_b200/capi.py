@@ -522,24 +522,46 @@ class Solver:
         self._check(fn(self._h, C.byref(a)))
         return out
 
+    def _list_outputs(self, w, all_limit, windows, inc, gamma, want_candidates, want_coeffs, extra=()):
+        """What the per-corridor-list entries share: each sweep's candidate offsets, from the factors_* of `w` or from
+        `windows`, and the returned arrays (results, cand_ofs_*, sigma_*, `extra`, the window outputs, and the candidate and
+        coeffs arrays when asked for).  -> (out, PairAssign, PairWindow or None)."""
+        n, Nw, Ns = w["n_prob"], w["N_whole"], w["N_safe"]
+        wins = None if windows is None else {k: np.ascontiguousarray(windows[k], np.float64) for k in WINDOW_IN_KEYS}
+        incs = (inc, inc) if np.isscalar(inc) else tuple(inc)
+        nc = {}
+        for kind, ik in (("whole", incs[0]), ("safe", incs[1])):
+            if wins is None:
+                ofs = assign_offsets(w["poly_ofs_" + kind], w["N_" + kind], len(w["factors_" + kind]), all_limit)
+            else:
+                nf = [len(window_factors(a, b, ik)) for a, b in zip(wins["init_" + kind], wins["final_" + kind])]
+                ofs = window_offsets(w["poly_ofs_" + kind], w["N_" + kind], nf, all_limit)
+            nc[kind] = int(ofs[-1])
+        out = dict(results=np.zeros(n, PAIR_RESULT_DTYPE), cand_ofs_whole=np.zeros(n + 1, np.int32), cand_ofs_safe=np.zeros(n + 1, np.int32),
+                   sigma_whole=np.zeros((n, Nw), np.uint8), sigma_safe=np.zeros((n, Ns), np.uint8))
+        out.update(extra)
+        if wins is not None:
+            out.update({k: (np.zeros(n, np.int32) if k.startswith("trials") else np.zeros(n)) for k in WINDOW_OUT_KEYS})
+        if want_candidates:
+            out.update(feasible_whole=np.zeros(nc["whole"], np.uint8), cost_whole=np.zeros(nc["whole"]),
+                       feasible_safe=np.zeros(nc["safe"], np.uint8), cost_safe=np.zeros(nc["safe"]))
+        if want_coeffs:
+            out.update(coeffs_whole=np.zeros((n, Nw, 12)), coeffs_safe=np.zeros((n, Ns, 12)))
+        s = assign_args(all_limit, {k: out[k].ctypes.data for k in ("cand_ofs_whole", "cand_ofs_safe", "sigma_whole", "sigma_safe")})
+        if wins is None:
+            return out, s, None
+        wa = window_args(lambda k: wins[k].ctypes.data, {k: out[k].ctypes.data for k in WINDOW_OUT_KEYS}, inc, gamma)
+        wa.arrays = wins                        # keeps the window arrays wa points to alive as long as wa
+        return out, s, wa
+
     def replan_pairs_assign(self, w, all_limit=0, want_candidates=True, want_coeffs=True, deferred=False):
         """fq_replan_pairs_assign on a make_pair_workload dict (host arrays; its sigmas_* are not used: every corridor
         gets its own list L(N, P_j, all_limit)).  -> dict(results, feasible_*/cost_* (per candidate, corridor j at
         cand_ofs_*[j] .. cand_ofs_*[j+1]), coeffs_*, cand_ofs_whole, cand_ofs_safe, sigma_whole, sigma_safe (the winners'
         assignments, 0s: none)).  deferred: valid after wait()."""
-        n = w["n_prob"]
-        ow = assign_offsets(w["poly_ofs_whole"], w["N_whole"], len(w["factors_whole"]), all_limit)
-        os_ = assign_offsets(w["poly_ofs_safe"], w["N_safe"], len(w["factors_safe"]), all_limit)
-        out = dict(results=np.zeros(n, PAIR_RESULT_DTYPE), cand_ofs_whole=np.zeros(n + 1, np.int32), cand_ofs_safe=np.zeros(n + 1, np.int32),
-                   sigma_whole=np.zeros((n, w["N_whole"]), np.uint8), sigma_safe=np.zeros((n, w["N_safe"]), np.uint8))
-        if want_candidates:
-            out.update(feasible_whole=np.zeros(int(ow[-1]), np.uint8), cost_whole=np.zeros(int(ow[-1])),
-                       feasible_safe=np.zeros(int(os_[-1]), np.uint8), cost_safe=np.zeros(int(os_[-1])))
-        if want_coeffs:
-            out.update(coeffs_whole=np.zeros((n, w["N_whole"], 12)), coeffs_safe=np.zeros((n, w["N_safe"], 12)))
+        out, s, _ = self._list_outputs(w, all_limit, None, 1.0, 20.0, want_candidates, want_coeffs)
         a = pair_args(w, lambda k: None if k.startswith("sigmas_") else w[k].ctypes.data, {k: v.ctypes.data for k, v in out.items()})
         a.n_sig_whole = a.n_sig_safe = 0
-        s = assign_args(all_limit, {k: out[k].ctypes.data for k in ("cand_ofs_whole", "cand_ofs_safe", "sigma_whole", "sigma_safe")})
         fn = self._L.fq_replan_pairs_assign_async if deferred else self._L.fq_replan_pairs_assign
         self._check(fn(self._h, C.byref(a), C.byref(s)))
         return out
@@ -549,28 +571,10 @@ class Solver:
         j sweeps its own window F_j and list L_j).  windows: dict of n_prob-arrays init_whole, final_whole, init_safe,
         final_safe; inc / gamma as window_args.  -> the dict of replan_pairs_assign plus factor_*, trials_* and the next
         windows next_init_* / next_final_*.  deferred: valid after wait()."""
-        n = w["n_prob"]
-        wins = {k: np.ascontiguousarray(windows[k], np.float64) for k in WINDOW_IN_KEYS}
-        incs = (inc, inc) if np.isscalar(inc) else tuple(inc)
-        offs = {}
-        for kind, ik in (("whole", incs[0]), ("safe", incs[1])):
-            nf = [len(window_factors(a, b, ik)) for a, b in zip(wins["init_" + kind], wins["final_" + kind])]
-            offs[kind] = window_offsets(w["poly_ofs_" + kind], w["N_" + kind], nf, all_limit)
-        out = dict(results=np.zeros(n, PAIR_RESULT_DTYPE), cand_ofs_whole=np.zeros(n + 1, np.int32), cand_ofs_safe=np.zeros(n + 1, np.int32),
-                   sigma_whole=np.zeros((n, w["N_whole"]), np.uint8), sigma_safe=np.zeros((n, w["N_safe"]), np.uint8),
-                   factor_whole=np.zeros(n), factor_safe=np.zeros(n), trials_whole=np.zeros(n, np.int32), trials_safe=np.zeros(n, np.int32),
-                   next_init_whole=np.zeros(n), next_final_whole=np.zeros(n), next_init_safe=np.zeros(n), next_final_safe=np.zeros(n))
-        if want_candidates:
-            ncw, ncs = int(offs["whole"][-1]), int(offs["safe"][-1])
-            out.update(feasible_whole=np.zeros(ncw, np.uint8), cost_whole=np.zeros(ncw), feasible_safe=np.zeros(ncs, np.uint8),
-                       cost_safe=np.zeros(ncs))
-        if want_coeffs:
-            out.update(coeffs_whole=np.zeros((n, w["N_whole"], 12)), coeffs_safe=np.zeros((n, w["N_safe"], 12)))
+        out, s, wa = self._list_outputs(w, all_limit, windows, inc, gamma, want_candidates, want_coeffs)
         a = pair_args(w, lambda k: None if k.startswith(("sigmas_", "factors_")) else w[k].ctypes.data,
                       {k: v.ctypes.data for k, v in out.items()})
         a.n_sig_whole = a.n_sig_safe = a.n_fac_whole = a.n_fac_safe = 0
-        s = assign_args(all_limit, {k: out[k].ctypes.data for k in ("cand_ofs_whole", "cand_ofs_safe", "sigma_whole", "sigma_safe")})
-        wa = window_args(lambda k: wins[k].ctypes.data, {k: out[k].ctypes.data for k in WINDOW_OUT_KEYS}, inc, gamma)
         fn = self._L.fq_replan_pairs_window_async if deferred else self._L.fq_replan_pairs_window
         self._check(fn(self._h, C.byref(a), C.byref(s), C.byref(wa)))
         return out
@@ -582,36 +586,14 @@ class Solver:
         dict of replan_pairs_assign (or _window) plus exact_whole, exact_safe (int32: 1 = the minimum over all assignments)
         and nodes_whole, nodes_safe (int64: tree nodes evaluated).  deferred: valid after wait()."""
         n = w["n_prob"]
-        if windows is None:
-            offs = {kind: assign_offsets(w["poly_ofs_" + kind], w["N_" + kind], len(w["factors_" + kind]), all_limit)
-                    for kind in ("whole", "safe")}
-        else:
-            wins = {k: np.ascontiguousarray(windows[k], np.float64) for k in WINDOW_IN_KEYS}
-            incs = (inc, inc) if np.isscalar(inc) else tuple(inc)
-            offs = {}
-            for kind, ik in (("whole", incs[0]), ("safe", incs[1])):
-                nf = [len(window_factors(a, b, ik)) for a, b in zip(wins["init_" + kind], wins["final_" + kind])]
-                offs[kind] = window_offsets(w["poly_ofs_" + kind], w["N_" + kind], nf, all_limit)
-        out = dict(results=np.zeros(n, PAIR_RESULT_DTYPE), cand_ofs_whole=np.zeros(n + 1, np.int32), cand_ofs_safe=np.zeros(n + 1, np.int32),
-                   sigma_whole=np.zeros((n, w["N_whole"]), np.uint8), sigma_safe=np.zeros((n, w["N_safe"]), np.uint8),
-                   exact_whole=np.zeros(n, np.int32), exact_safe=np.zeros(n, np.int32), nodes_whole=np.zeros(n, np.int64),
-                   nodes_safe=np.zeros(n, np.int64))
-        if windows is not None:
-            out.update({k: (np.zeros(n, np.int32) if k.startswith("trials") else np.zeros(n)) for k in WINDOW_OUT_KEYS})
-        if want_candidates:
-            ncw, ncs = int(offs["whole"][-1]), int(offs["safe"][-1])
-            out.update(feasible_whole=np.zeros(ncw, np.uint8), cost_whole=np.zeros(ncw), feasible_safe=np.zeros(ncs, np.uint8),
-                       cost_safe=np.zeros(ncs))
-        if want_coeffs:
-            out.update(coeffs_whole=np.zeros((n, w["N_whole"], 12)), coeffs_safe=np.zeros((n, w["N_safe"], 12)))
+        exact = dict(exact_whole=np.zeros(n, np.int32), exact_safe=np.zeros(n, np.int32), nodes_whole=np.zeros(n, np.int64),
+                     nodes_safe=np.zeros(n, np.int64))
+        out, s, wa = self._list_outputs(w, all_limit, windows, inc, gamma, want_candidates, want_coeffs, exact)
         skip = ("sigmas_",) if windows is None else ("sigmas_", "factors_")
         a = pair_args(w, lambda k: None if k.startswith(skip) else w[k].ctypes.data, {k: v.ctypes.data for k, v in out.items()})
         a.n_sig_whole = a.n_sig_safe = 0
         if windows is not None:
             a.n_fac_whole = a.n_fac_safe = 0
-        s = assign_args(all_limit, {k: out[k].ctypes.data for k in ("cand_ofs_whole", "cand_ofs_safe", "sigma_whole", "sigma_safe")})
-        wa = None if windows is None else window_args(lambda k: wins[k].ctypes.data, {k: out[k].ctypes.data for k in WINDOW_OUT_KEYS},
-                                                       inc, gamma)
         ex = exact_args({k: out[k].ctypes.data for k in EXACT_KEYS})
         fn = self._L.fq_replan_pairs_exact_async if deferred else self._L.fq_replan_pairs_exact
         self._check(fn(self._h, C.byref(a), C.byref(s), C.byref(wa) if wa is not None else None, C.byref(ex)))
@@ -624,32 +606,13 @@ class Solver:
         dict of replan_pairs_assign (plus the window / exact outputs when asked for) and the corridors the sweeps used:
         face_ofs_* / Ab_* (CSR), E, M (n_prob x 3) and status_whole / status_safe (FQ_DECOMP_*).  deferred: valid after wait()."""
         n, Nw, Ns = w["n_prob"], w["N_whole"], w["N_safe"]
-        if windows is None:
-            offs = {kind: assign_offsets(w["poly_ofs_" + kind], w["N_" + kind], len(w["factors_" + kind]), all_limit)
-                    for kind in ("whole", "safe")}
-        else:
-            wins = {k: np.ascontiguousarray(windows[k], np.float64) for k in WINDOW_IN_KEYS}
-            incs = (inc, inc) if np.isscalar(inc) else tuple(inc)
-            offs = {}
-            for kind, ik in (("whole", incs[0]), ("safe", incs[1])):
-                nf = [len(window_factors(a, b, ik)) for a, b in zip(wins["init_" + kind], wins["final_" + kind])]
-                offs[kind] = window_offsets(w["poly_ofs_" + kind], w["N_" + kind], nf, all_limit)
-        out = dict(results=np.zeros(n, PAIR_RESULT_DTYPE), cand_ofs_whole=np.zeros(n + 1, np.int32), cand_ofs_safe=np.zeros(n + 1, np.int32),
-                   sigma_whole=np.zeros((n, Nw), np.uint8), sigma_safe=np.zeros((n, Ns), np.uint8),
-                   face_ofs_whole=np.zeros(int(w["poly_ofs_whole"][-1]) + 1, np.int32), face_ofs_safe=np.zeros(int(w["poly_ofs_safe"][-1]) + 1, np.int32),
-                   Ab_whole=np.zeros((n * w["max_faces_whole"], 4)), Ab_safe=np.zeros((n * w["max_faces_safe"], 4)),
-                   E=np.zeros((n, 3)), M=np.zeros((n, 3)), status_whole=np.zeros(n, np.int32), status_safe=np.zeros(n, np.int32))
-        if windows is not None:
-            out.update({k: (np.zeros(n, np.int32) if k.startswith("trials") else np.zeros(n)) for k in WINDOW_OUT_KEYS})
+        extra = dict(face_ofs_whole=np.zeros(int(w["poly_ofs_whole"][-1]) + 1, np.int32), face_ofs_safe=np.zeros(int(w["poly_ofs_safe"][-1]) + 1, np.int32),
+                     Ab_whole=np.zeros((n * w["max_faces_whole"], 4)), Ab_safe=np.zeros((n * w["max_faces_safe"], 4)),
+                     E=np.zeros((n, 3)), M=np.zeros((n, 3)), status_whole=np.zeros(n, np.int32), status_safe=np.zeros(n, np.int32))
         if exact:
-            out.update(exact_whole=np.zeros(n, np.int32), exact_safe=np.zeros(n, np.int32), nodes_whole=np.zeros(n, np.int64),
-                       nodes_safe=np.zeros(n, np.int64))
-        if want_candidates:
-            ncw, ncs = int(offs["whole"][-1]), int(offs["safe"][-1])
-            out.update(feasible_whole=np.zeros(ncw, np.uint8), cost_whole=np.zeros(ncw), feasible_safe=np.zeros(ncs, np.uint8),
-                       cost_safe=np.zeros(ncs))
-        if want_coeffs:
-            out.update(coeffs_whole=np.zeros((n, Nw, 12)), coeffs_safe=np.zeros((n, Ns, 12)))
+            extra.update(exact_whole=np.zeros(n, np.int32), exact_safe=np.zeros(n, np.int32), nodes_whole=np.zeros(n, np.int64),
+                         nodes_safe=np.zeros(n, np.int64))
+        out, s, wa = self._list_outputs(w, all_limit, windows, inc, gamma, want_candidates, want_coeffs, extra)
         a = PairArgs()
         a.n_prob, a.N_whole, a.N_safe, a.DC, a.r_fraction = n, Nw, Ns, w["DC"], w["r_fraction"]
         for k in ("x0", "lim", "poly_ofs_whole", "poly_ofs_safe"):
@@ -661,9 +624,6 @@ class Solver:
             setattr(a, k, out[k].ctypes.data if k in out else None)
         for k in ("max_faces_whole", "max_poly_faces_whole", "max_faces_safe", "max_poly_faces_safe"):
             setattr(a, k, int(w[k]))
-        s = assign_args(all_limit, {k: out[k].ctypes.data for k in ("cand_ofs_whole", "cand_ofs_safe", "sigma_whole", "sigma_safe")})
-        wa = None if windows is None else window_args(lambda k: wins[k].ctypes.data, {k: out[k].ctypes.data for k in WINDOW_OUT_KEYS},
-                                                       inc, gamma)
         ex = exact_args({k: out[k].ctypes.data for k in EXACT_KEYS}) if exact else None
         dc = decomp_args(lambda k: None if (k == "goal" and not use_goal) else w[k].ctypes.data,
                          {k: out[k].ctypes.data for k in DECOMP_OUT_KEYS}, bbox, inflate, z_ground)

@@ -114,6 +114,12 @@ int fq_solve_multi_host_ex(fq_ctx* ctx, int N, int force_final, int n_prob, cons
                            const int* poly_ofs, const int* face_ofs, const double* Ab, const int* cand_ofs, const double* dt,
                            const uint8_t* sigma, uint8_t* feasible, double* cost, double* coeffs, int32_t* iters, bool deferred,
                            int** d_win_idx, double** d_win_cost);
+// Candidate offsets of one sweep with per-corridor assignment lists (fq_pair_capi.cu): corridor j (P_j polytopes) has
+// |L(N, P_j, all_limit)| candidates per factor and n_fac factors, or the |F_j| of its window (init[j], final_[j], inc) when
+// init is not NULL.  Fills ofs[0 .. n_prob], *max_fac (largest |F_j|, 0 without windows) and *max_poly (largest P_j), and
+// returns why the sweep is refused, or nullptr.
+const char* fq_list_offsets(int n_prob, const int* poly_ofs, int N, long all_limit, int n_fac, const double* init,
+                            const double* final_, double inc, std::vector<long long>* ofs, int* max_fac, int* max_poly);
 // fq_pair_capi.cu.  d_results (may be NULL): receives the device address of the result records; copy_results = false
 // leaves the caller's `results` array untouched (the multi-GPU path reads the all-gathered table instead).  as != NULL:
 // per-corridor assignment lists (fq_replan_pairs_assign*, host pointers); win != NULL (with as): per-corridor windows

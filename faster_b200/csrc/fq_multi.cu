@@ -6,9 +6,7 @@
 //   * one process, several GPUs (what the reference's single planner process would do): fq_create_multi.
 // NCCL is loaded lazily with dlopen (libnccl.so.2; FQ_NCCL_LIB overrides), so the library has no link-time dependency
 // on it and single-GPU use needs no NCCL at all.
-#include "fq_assign.h"
 #include "fq_ctx.h"
-#include "fq_window.h"
 
 #include <algorithm>
 #include <cstdlib>
@@ -301,26 +299,15 @@ int fq_replan_pairs_sharded(fq_ctx* g, const fq_pair_args* a, bool deferred, con
   std::vector<int> ofb;
   if (as)
   {
-    if (as->all_limit < 0) return fq_fail(g, FQ_E_ARG, "all_limit < 0");
-    ofw.assign(P + 1, 0); ofs.assign(P + 1, 0); ofb.assign(P + 1, 0);
-    for (int j = 0; j < P; j++)
-    {
-      const int pw = a->poly_ofs_whole[j + 1] - a->poly_ofs_whole[j], ps = a->poly_ofs_safe[j + 1] - a->poly_ofs_safe[j];
-      if (pw > FQ_MAX_POLY || ps > FQ_MAX_POLY) return fq_fail(g, FQ_E_ARG, "more than FQ_MAX_POLY polytopes in a corridor");
-      const long long lw = fqa::list_len(a->N_whole, pw, as->all_limit), ls = fqa::list_len(a->N_safe, ps, as->all_limit);
-      if (lw < 0 || ls < 0) return fq_fail(g, FQ_E_ARG, "assignment list of a corridor longer than 2^20");
-      int nfw = a->n_fac_whole, nfs = a->n_fac_safe;
-      if (win)
-      {
-        nfw = fqw::factors(win->init_whole[j], win->final_whole[j], win->inc_whole, nullptr, 0);
-        nfs = fqw::factors(win->init_safe[j], win->final_safe[j], win->inc_safe, nullptr, 0);
-        if (nfw < 0 || nfs < 0) return fq_fail(g, FQ_E_ARG, "time-allocation window refused (not finite, init <= 0, more than 4096 factors or a stalled accumulation)");
-      }
-      ofw[j + 1] = ofw[j] + lw * nfw;
-      ofs[j + 1] = ofs[j] + ls * nfs;
-      if (ofw[j + 1] > (1LL << 30) || ofs[j + 1] > (1LL << 30)) return fq_fail(g, FQ_E_ARG, "too many candidates");
-      ofb[j + 1] = (int)std::min<long long>(ofw[j + 1] + ofs[j + 1], 0x7fffffffLL);
-    }
+    int mf = 0, mp = 0;
+    const char* why = fq_list_offsets(P, a->poly_ofs_whole, a->N_whole, as->all_limit, a->n_fac_whole, win ? win->init_whole : nullptr,
+                                      win ? win->final_whole : nullptr, win ? win->inc_whole : 0, &ofw, &mf, &mp);
+    if (!why)
+      why = fq_list_offsets(P, a->poly_ofs_safe, a->N_safe, as->all_limit, a->n_fac_safe, win ? win->init_safe : nullptr,
+                            win ? win->final_safe : nullptr, win ? win->inc_safe : 0, &ofs, &mf, &mp);
+    if (why) return fq_fail(g, FQ_E_ARG, why);
+    ofb.assign(P + 1, 0);
+    for (int j = 1; j <= P; j++) ofb[j] = (int)std::min<long long>(ofw[j] + ofs[j], 0x7fffffffLL);
   }
   int pad = 0;
   std::vector<int> lo(world), hi(world);
