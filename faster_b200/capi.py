@@ -18,7 +18,8 @@ EXPORTS = ["fq_abi_version", "fq_create", "fq_destroy", "fq_last_error", "fq_set
            "fq_pair_assign_count", "fq_replan_pairs_assign", "fq_replan_pairs_assign_async", "fq_replan_pairs_assign_dev",
            "fq_pair_window_factors", "fq_replan_pairs_window", "fq_replan_pairs_window_async", "fq_replan_pairs_window_dev",
            "fq_replan_pairs_exact", "fq_replan_pairs_exact_async", "fq_replan_pairs_exact_dev", "fq_replan_pairs_decomp",
-           "fq_replan_pairs_decomp_async", "fq_replan_pairs_decomp_dev"]
+           "fq_replan_pairs_decomp_async", "fq_replan_pairs_decomp_dev", "fq_replan_pairs_hr", "fq_replan_pairs_hr_async",
+           "fq_replan_pairs_hr_dev"]
 
 
 class FqError(RuntimeError):
@@ -84,6 +85,16 @@ class PairDecomp(C.Structure):
                 ("inflate", C.c_double), ("z_ground", C.c_double), ("max_obs_whole", C.c_int), ("max_obs_safe", C.c_int),
                 ("face_ofs_whole", C.c_void_p), ("face_ofs_safe", C.c_void_p), ("Ab_whole", C.c_void_p), ("Ab_safe", C.c_void_p),
                 ("E", C.c_void_p), ("M", C.c_void_p), ("status_whole", C.c_void_p), ("status_safe", C.c_void_p)]
+
+
+class PairHR(C.Structure):
+    """fq_pair_hr of include/faster_b200.h: the unknown clouds and parameters of findIndexH / findIndexR."""
+    _fields_ = [("unk_ofs", C.c_void_p), ("unk", C.c_void_p), ("drone_radius", C.c_double), ("delta_a", C.c_double),
+                ("delta_H", C.c_double), ("last_factor_safe", C.c_void_p), ("index_H", C.c_void_p), ("need_safe", C.c_void_p)]
+
+
+HR_OUT_KEYS = ["last_factor_safe", "index_H", "need_safe"]
+HR_DEFAULTS = dict(drone_radius=0.42, delta_a=0.5, delta_H=1.0)         # faster.yaml:7,35,36
 
 
 DECOMP_IN_KEYS = ["path_whole", "path_safe", "obs_ofs_whole", "obs_ofs_safe", "obs_whole", "obs_safe", "goal"]
@@ -155,6 +166,9 @@ def lib():
         L.fq_replan_pairs_decomp_async.argtypes = L.fq_replan_pairs_decomp.argtypes
         L.fq_replan_pairs_decomp_dev.argtypes = [C.c_void_p, C.POINTER(PairArgs), C.POINTER(PairAssign), C.POINTER(PairWindow),
                                                  C.POINTER(PairExact), C.POINTER(PairDecomp), C.c_void_p, C.c_void_p]
+        L.fq_replan_pairs_hr.argtypes = L.fq_replan_pairs_decomp.argtypes + [C.POINTER(PairHR)]
+        L.fq_replan_pairs_hr_async.argtypes = L.fq_replan_pairs_hr.argtypes
+        L.fq_replan_pairs_hr_dev.argtypes = L.fq_replan_pairs_hr.argtypes + [C.c_void_p, C.c_void_p]
         L.fq_create_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_void_p]
         L.fq_comm_unique_id.argtypes = [C.c_void_p]
         L.fq_comm_init.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
@@ -281,6 +295,18 @@ def decomp_args(ptr, out_ptrs, bbox=(2.0, 2.0, 1.0), inflate=0.42, z_ground=0.0,
     return s
 
 
+def hr_args(unk_ofs, unk, out_ptrs, drone_radius=HR_DEFAULTS["drone_radius"], delta_a=HR_DEFAULTS["delta_a"],
+            delta_H=HR_DEFAULTS["delta_H"]):
+    """PairHR; unk_ofs / unk: addresses of the unknown clouds' CSR, out_ptrs: addresses of HR_OUT_KEYS (0/None/missing =
+    NULL; last_factor_safe is in/out)."""
+    s = PairHR()
+    s.unk_ofs, s.unk = unk_ofs, unk
+    s.drone_radius, s.delta_a, s.delta_H = float(drone_radius), float(delta_a), float(delta_H)
+    for k in HR_OUT_KEYS:
+        setattr(s, k, out_ptrs.get(k) or None)
+    return s
+
+
 def make_decomp_workload(pairs, max_faces=400, max_poly_faces=64):
     """Packs corridor.forest_pair_paths dicts (one per corridor) into the host arrays of fq_pair_args (face_ofs_*, Ab_* and
     xf_* absent: the chain makes them) and of fq_pair_decomp.  max_faces / max_poly_faces are the caps of both sweeps.
@@ -300,6 +326,10 @@ def make_decomp_workload(pairs, max_faces=400, max_poly_faces=64):
     ofs = np.concatenate([[0], np.cumsum([len(o) for o in obs])]).astype(np.int32)
     cloud = np.ascontiguousarray(np.vstack(obs)) if ofs[-1] else np.zeros((1, 3))
     out.update(obs_ofs_whole=ofs, obs_ofs_safe=ofs, obs_whole=cloud, obs_safe=cloud)
+    if all("unk" in p for p in pairs):          # unknown clouds (fq_pair_hr), e.g. corridor.forest_unknown_cloud
+        unk = [np.asarray(p["unk"], np.float64).reshape(-1, 3) for p in pairs]
+        out["unk_ofs"] = np.concatenate([[0], np.cumsum([len(u) for u in unk])]).astype(np.int32)
+        out["unk"] = np.ascontiguousarray(np.vstack(unk + [np.zeros((1, 3))]))
     return out
 
 
@@ -605,6 +635,35 @@ class Solver:
         factor lists) or `windows` (per-corridor windows, as replan_pairs_window); exact=True adds the exact stage.  -> the
         dict of replan_pairs_assign (plus the window / exact outputs when asked for) and the corridors the sweeps used:
         face_ofs_* / Ab_* (CSR), E, M (n_prob x 3) and status_whole / status_safe (FQ_DECOMP_*).  deferred: valid after wait()."""
+        out, structs = self._decomp_structs(w, all_limit, windows, inc, gamma, exact, bbox, inflate, z_ground, use_goal,
+                                            want_candidates, want_coeffs)
+        fn = self._L.fq_replan_pairs_decomp_async if deferred else self._L.fq_replan_pairs_decomp
+        self._check(fn(self._h, *structs))
+        return out
+
+    def replan_pairs_hr(self, w, last_factor_safe=None, drone_radius=HR_DEFAULTS["drone_radius"], delta_a=HR_DEFAULTS["delta_a"],
+                        delta_H=HR_DEFAULTS["delta_H"], all_limit=0, windows=None, inc=1.0, gamma=20.0, exact=False,
+                        bbox=(2.0, 2.0, 1.0), inflate=0.42, z_ground=0.0, use_goal=True, want_candidates=False, want_coeffs=True,
+                        deferred=False):
+        """fq_replan_pairs_hr on a make_decomp_workload dict with unknown clouds (unk_ofs, unk): replan_pairs_decomp with H and
+        R chosen from the clouds.  last_factor_safe: n_prob factors (default 0, the start-up value; required in effect with
+        `windows`).  -> the dict of replan_pairs_decomp plus index_H (int32), need_safe (uint8) and last_factor_safe (the
+        updated copy).  deferred: valid after wait()."""
+        n = w["n_prob"]
+        last = np.zeros(n) if last_factor_safe is None else np.array(last_factor_safe, np.float64).reshape(n)
+        extra = dict(last_factor_safe=last, index_H=np.zeros(n, np.int32), need_safe=np.zeros(n, np.uint8))
+        out, structs = self._decomp_structs(w, all_limit, windows, inc, gamma, exact, bbox, inflate, z_ground, use_goal,
+                                            want_candidates, want_coeffs, extra)
+        hr = hr_args(w["unk_ofs"].ctypes.data, w["unk"].ctypes.data, {k: out[k].ctypes.data for k in HR_OUT_KEYS}, drone_radius,
+                     delta_a, delta_H)
+        fn = self._L.fq_replan_pairs_hr_async if deferred else self._L.fq_replan_pairs_hr
+        self._check(fn(self._h, *structs, C.byref(hr)))
+        return out
+
+    def _decomp_structs(self, w, all_limit, windows, inc, gamma, exact, bbox, inflate, z_ground, use_goal, want_candidates,
+                        want_coeffs, extra_out=()):
+        """The returned arrays and the (PairArgs, PairAssign, PairWindow, PairExact, PairDecomp) arguments of
+        replan_pairs_decomp / replan_pairs_hr (ctypes references or None)."""
         n, Nw, Ns = w["n_prob"], w["N_whole"], w["N_safe"]
         extra = dict(face_ofs_whole=np.zeros(int(w["poly_ofs_whole"][-1]) + 1, np.int32), face_ofs_safe=np.zeros(int(w["poly_ofs_safe"][-1]) + 1, np.int32),
                      Ab_whole=np.zeros((n * w["max_faces_whole"], 4)), Ab_safe=np.zeros((n * w["max_faces_safe"], 4)),
@@ -612,6 +671,7 @@ class Solver:
         if exact:
             extra.update(exact_whole=np.zeros(n, np.int32), exact_safe=np.zeros(n, np.int32), nodes_whole=np.zeros(n, np.int64),
                          nodes_safe=np.zeros(n, np.int64))
+        extra.update(extra_out)
         out, s, wa = self._list_outputs(w, all_limit, windows, inc, gamma, want_candidates, want_coeffs, extra)
         a = PairArgs()
         a.n_prob, a.N_whole, a.N_safe, a.DC, a.r_fraction = n, Nw, Ns, w["DC"], w["r_fraction"]
@@ -627,10 +687,13 @@ class Solver:
         ex = exact_args({k: out[k].ctypes.data for k in EXACT_KEYS}) if exact else None
         dc = decomp_args(lambda k: None if (k == "goal" and not use_goal) else w[k].ctypes.data,
                          {k: out[k].ctypes.data for k in DECOMP_OUT_KEYS}, bbox, inflate, z_ground)
-        fn = self._L.fq_replan_pairs_decomp_async if deferred else self._L.fq_replan_pairs_decomp
-        self._check(fn(self._h, C.byref(a), C.byref(s), C.byref(wa) if wa is not None else None, C.byref(ex) if ex is not None else None,
-                       C.byref(dc)))
-        return out
+        return out, [C.byref(x) if x is not None else None for x in (a, s, wa, ex, dc)]
+
+    def replan_pairs_hr_dev(self, a, s, win, ex, dc, hr, results_all=0, stream=0):
+        """fq_replan_pairs_hr_dev: as replan_pairs_decomp_dev, with `hr` (PairHR) holding device addresses."""
+        self._check(self._L.fq_replan_pairs_hr_dev(self._h, C.byref(a), C.byref(s), C.byref(win) if win is not None else None,
+                                                   C.byref(ex) if ex is not None else None, C.byref(dc), C.byref(hr),
+                                                   results_all or None, stream or None))
 
     def replan_pairs_decomp_dev(self, a, s, win, ex, dc, results_all=0, stream=0):
         """fq_replan_pairs_decomp_dev: `a`, `s`, `win` (PairWindow or None), `ex` (PairExact or None) and `dc` (PairDecomp)

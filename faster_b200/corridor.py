@@ -407,6 +407,38 @@ def forest_pair_paths(seed, N=10, max_poly_whole=3, max_poly_safe=4, Ra=4.0, r_f
                 goal=np.asarray(t, float), x0=x0, xf_whole=xf, xf_safe=xfs, lim=lim, R_estimate=R9, seed=seed, profile="uav")
 
 
+def forest_unknown_cloud(p, seed=None, half=3.0, dz=0.6, sensing=(1.6, 4.5), n_trees=60):
+    """A seeded unknown cloud for the forest replan `p` (forest_pair_paths), as kdtree_unk_ holds it: the centres of the free
+    cells of the local window |x - A.x|, |y - A.y| <= half, |z - A.z| <= dz around A = p["x0"] that A has not seen -- out
+    of a sensing range drawn from `sensing` (U[lo, hi], seeded), or shadowed in xy by a trunk between A and the cell.
+    With the defaults a corridor holds a few thousand points, and about half the corridors of a batch have a whole
+    trajectory that comes within drone_radius of one (need a safe path).  -> [m, 3] float64."""
+    rng = np.random.default_rng(p["seed"] + 7919 if seed is None else seed)
+    _, centres, radii = make_forest(p["seed"], n_trees=n_trees)
+    grid, origin, res = voxelise_forest(centres, radii)
+    A = np.asarray(p["x0"][:3], float)
+    reach = rng.uniform(*sensing)
+    zd, yd, xd = grid.shape
+    cx = (np.arange(xd) + 0.5) * res + origin[0]
+    cy = (np.arange(yd) + 0.5) * res + origin[1]
+    cz = (np.arange(zd) + 0.5) * res + origin[2]
+    ix = np.flatnonzero(np.abs(cx - A[0]) <= half)
+    iy = np.flatnonzero(np.abs(cy - A[1]) <= half)
+    iz = np.flatnonzero(np.abs(cz - A[2]) <= dz)
+    Y, X = np.meshgrid(cy[iy], cx[ix], indexing="ij")
+    dx, dy = X - A[0], Y - A[1]
+    dist = np.hypot(dx, dy)
+    unseen = dist > reach
+    for c, r in zip(centres, radii):                      # a trunk between A and the cell hides it
+        ox, oy = c[0] - A[0], c[1] - A[1]
+        t = np.clip((ox * dx + oy * dy) / np.maximum(dist * dist, 1e-12), 0.0, 1.0)
+        unseen |= (np.hypot(t * dx - ox, t * dy - oy) <= r) & (t < 1.0) & (np.hypot(ox, oy) < dist)
+    free = grid[np.ix_(iz, iy, ix)] == 0
+    cells = free & unseen[None]
+    kz, ky, kx = np.nonzero(cells)
+    return np.ascontiguousarray(np.stack([cx[ix][kx], cy[iy][ky], cz[iz][kz]], axis=1))
+
+
 # ------------------------------------------------------------------------------------------------------------------
 # Feasibility margins (SURVEY.md section 7, "hard parts"): Gurobi decides feasibility with FeasibilityTol 1e-6 on its own
 # scaled rows, this library with an absolute row tolerance (default 1e-8).  Candidates whose feasibility depends on

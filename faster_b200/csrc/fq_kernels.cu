@@ -766,6 +766,13 @@ cudaError_t fq_launch_pair_mid(const FqPairMidArgs& a, cudaStream_t stream)
   return cudaGetLastError();
 }
 
+cudaError_t fq_launch_pair_hr(const FqPairHrArgs& a, cudaStream_t stream)
+{
+  if (a.n_prob <= 0) return cudaSuccess;
+  fqp::fq_pair_hr_kernel<<<a.n_prob, 256, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+
 cudaError_t fq_launch_pair_final(const FqPairFinalArgs& a, cudaStream_t stream)
 {
   if (a.n_prob <= 0) return cudaSuccess;

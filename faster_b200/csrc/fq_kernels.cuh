@@ -198,6 +198,27 @@ struct FqPairMidArgs
   double* x0_safe;                      // n_prob x 9 (NaN when there is no whole trajectory to branch from)
   int* n_samples;                       // n_prob
   int* k_safe;                          // n_prob
+  // fq_replan_pairs_hr*: R's index per corridor from fq_pair_hr_kernel in place of the r_fraction rule; < 0: no safe path
+  // is needed (no R, k_safe = n - 1).  NULL: the r_fraction rule.
+  const int* r_index = nullptr;
+};
+
+// indexH / needToComputeSafePath / indexR of every corridor (fq_pair_hr_kernel, faster.cpp:173-251), after the whole
+// sweep's coefficients
+struct FqPairHrArgs
+{
+  int n_prob, N;
+  double DC, drone_radius, delta_a, delta_H;
+  const double* coeffs;                 // n_prob x N x 12: the whole winners
+  const double* win_dt;                 // n_prob (NaN: no winner)
+  const int* win_idx;
+  const double* lim;                    // n_prob x 3: a_max = lim[3 j + 1]
+  const int* unk_ofs;                   // n_prob + 1: corridor j's unknown cloud is rows unk_ofs[j] .. unk_ofs[j+1]-1 of unk
+  const double* unk;
+  int* r_index;                         // out n_prob: k_safe when a safe path is needed, else -1 (FqPairMidArgs::r_index)
+  uint8_t* need;                        // out n_prob: needToComputeSafePath (0 without a whole winner)
+  uint8_t* need_out;                    // out n_prob, or NULL: a copy for the caller
+  int* index_H;                         // out n_prob, or NULL: indexH (-1 without a whole winner)
 };
 
 struct FqPairFinalArgs
@@ -241,6 +262,11 @@ struct FqPairWindowArgs
   double *factor_w, *factor_s;          // out, or NULL
   int *trials_w, *trials_s;             // out, or NULL
   double *next_init_w, *next_final_w, *next_init_s, *next_final_s;   // out, or NULL; may alias init_* / final_*
+  // fq_replan_pairs_hr*: need_safe[j] = 0 means the replan needed no safe sweep and still succeeded when the whole sweep
+  // won; the safe window then follows last_factor_safe[j] (in/out: the safe winner's factor when the safe sweep wins).
+  // NULL: every replan runs both sweeps.
+  const uint8_t* need_safe = nullptr;
+  double* last_factor_safe = nullptr;
 };
 
 // the device decomposition of one sweep's corridors (fq_decomp.cuh): fq_decomp_kernel stages every polytope's rows in a slot
@@ -296,4 +322,5 @@ cudaError_t fq_launch_expand_window(int n_prob, int N, int max_fac, long long al
 cudaError_t fq_launch_pair_window(const FqPairWindowArgs& a, cudaStream_t stream);
 cudaError_t fq_launch_select_multi(const FqSelectMultiArgs& a, cudaStream_t stream);
 cudaError_t fq_launch_pair_mid(const FqPairMidArgs& a, cudaStream_t stream);
+cudaError_t fq_launch_pair_hr(const FqPairHrArgs& a, cudaStream_t stream);
 cudaError_t fq_launch_pair_final(const FqPairFinalArgs& a, cudaStream_t stream);

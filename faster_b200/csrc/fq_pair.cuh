@@ -205,9 +205,33 @@ __global__ void __launch_bounds__(128) fq_select_multi_kernel(const FqSelectMult
     for (int t = threadIdx.x; t < a.N; t += blockDim.x) a.win_sigma[(size_t)j * a.N + t] = w >= 0 && a.sigma ? a.sigma[(size_t)(c0 + w) * a.N + t] : (uint8_t)0;
 }
 
-// Between the two sweeps: R = X_temp_[k_safe] of the whole winner (faster.cpp:475; fillX, solverGurobi.cpp:122-168, with the
-// reference's accumulated sample time and lagging interval index), k_safe = min(n - 1, (int)(r_fraction * n)) standing in
-// for findIndexR (faster.cpp:173-216, out of scope: needs the map).  One thread per problem.
+// fillX's sample clock (solverGurobi.cpp:122-168): the reference's accumulated sample time and lagging interval index.  A
+// clock only moves forward; sample i is always reached through samples 0 .. i-1, so every sample has the bits of fillX's.
+struct SampleClock
+{
+  double t = 0;
+  int interval = 0, next = 0;           // `next`: the first sample not reached yet
+};
+
+// sample i (>= the clock's last one) of corridor j's whole winner: pos vel accel jerk into o; the last sample (n - 1) is at rest
+FQ_HD void sample_at(SampleClock& c, int i, const double* coeffs_j, int N, double dt, double DC, int n, double* o)
+{
+  for (; c.next <= i; c.next++)
+  {
+    c.t = FQ_ADD(c.t, DC);
+    if (c.t > FQ_MUL(dt, (double)(c.interval + 1))) c.interval = c.interval + 1 < N - 1 ? c.interval + 1 : N - 1;
+  }
+  const double tau = FQ_SUB(c.t, FQ_MUL((double)c.interval, dt));
+  double x[12];
+  for (int q = 0; q < 12; q++) x[q] = coeffs_j[c.interval * 12 + q];
+  fqdt::eval_sample(x, tau, o);
+  if (i == n - 1)
+    for (int q = 3; q < 12; q++) o[q] = 0.0;                       // :165-167: the last sample is at rest
+}
+
+// Between the two sweeps: R = X_temp_[k_safe] of the whole winner (faster.cpp:475; fillX, solverGurobi.cpp:122-168).  k_safe
+// is r_index[j] from fq_pair_hr_kernel (findIndexR, faster.cpp:173-216; < 0: no safe path is needed, so no R and k_safe =
+// indexH = n - 1, :465-469), or without r_index min(n - 1, (int)(r_fraction * n)).  One thread per problem.
 
 __global__ void fq_pair_mid_kernel(const FqPairMidArgs a)
 {
@@ -222,23 +246,130 @@ __global__ void fq_pair_mid_kernel(const FqPairMidArgs a)
   }
   const double dt = a.win_dt[j], DC = a.DC;
   const int n = fqdt::num_samples(a.N, dt, DC);
-  int k = (int)(a.r_fraction * (double)n);
-  k = k < 0 ? 0 : (k > n - 1 ? n - 1 : k);
-  double t = 0;
-  int interval = 0;
-  for (int i = 0; i <= k; i++)
+  int k;
+  if (a.r_index)
   {
-    t = FQ_ADD(t, DC);
-    if (t > FQ_MUL(dt, (double)(interval + 1))) interval = interval + 1 < a.N - 1 ? interval + 1 : a.N - 1;
+    k = a.r_index[j];
+    if (k < 0)
+    {
+      for (int i = 0; i < 9; i++) a.x0_safe[j * 9 + i] = nan;
+      a.n_samples[j] = n; a.k_safe[j] = n - 1;
+      return;
+    }
   }
-  const double tau = FQ_SUB(t, FQ_MUL((double)interval, dt));
-  double x[12], o[12];
-  for (int i = 0; i < 12; i++) x[i] = a.coeffs[((size_t)j * a.N + interval) * 12 + i];
-  fqdt::eval_sample(x, tau, o);
-  if (k == n - 1)
-    for (int i = 3; i < 12; i++) o[i] = 0.0;                       // :165-167: the last sample is at rest
+  else
+  {
+    k = (int)(a.r_fraction * (double)n);
+    k = k < 0 ? 0 : (k > n - 1 ? n - 1 : k);
+  }
+  SampleClock c;
+  double o[12];
+  sample_at(c, k, a.coeffs + (size_t)j * a.N * 12, a.N, dt, DC, n, o);
   for (int i = 0; i < 9; i++) a.x0_safe[j * 9 + i] = o[i];
   a.n_samples[j] = n; a.k_safe[j] = k;
+}
+
+// findIndexH and findIndexR (faster.cpp:173-251) for every corridor, from its whole winner and its unknown cloud; one CTA per
+// corridor, any block size.
+//   H: for the samples i = 0, 10, 20, ... < n of X_temp_ in order, the nearest unknown point (kdtree_unk_.nearestKSearch)
+//      with pcl::PointXYZ's float coordinates and FLANN's float L2 order ((0 + dx^2) + dy^2) + dz^2; the first sample with
+//      sqrtf(d^2) < drone_radius (in double) sets needToComputeSafePath and indexH = (int)(delta_H i); none: indexH = n - 1.
+//      Since sqrtf is monotone, "the nearest point is that close" is "some point is that close": the CTA scans the cloud for
+//      any such point (__syncthreads_or), which neither thread count nor warp order can change.
+//   R: the first i in 0 .. indexH whose braking distance sign(v (H - p)) v^2 / (2 delta_a a_max) exceeds |H - p| in x or y,
+//      else indexH.  Threads take strided samples, each walking its own sample clock; the first index is a block minimum.
+#if defined(__CUDA_ARCH__)
+#define FQ_F2(x) __double2float_rn(x)
+#define FQ_FMUL(a, b) __fmul_rn((a), (b))
+#define FQ_FADD(a, b) __fadd_rn((a), (b))
+#define FQ_FSUB(a, b) __fsub_rn((a), (b))
+#define FQ_FSQRT(a) __fsqrt_rn(a)
+#else
+#define FQ_F2(x) ((float)(x))
+#define FQ_FMUL(a, b) ((a) * (b))
+#define FQ_FADD(a, b) ((a) + (b))
+#define FQ_FSUB(a, b) ((a) - (b))
+#define FQ_FSQRT(a) std::sqrt((float)(a))
+#endif
+
+// squared float distance in FLANN's L2 order (flann/algorithms/dist.h, L2::operator() for 3 values)
+FQ_HD float flann_l2(const float* q, const double* p)
+{
+  const float dx = FQ_FSUB(FQ_F2(p[0]), q[0]), dy = FQ_FSUB(FQ_F2(p[1]), q[1]), dz = FQ_FSUB(FQ_F2(p[2]), q[2]);
+  return FQ_FADD(FQ_FADD(FQ_FADD(0.0f, FQ_FMUL(dx, dx)), FQ_FMUL(dy, dy)), FQ_FMUL(dz, dz));
+}
+
+// findIndexR's test of one sample (faster.cpp:186-196): any of x, y with a braking distance above |H - p|
+FQ_HD bool brakes_past(const double* H, const double* o, double delta_a, double a_max)
+{
+  const double den = FQ_MUL(FQ_MUL(2.0, delta_a), a_max);
+  bool hit = false;
+  for (int ax = 0; ax < 2; ax++)
+  {
+    const double d = FQ_SUB(H[ax], o[ax]), v = o[3 + ax], sv = FQ_MUL(v, d);
+    const double sgn = sv > 0 ? 1.0 : (sv < 0 ? -1.0 : 0.0);             // Eigen's sign(): 0 for 0
+    const double b = FQ_DIV(FQ_MUL(sgn, FQ_MUL(v, v)), den);
+    hit = hit || b > fabs(d);
+  }
+  return hit;
+}
+
+__global__ void __launch_bounds__(256) fq_pair_hr_kernel(const FqPairHrArgs a)
+{
+  __shared__ float s_q[3];
+  __shared__ double s_H[2];
+  __shared__ int s_k;
+  const int j = blockIdx.x, tid = threadIdx.x, T = blockDim.x;
+  if (j >= a.n_prob) return;
+  auto put = [&](int r, int need, int h) {
+    if (tid != 0) return;
+    a.r_index[j] = r; a.need[j] = (uint8_t)need;
+    if (a.need_out) a.need_out[j] = (uint8_t)need;
+    if (a.index_H) a.index_H[j] = h;
+  };
+  if (a.win_idx[j] < 0) { put(-1, 0, -1); return; }
+  const double dt = a.win_dt[j], DC = a.DC;
+  const int N = a.N, n = fqdt::num_samples(N, dt, DC);
+  const double* co = a.coeffs + (size_t)j * N * 12;
+  const int lo = a.unk_ofs[j], hi = a.unk_ofs[j + 1];
+  SampleClock c0;                                                   // thread 0's clock through the H queries
+  int hit_i = -1;
+  for (int i = 0; i < n && hi > lo; i += 10)
+  {
+    if (tid == 0)
+    {
+      double o[12];
+      sample_at(c0, i, co, N, dt, DC, n, o);
+      for (int q = 0; q < 3; q++) s_q[q] = FQ_F2(o[q]);            // pcl::PointXYZ searchPoint(tmp(0), tmp(1), tmp(2))
+    }
+    __syncthreads();
+    const float q[3] = { s_q[0], s_q[1], s_q[2] };
+    int near = 0;
+    for (int p = lo + tid; p < hi && !near; p += T)
+      near = (double)FQ_FSQRT(flann_l2(q, a.unk + 3 * (size_t)p)) < a.drone_radius;
+    if (__syncthreads_or(near)) { hit_i = i; break; }               // also the barrier before s_q is written again
+  }
+  if (hit_i < 0) { put(-1, 0, n - 1); return; }
+  const int iH = (int)FQ_MUL(a.delta_H, (double)hit_i);
+  if (tid == 0)
+  {
+    SampleClock c;
+    double o[12];
+    sample_at(c, iH, co, N, dt, DC, n, o);
+    s_H[0] = o[0]; s_H[1] = o[1];
+    s_k = 0x7fffffff;
+  }
+  __syncthreads();
+  const double H[2] = { s_H[0], s_H[1] }, a_max = a.lim[3 * j + 1];
+  SampleClock c;
+  for (int i = tid; i <= iH; i += T)
+  {
+    double o[12];
+    sample_at(c, i, co, N, dt, DC, n, o);
+    if (brakes_past(H, o, a.delta_a, a_max)) { atomicMin(&s_k, i); break; }
+  }
+  __syncthreads();
+  put(s_k == 0x7fffffff ? iH : s_k, 1, iH);
 }
 
 // result records (fq_pair_result of include/faster_b200.h; 16 doubles each)
@@ -283,27 +414,32 @@ __global__ void fq_pair_final_kernel(const FqPairFinalArgs a)
 // factor_that_worked_, trials_ and the next windows of every corridor (fq_window.h), after fq_pair_final_kernel.  trials:
 // the winner's index in F_j + 1; |F_j| without a winner; 0 for a sweep that did not run (a safe sweep after a whole sweep
 // without winner, or a sweep the offsets kernel emptied).  Each thread reads its corridor's windows before it writes the
-// next ones, so those may alias.
+// next ones, so those may alias.  With need_safe (fq_replan_pairs_hr*), a replan that needed no safe path ran no safe sweep
+// (trials 0) and succeeds when the whole sweep won; its safe window then follows the safe solver's previous
+// factor_that_worked_ (faster.cpp:586-588), last_factor_safe, which only a safe winner changes.
 __global__ void fq_pair_window_kernel(const FqPairWindowArgs a)
 {
   const int j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= a.n_prob) return;
   const double nan = __longlong_as_double(0x7ff8000000000000ll);
   const int dw = a.rec[j].whole_dt_index, ds = a.rec[j].safe_dt_index;
-  const bool ran_w = a.cand_ofs_w[a.n_prob] > 0, ran_s = ran_w && dw >= 0 && a.cand_ofs_s[a.n_prob] > 0;
+  const bool no_safe = a.need_safe && !a.need_safe[j];
+  const bool ran_w = a.cand_ofs_w[a.n_prob] > 0, ran_s = ran_w && dw >= 0 && a.cand_ofs_s[a.n_prob] > 0 && !no_safe;
   const double fw = dw >= 0 ? a.fac_w[(size_t)j * a.max_fac_w + dw] : nan;
   const double fs = ds >= 0 ? a.fac_s[(size_t)j * a.max_fac_s + ds] : nan;
   const double iw = a.init_w[j], ew = a.final_w[j], is = a.init_s[j], es = a.final_s[j];
+  const double last_s = a.last_factor_safe ? a.last_factor_safe[j] : nan;
   if (a.factor_w) a.factor_w[j] = fw;
   if (a.factor_s) a.factor_s[j] = fs;
   if (a.trials_w) a.trials_w[j] = !ran_w ? 0 : (dw >= 0 ? dw + 1 : a.n_fac_w[j]);
   if (a.trials_s) a.trials_s[j] = !ran_s ? 0 : (ds >= 0 ? ds + 1 : a.n_fac_s[j]);
-  const bool both = dw >= 0 && ds >= 0;
+  if (a.last_factor_safe && ds >= 0) a.last_factor_safe[j] = fs;
+  const bool both = dw >= 0 && (ds >= 0 || no_safe);
   double ni, nf;
   fqw::next_window(both, fw, a.gamma_w, a.gammap_w, iw, ew, &ni, &nf);
   if (a.next_init_w) a.next_init_w[j] = ni;
   if (a.next_final_w) a.next_final_w[j] = nf;
-  fqw::next_window(both, fs, a.gamma_s, a.gammap_s, is, es, &ni, &nf);
+  fqw::next_window(both, no_safe ? last_s : fs, a.gamma_s, a.gammap_s, is, es, &ni, &nf);
   if (a.next_init_s) a.next_init_s[j] = ni;
   if (a.next_final_s) a.next_final_s[j] = nf;
 }

@@ -165,12 +165,27 @@ int check_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, co
   return 0;
 }
 
+// the checks of fq_pair_hr that need no device memory (the chain with H and R needs the decomposing chain's arguments)
+int check_hr(fq_ctx* ctx, const fq_pair_window* win, const fq_pair_decomp* dc, const fq_pair_hr* hr)
+{
+  if (!hr) return fq_fail(ctx, FQ_E_ARG, "hr is NULL");
+  if (!dc) return fq_fail(ctx, FQ_E_ARG, "decomp is NULL");
+  if (!std::isfinite(hr->drone_radius) || hr->drone_radius < 0) return fq_fail(ctx, FQ_E_ARG, "hr: drone_radius must be finite and >= 0");
+  if (!std::isfinite(hr->delta_a) || !(hr->delta_a > 0)) return fq_fail(ctx, FQ_E_ARG, "hr: delta_a must be finite and > 0");
+  if (!(hr->delta_H >= 0 && hr->delta_H <= 1)) return fq_fail(ctx, FQ_E_ARG, "hr: delta_H must be in [0, 1]");
+  if (!hr->unk_ofs || !hr->unk) return fq_fail(ctx, FQ_E_ARG, "hr: unk_ofs / unk must not be NULL");
+  if (win && !hr->last_factor_safe) return fq_fail(ctx, FQ_E_ARG, "hr: last_factor_safe is required with a window");
+  return 0;
+}
+
 // the chain's intermediate arrays, carved from ctx->d_pair: those of both sweeps, and a SweepScratch per sweep
 struct Shared
 {
   double *x0_safe, *re_cost;            // R, the safe sweep's start states; the winners' re-solves (costs and flags)
   uint8_t* re_feas;
   int *win_ofs, *n_samples, *k_safe;
+  int* hr_r;                            // H and R from the unknown clouds: R's index (-1: no safe path) and needToComputeSafePath
+  uint8_t* hr_need;
   // decomposing chain: staging and spill, used by one sweep after the other
   double *dc_stage, *dc_spill;
   int* dc_stage_n;
@@ -287,7 +302,7 @@ long long longest_list(int N, int max_poly, long long all_limit)
 // the chain itself, every pointer a device pointer and every argument checked.  as == NULL: the shared lists of `a`;
 // sw: the two sweeps, their candidate counts set by the entry
 int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex,
-              const fq_pair_decomp* dc, const Sweep* sw, fq_pair_result* results_all, cudaStream_t st)
+              const fq_pair_decomp* dc, const fq_pair_hr* hr, const Sweep* sw, fq_pair_result* results_all, cudaStream_t st)
 {
   const int P = a->n_prob;
   // decomposing chain: staging slots of both sweeps (the larger), rows per slot, spilled survivors per slot
@@ -304,6 +319,7 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
     char* p = base;
     sh.x0_safe = carve<double>(p, (size_t)9 * P);  sh.re_cost = carve<double>(p, P);  sh.re_feas = carve<uint8_t>(p, P);
     sh.win_ofs = carve<int>(p, P + 1);  sh.n_samples = carve<int>(p, P);  sh.k_safe = carve<int>(p, P);
+    sh.hr_r = carve<int>(p, hr ? P : 0);  sh.hr_need = carve<uint8_t>(p, hr ? P : 0);
     sh.dc_stage = carve<double>(p, dslots * dcap * 4);    sh.dc_stage_n = carve<int>(p, dslots);
     sh.dc_spill = carve<double>(p, dslots * dspill * 4);  sh.dc_spill_flag = carve<uint8_t>(p, dslots * dspill);
     for (int i = 0; i < 2; i++)
@@ -415,10 +431,21 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
   double* coeffs_w = sw[0].coeffs ? sw[0].coeffs : ss[0].coeffs;
   if (int rc = run_sweep(sw[0], ss[0], a->x0, nullptr, coeffs_w, tree.changed_w)) return rc;
   // ---- R (faster.cpp:474-475) and the safe sweep from it (faster.cpp:521-537), in corridors around R when the chain
-  //      decomposes them; the exact stage re-solves its winners to confirm them, wanted or not
+  //      decomposes them; the exact stage re-solves its winners to confirm them, wanted or not.  With hr, H and R come
+  //      from the unknown clouds (faster.cpp:452-475), and a corridor that needs no safe path gets a NaN R, so that the
+  //      safe decomposition and sweep skip it as they skip a corridor without a whole winner.
   FqPairMidArgs m;
   m.n_prob = P; m.N = sw[0].N; m.DC = a->DC; m.r_fraction = a->r_fraction; m.coeffs = coeffs_w; m.win_dt = ss[0].win_dt;
   m.win_idx = ss[0].win_idx; m.x0_safe = sh.x0_safe; m.n_samples = sh.n_samples; m.k_safe = sh.k_safe;
+  if (hr)
+  {
+    FqPairHrArgs h;
+    h.n_prob = P; h.N = sw[0].N; h.DC = a->DC; h.drone_radius = hr->drone_radius; h.delta_a = hr->delta_a; h.delta_H = hr->delta_H;
+    h.coeffs = coeffs_w; h.win_dt = ss[0].win_dt; h.win_idx = ss[0].win_idx; h.lim = a->lim; h.unk_ofs = hr->unk_ofs; h.unk = hr->unk;
+    h.r_index = sh.hr_r; h.need = sh.hr_need; h.need_out = hr->need_safe; h.index_H = hr->index_H;
+    FQ_CUDA(fq_launch_pair_hr(h, st));
+    m.r_index = sh.hr_r;
+  }
   FQ_CUDA(fq_launch_pair_mid(m, st));
   double* coeffs_s = sw[1].coeffs ? sw[1].coeffs : ex ? ss[1].coeffs : nullptr;
   if (int rc = run_sweep(sw[1], ss[1], sh.x0_safe, sh.x0_safe, coeffs_s, tree.changed_s)) return rc;
@@ -455,6 +482,7 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
     wa.factor_w = sw[0].factor; wa.factor_s = sw[1].factor; wa.trials_w = sw[0].trials; wa.trials_s = sw[1].trials;
     wa.next_init_w = sw[0].next_init; wa.next_final_w = sw[0].next_final;
     wa.next_init_s = sw[1].next_init; wa.next_final_s = sw[1].next_final;
+    if (hr) { wa.need_safe = sh.hr_need; wa.last_factor_safe = hr->last_factor_safe; }
     FQ_CUDA(fq_launch_pair_window(wa, st));
   }
   // ---- the path's one exchange: every rank's result records to every rank (north_star: one all-gather, only when the
@@ -469,7 +497,7 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
 // the chains with per-corridor lists (fq_replan_pairs_assign_dev, _window_dev, _exact_dev, _decomp_dev): every pointer
 // of the structs is a device pointer; the sweeps' sizes come from the hints of `as` (capacities) and `win` (factor rows)
 int chain_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex,
-              const fq_pair_decomp* dc, fq_pair_result* results_all, void* stream_v)
+              const fq_pair_decomp* dc, fq_pair_result* results_all, void* stream_v, const fq_pair_hr* hr = nullptr)
 {
   if (!ctx) return FQ_E_ARG;
   if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
@@ -492,7 +520,7 @@ int chain_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
     w.ee_width = (int)longest;
   }
   FQ_CUDA(cudaSetDevice(ctx->device));
-  return run_chain(ctx, a, as, win, ex, dc, sw, results_all, stream_v ? (cudaStream_t)stream_v : ctx->stream);
+  return run_chain(ctx, a, as, win, ex, dc, hr, sw, results_all, stream_v ? (cudaStream_t)stream_v : ctx->stream);
 }
 }  // namespace
 
@@ -510,7 +538,7 @@ extern "C" int fq_replan_pairs_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_r
     w.ee_width = w.n_sig;
   }
   FQ_CUDA(cudaSetDevice(ctx->device));
-  return run_chain(ctx, a, nullptr, nullptr, nullptr, nullptr, sw, results_all, stream_v ? (cudaStream_t)stream_v : ctx->stream);
+  return run_chain(ctx, a, nullptr, nullptr, nullptr, nullptr, nullptr, sw, results_all, stream_v ? (cudaStream_t)stream_v : ctx->stream);
 }
 
 extern "C" int fq_replan_pairs_assign_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, fq_pair_result* results_all,
@@ -541,6 +569,15 @@ extern "C" int fq_replan_pairs_decomp_dev(fq_ctx* ctx, const fq_pair_args* a, co
   if (!ctx) return FQ_E_ARG;
   if (!dc) return fq_fail(ctx, FQ_E_ARG, "decomp is NULL");
   return chain_dev(ctx, a, as, win, ex, dc, results_all, stream_v);
+}
+
+extern "C" int fq_replan_pairs_hr_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
+                                      const fq_pair_exact* ex, const fq_pair_decomp* dc, const fq_pair_hr* hr, fq_pair_result* results_all,
+                                      void* stream_v)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (int rc = check_hr(ctx, win, dc, hr)) return rc;
+  return chain_dev(ctx, a, as, win, ex, dc, results_all, stream_v, hr);
 }
 
 const char* fq_list_offsets(int n_prob, const int* poly_ofs, int N, long all_limit, int n_fac, const double* init,
@@ -629,7 +666,8 @@ const char* scan_sweep(Sweep& w, int P, const fq_pair_assign* as, const fq_pair_
 }  // namespace
 
 int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results,
-                            const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex, const fq_pair_decomp* dc)
+                            const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex, const fq_pair_decomp* dc,
+                            const fq_pair_hr* hr)
 {
   if (!ctx) return FQ_E_ARG;
   if (int rc = fq_settle(ctx)) return rc;
@@ -640,6 +678,13 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   if (!fq_scan_all_positive_finite(a->lim, 3 * (size_t)P)) return fq_fail(ctx, FQ_E_ARG, "limits and factors must be finite and > 0");
   if (dc && dc->goal && !fq_scan_all_finite(dc->goal, 3 * (size_t)P))
     return fq_fail(ctx, FQ_E_ARG, "decomp: non-finite value in a path, a cloud or the goal");
+  int n_unk = 0, largest_unk = 0;
+  if (hr)
+  {
+    if (int rc = check_hr(ctx, win, dc, hr)) return rc;
+    if (!scan_offsets(hr->unk_ofs, P, 1 << 30, &n_unk, &largest_unk)) return fq_fail(ctx, FQ_E_ARG, "hr: unk_ofs must start at 0 and be non-decreasing");
+    if (!fq_scan_all_finite(hr->unk, 3 * (size_t)n_unk)) return fq_fail(ctx, FQ_E_ARG, "hr: non-finite value in an unknown cloud");
+  }
   FqCorridorSizes cs[2];
   int n_obs[2] = { 0, 0 };
   for (int i = 0; i < 2; i++)
@@ -652,6 +697,7 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   fq_pair_window dw{};
   fq_pair_exact dx{};
   fq_pair_decomp dd = dc ? *dc : fq_pair_decomp{};
+  fq_pair_hr dh = hr ? *hr : fq_pair_hr{};
   if (as) da.all_limit = as->all_limit;
   Sweep dv[2];
   char *hi = nullptr, *din = nullptr, *dout = nullptr;
@@ -687,6 +733,12 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
     d.lim = in(a->lim, 3 * (size_t)P);
     d.results = out(a->results, P);
     if (dc) dd.goal = in(dc->goal, 3 * (size_t)P);
+    if (hr)
+    { // last_factor_safe is updated in its uploaded copy, which goes back to the caller's array
+      dh.unk_ofs = in(hr->unk_ofs, P + 1);  dh.unk = in(hr->unk, 3 * (size_t)n_unk);
+      dh.last_factor_safe = in(hr->last_factor_safe, P);
+      dh.index_H = out(hr->index_H, P);  dh.need_safe = out(hr->need_safe, P);
+    }
     for (int i = 0; i < 2; i++)
     {
       const Sweep& w = sw[i];
@@ -710,7 +762,8 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   cudaStream_t st = ctx->stream;
   FQ_CUDA(cudaMemcpyAsync(din, hi, in_bytes, cudaMemcpyHostToDevice, st));
   for (int i = 0; i < 2; i++) put_sweep(dv[i], i, &d, &da, &dw, &dx, &dd);
-  int rc = dc ? fq_replan_pairs_decomp_dev(ctx, &d, &da, win ? &dw : nullptr, ex ? &dx : nullptr, &dd, nullptr, st)
+  int rc = hr ? fq_replan_pairs_hr_dev(ctx, &d, &da, win ? &dw : nullptr, ex ? &dx : nullptr, &dd, &dh, nullptr, st)
+         : dc ? fq_replan_pairs_decomp_dev(ctx, &d, &da, win ? &dw : nullptr, ex ? &dx : nullptr, &dd, nullptr, st)
          : ex ? fq_replan_pairs_exact_dev(ctx, &d, &da, win ? &dw : nullptr, &dx, nullptr, st)
          : win ? fq_replan_pairs_window_dev(ctx, &d, &da, &dw, nullptr, st)
          : as ? fq_replan_pairs_assign_dev(ctx, &d, &da, nullptr, st) : fq_replan_pairs_dev(ctx, &d, nullptr, st);
@@ -725,6 +778,12 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
       if (host && e == cudaSuccess) e = cudaMemcpyAsync(host, dev, sizeof(*host) * n, cudaMemcpyDeviceToHost, st);
     });
   FQ_CUDA(e);
+  if (hr)
+  {
+    if (hr->last_factor_safe) FQ_CUDA(cudaMemcpyAsync(hr->last_factor_safe, dh.last_factor_safe, sizeof(double) * P, cudaMemcpyDeviceToHost, st));
+    if (hr->index_H) FQ_CUDA(cudaMemcpyAsync(hr->index_H, dh.index_H, sizeof(int) * P, cudaMemcpyDeviceToHost, st));
+    if (hr->need_safe) FQ_CUDA(cudaMemcpyAsync(hr->need_safe, dh.need_safe, P, cudaMemcpyDeviceToHost, st));
+  }
   if (deferred) { ctx->pending = true; return 0; }
   FQ_CUDA(cudaStreamSynchronize(st));
   return 0;
@@ -747,13 +806,13 @@ namespace
 // chains run on one GPU only, since gathering their per-corridor exact / nodes / corridor arrays would need a second
 // exchange besides the records'.
 int lists_host(fq_ctx* ctx, const fq_pair_args* a, bool deferred, const fq_pair_assign* as, const fq_pair_window* win,
-               const fq_pair_exact* ex = nullptr, const fq_pair_decomp* dc = nullptr)
+               const fq_pair_exact* ex = nullptr, const fq_pair_decomp* dc = nullptr, const fq_pair_hr* hr = nullptr)
 {
   if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
   if ((ex || dc) && (ctx->is_group || ctx->comm))
-    return fq_fail(ctx, FQ_E_ARG, "fq_replan_pairs_exact / _decomp: multi-GPU contexts are not supported (use the _dev entry)");
+    return fq_fail(ctx, FQ_E_ARG, "fq_replan_pairs_exact / _decomp / _hr: multi-GPU contexts are not supported (use the _dev entry)");
   if (ctx->is_group || ctx->comm) return fq_replan_pairs_sharded(ctx, a, deferred, as, win);
-  return fq_replan_pairs_host_ex(ctx, a, deferred, nullptr, true, as, win, ex, dc);
+  return fq_replan_pairs_host_ex(ctx, a, deferred, nullptr, true, as, win, ex, dc, hr);
 }
 }  // namespace
 
@@ -801,4 +860,19 @@ extern "C" int fq_replan_pairs_decomp_async(fq_ctx* ctx, const fq_pair_args* a, 
 {
   if (!ctx) return FQ_E_ARG;
   return dc ? lists_host(ctx, a, true, as, win, ex, dc) : fq_fail(ctx, FQ_E_ARG, "decomp is NULL");
+}
+
+extern "C" int fq_replan_pairs_hr(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
+                                  const fq_pair_exact* ex, const fq_pair_decomp* dc, const fq_pair_hr* hr)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (int rc = check_hr(ctx, win, dc, hr)) return rc;
+  return lists_host(ctx, a, false, as, win, ex, dc, hr);
+}
+extern "C" int fq_replan_pairs_hr_async(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
+                                        const fq_pair_exact* ex, const fq_pair_decomp* dc, const fq_pair_hr* hr)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (int rc = check_hr(ctx, win, dc, hr)) return rc;
+  return lists_host(ctx, a, true, as, win, ex, dc, hr);
 }

@@ -47,7 +47,7 @@ typedef struct fq_ctx fq_ctx;     /* opaque: device, stream, plan tables, scratc
 
 int fq_abi_version(void);
 /* 1 if this build has the named feature: "sweep_early_exit", "replan_pairs", "multi_gpu", "row_tol", "certificates",
- * "replan_pairs_assign", "replan_pairs_window". */
+ * "replan_pairs_assign", "replan_pairs_window", "replan_pairs_exact", "replan_pairs_decomp", "replan_pairs_hr". */
 int fq_has_feature(const char* name);
 
 /* Threading: a context is used from one thread at a time, like a SolverGurobi instance in the reference (one replan
@@ -451,6 +451,56 @@ int fq_replan_pairs_decomp_async(fq_ctx* ctx, const fq_pair_args* args, const fq
  * into results_all as fq_replan_pairs_dev does. */
 int fq_replan_pairs_decomp_dev(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
                                const fq_pair_exact* exact, const fq_pair_decomp* decomp, fq_pair_result* results_all, void* stream);
+
+/* ---- chained replan that chooses H and R from each corridor's unknown space ------------------------------------------
+ *
+ * Faster::replan places R on the whole trajectory from the map (faster.cpp:452-538): findIndexH (:218-251) and findIndexR
+ * (:173-216).  The entry points below do that on the device, between the whole sweep and the safe corridor's decomposition,
+ * instead of the r_fraction rule (r_fraction is still validated but not used).  They are fq_replan_pairs_decomp* otherwise:
+ * `assign`, `decomp` and `hr` are required, `window` and `exact` optional.  Feature "replan_pairs_hr".
+ *
+ * Per corridor j whose whole winner has n = resetX samples X_temp_ (fillX's accumulated clock, the last sample at rest):
+ *   H   for i = 0, 10, 20, ... < n: q = sample i's position rounded to float (pcl::PointXYZ), d^2 = the minimum over the
+ *       corridor's unknown points p (rounded to float) of ((0 + dx^2) + dy^2) + dz^2 in float (FLANN's L2 order).  At the
+ *       first i with sqrtf(d^2) < drone_radius (compared in double): need_safe = 1, indexH = (int)(delta_H i).  Without
+ *       such a sample, or with an empty cloud: need_safe = 0, indexH = n - 1.  (FLANN's kd-tree may differ from this exact
+ *       float minimum only through the rounding of its pruning bounds; DESIGN.md 3.2.)
+ *   R   (need_safe = 1) k_safe = the first i in 0 .. indexH whose braking distance (sign(v (H - p)) v^2) / ((2 delta_a) a_max)
+ *       exceeds |H - p| in x or in y (double; sign(0) = 0; H = X_temp_[indexH], a_max = lim[3 j + 1]), else indexH.  R is
+ *       X_temp_[k_safe], bit-equal to fq_fill_x's sample.
+ *   need_safe = 0 (whole won): k_safe = n - 1, R NaN, no safe decomposition (status FQ_DECOMP_NOT_RUN), no safe sweep and
+ *       no safe winner; trials_safe 0.  The replan still succeeds: the next whole window follows the whole winner, the next
+ *       safe window is [max(last_factor_safe - gamma_safe, 1), last_factor_safe + gammap_safe] (faster.cpp:465-469,
+ *       :586-588).
+ *   no whole winner: index_H = -1, k_safe = -1, R NaN, as in fq_replan_pairs_decomp.
+ * last_factor_safe[j] becomes the safe winner's factor when the safe sweep wins and is unchanged otherwise; every window is
+ * read before anything is written, so the outputs may alias the inputs. */
+typedef struct fq_pair_hr
+{
+  const int* unk_ofs;        /* n_prob + 1: corridor j's unknown cloud is rows unk_ofs[j] .. unk_ofs[j+1]-1 of unk       */
+  const double* unk;         /* rows x 3; rounded to float on the device, as pcl::PointXYZ holds them. May point into obs_safe */
+  double drone_radius;       /* par_.drone_radius (findIndexH)                                                         */
+  double delta_a, delta_H;   /* par_.delta_a (findIndexR), par_.delta_H (findIndexH)                                   */
+  double* last_factor_safe;  /* in/out n_prob: the safe solver's factor_that_worked_ (0 at start-up).  Required with a window */
+  int* index_H;              /* out n_prob, or NULL: indexH (-1: no whole winner)                                      */
+  uint8_t* need_safe;        /* out n_prob, or NULL: needToComputeSafePath                                             */
+} fq_pair_hr;
+
+/* HOST pointers everywhere; blocks until every output is in the caller's arrays.  FQ_E_ARG: the refusals of
+ * fq_replan_pairs_decomp, hr NULL, drone_radius not finite or < 0, delta_a not finite or <= 0, delta_H outside [0, 1],
+ * unk_ofs or unk NULL, unk_ofs not starting at 0 or decreasing, a non-finite unknown value, a window without
+ * last_factor_safe, and multi-GPU contexts. */
+int fq_replan_pairs_hr(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
+                       const fq_pair_exact* exact, const fq_pair_decomp* decomp, const fq_pair_hr* hr);
+/* The same, returning once everything is enqueued; outputs are valid after fq_wait(ctx).  Arrays must stay alive. */
+int fq_replan_pairs_hr_async(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
+                             const fq_pair_exact* exact, const fq_pair_decomp* decomp, const fq_pair_hr* hr);
+/* DEVICE pointers everywhere (the structs live on the host), as fq_replan_pairs_decomp_dev; never synchronises.  Every
+ * thread of the H/R kernel walks the sample clock itself, so n has no cap.  On a rank context the records are all-gathered
+ * into results_all as fq_replan_pairs_dev does. */
+int fq_replan_pairs_hr_dev(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
+                           const fq_pair_exact* exact, const fq_pair_decomp* decomp, const fq_pair_hr* hr, fq_pair_result* results_all,
+                           void* stream);
 
 /* ---- several GPUs behind the boundary (SURVEY.md 8b/8e) ---------------------------------------------------------
  *
