@@ -9,7 +9,8 @@
 #define FQ_MIN_CTAS_PER_SM 4
 #endif
 #ifndef FQ_MIN_CTAS_WHOLE
-#define FQ_MIN_CTAS_WHOLE 4   // whole-mode kernels for N <= 10; 5 needs <= 96 registers and spills
+#define FQ_MIN_CTAS_WHOLE 4   // whole-mode kernels for N <= 10 (128 registers, no spills); 5 needs <= 96 registers, spills, and
+                              // measured slower on config 4 (DESIGN section 9)
 #endif
 #ifndef FQ_MAX_N_3CTAS
 #define FQ_MAX_N_3CTAS 15      // largest N whose kernels are compiled for 3 CTAs per SM (<= 168 registers); beyond: 2 CTAs.  N = 14, 15

@@ -343,13 +343,18 @@ __device__ __forceinline__ int build_items(const WarpState<D>& m, const int* __r
 // cannot be reached (0) or the iteration cap / a NaN is hit (-1).  Enabled rows = box rows + the `total_rows` items of
 // m.items.  Used by the fixed-assignment solve below and by the branch-and-bound node solve (fq_bnb.cuh), which enters
 // with a parent's factorisation instead of the identity.
-template <class D>
+// A box row's scale 1/dt^k (inv1..3) and limit (lim0..2) are held in registers through the iteration, except with
+// BOX_AT_ENTRY: then they are read through `dtp` (the time allocation dt) and `lim` (the problem's three limits) and
+// recomputed, bit for bit, where such a row enters.  That frees twelve registers in the N <= 10 solve kernels, which fill
+// the register file at 4 CTAs per SM and spilled without it; the other instances keep the registers.
+template <class D, bool BOX_AT_ENTRY = false>
 __device__ __forceinline__ int gi_loop(const WarpState<D>& m, const double* __restrict__ TZ, const double* __restrict__ SY,
                                        const double* __restrict__ sAb, const double (&Yeq)[D::RPL][3],
                                        const double (&bthr)[D::RPL], int lane, int total_rows, double inv1, double inv2,
                                        double inv3, double lim0, double lim1, double lim2, double row_tol,
                                        double (&lam)[D::SLOTS], double (&rdinv)[D::SLOTS], int& q, int& it, int bkey,
-                                       unsigned bcode)
+                                       unsigned bcode, const double* __restrict__ dtp = nullptr,
+                                       const double* __restrict__ lim = nullptr)
 {
   constexpr int N = D::N, NZ = D::NZ, NW = D::NW, NYP = D::NYP, LD = D::LD, SLOTS = D::SLOTS;
   double r[SLOTS], z[SLOTS], dreg[SLOTS];
@@ -389,8 +394,18 @@ __device__ __forceinline__ int gi_loop(const WarpState<D>& m, const double* __re
       y = code & 0xff;
       const int ax = (code >> 8) & 3;
       const double val = m.Y[ax * NYP + y];
-      const double sinv = y <= 2 * N ? inv1 : (y <= 3 * N ? inv2 : inv3);
-      h = y <= 2 * N ? lim0 : (y <= 3 * N ? lim1 : lim2);
+      double sinv;
+      if (BOX_AT_ENTRY)
+      { // inv2 = inv1 * inv1, inv3 = inv2 * inv1, as the callers compute them
+        const double i1 = 1.0 / *dtp;
+        sinv = y <= 2 * N ? i1 : (y <= 3 * N ? i1 * i1 : i1 * i1 * i1);
+        h = lim[y <= 2 * N ? 0 : (y <= 3 * N ? 1 : 2)];
+      }
+      else
+      {
+        sinv = y <= 2 * N ? inv1 : (y <= 3 * N ? inv2 : inv3);
+        h = y <= 2 * N ? lim0 : (y <= 3 * N ? lim1 : lim2);
+      }
       const double s = val > 0 ? sinv : -sinv;
       w0 = ax == 0 ? s : 0.0; w1 = ax == 1 ? s : 0.0; w2 = ax == 2 ? s : 0.0;
     }
@@ -627,6 +642,9 @@ __device__ void solve_candidate(const FqKernelArgs& a, const double* __restrict_
                                 int prob, int cand, int lane, int rows_bad)
 {
   constexpr int N = D::N, NW = D::NW, NYP = D::NYP, SLOTS = D::SLOTS;
+  // N <= 10: 4 CTAs per SM at 128 registers, the whole register file.  These instances keep nothing through the
+  // iteration that can be read or recomputed after it (gi_loop's BOX_AT_ENTRY); the others have registers to spare.
+  constexpr bool LEAN = N <= 10;
   const double dt = a.dt[cand];
   const double inv1 = 1.0 / dt, inv2 = inv1 * inv1, inv3 = inv2 * inv1;
   const double lim0 = a.lim[prob * 3 + 0], lim1 = a.lim[prob * 3 + 1], lim2 = a.lim[prob * 3 + 2];
@@ -732,10 +750,17 @@ __device__ void solve_candidate(const FqKernelArgs& a, const double* __restrict_
   int bkey = 0;
   unsigned bcode = 0;
   update_Y<D, true>(m, TZ, Yeq, bthr, SY, lane, bkey, bcode);
-  const int status = gi_loop<D>(m, TZ, SY, sAb, Yeq, bthr, lane, total_rows, inv1, inv2, inv3, lim0, lim1, lim2, a.row_tol,
-                                lam, rdinv, q, it, bkey, bcode);
+  const int status = gi_loop<D, LEAN>(m, TZ, SY, sAb, Yeq, bthr, lane, total_rows, inv1, inv2, inv3, lim0, lim1, lim2,
+                                      a.row_tol, lam, rdinv, q, it, bkey, bcode, a.dt + cand, a.lim + prob * 3);
 
   // ================= outputs =================
+#ifndef FQ_EMULATE_ON_HOST
+  // LEAN: the output addresses are formed here from the 32-bit index; the compiler would otherwise form them once before
+  // the solve (every exit path writes them) and hold them through the iteration
+  if (LEAN) asm("" : "+r"(cand));
+#endif
+  // LEAN: the scales are recomputed (bit for bit) rather than held through the iteration
+  const double oinv1 = LEAN ? 1.0 / dt : inv1, oinv2 = LEAN ? oinv1 * oinv1 : inv2, oinv3 = LEAN ? oinv2 * oinv1 : inv3;
   double cp = 0;
   if (status == 1)
     for (int i = lane; i < 3 * N; i += 32)
@@ -744,7 +769,7 @@ __device__ void solve_candidate(const FqKernelArgs& a, const double* __restrict_
       const double u = m.Y[ax * NYP + 3 * N + 1 + t];
       cp = fma(u, u, cp);
     }
-  const double cost = status == 1 ? warp_sum(cp) * (inv3 * inv3) : INFINITY;   // (status is warp-uniform)
+  const double cost = status == 1 ? warp_sum(cp) * (oinv3 * oinv3) : INFINITY;   // (status is warp-uniform)
   if (lane == 0)
   {
     a.feasible[cand] = status == 1;
@@ -760,9 +785,9 @@ __device__ void solve_candidate(const FqKernelArgs& a, const double* __restrict_
       const int t = idx / 12, c = idx - 12 * t, kind = c / 3, ax = c - 3 * kind;
       const double* Ya = m.Y + ax * NYP;
       double v;
-      if (kind == 0) v = Ya[3 * N + 1 + t] * inv3 * (1.0 / 6.0);
-      else if (kind == 1) v = Ya[2 * N + 1 + t] * inv2 * 0.5;
-      else if (kind == 2) v = Ya[N + 1 + t] * inv1;
+      if (kind == 0) v = Ya[3 * N + 1 + t] * oinv3 * (1.0 / 6.0);
+      else if (kind == 1) v = Ya[2 * N + 1 + t] * oinv2 * 0.5;
+      else if (kind == 2) v = Ya[N + 1 + t] * oinv1;
       else v = Ya[t];
       out[idx] = status == 1 ? v : 0.0;
     }
