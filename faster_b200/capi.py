@@ -19,7 +19,8 @@ EXPORTS = ["fq_abi_version", "fq_create", "fq_destroy", "fq_last_error", "fq_set
            "fq_pair_window_factors", "fq_replan_pairs_window", "fq_replan_pairs_window_async", "fq_replan_pairs_window_dev",
            "fq_replan_pairs_exact", "fq_replan_pairs_exact_async", "fq_replan_pairs_exact_dev", "fq_replan_pairs_decomp",
            "fq_replan_pairs_decomp_async", "fq_replan_pairs_decomp_dev", "fq_replan_pairs_hr", "fq_replan_pairs_hr_async",
-           "fq_replan_pairs_hr_dev"]
+           "fq_replan_pairs_hr_dev", "fq_map_create", "fq_map_destroy", "fq_map_update", "fq_map_update_dev", "fq_map_size",
+           "fq_replan_pairs_map", "fq_replan_pairs_map_async", "fq_replan_pairs_map_dev"]
 
 
 class FqError(RuntimeError):
@@ -91,6 +92,11 @@ class PairHR(C.Structure):
     """fq_pair_hr of include/faster_b200.h: the unknown clouds and parameters of findIndexH / findIndexR."""
     _fields_ = [("unk_ofs", C.c_void_p), ("unk", C.c_void_p), ("drone_radius", C.c_double), ("delta_a", C.c_double),
                 ("delta_H", C.c_double), ("last_factor_safe", C.c_void_p), ("index_H", C.c_void_p), ("need_safe", C.c_void_p)]
+
+
+class PairMap(C.Structure):
+    """fq_pair_map of include/faster_b200.h: the indexed maps the corridors of a submission read."""
+    _fields_ = [("maps", C.c_void_p), ("n_maps", C.c_int), ("map_index", C.c_void_p), ("max_local", C.c_int)]
 
 
 HR_OUT_KEYS = ["last_factor_safe", "index_H", "need_safe"]
@@ -169,6 +175,15 @@ def lib():
         L.fq_replan_pairs_hr.argtypes = L.fq_replan_pairs_decomp.argtypes + [C.POINTER(PairHR)]
         L.fq_replan_pairs_hr_async.argtypes = L.fq_replan_pairs_hr.argtypes
         L.fq_replan_pairs_hr_dev.argtypes = L.fq_replan_pairs_hr.argtypes + [C.c_void_p, C.c_void_p]
+        L.fq_replan_pairs_map.argtypes = L.fq_replan_pairs_hr.argtypes + [C.POINTER(PairMap)]
+        L.fq_replan_pairs_map_async.argtypes = L.fq_replan_pairs_map.argtypes
+        L.fq_replan_pairs_map_dev.argtypes = L.fq_replan_pairs_map.argtypes + [C.c_void_p, C.c_void_p]
+        L.fq_map_create.argtypes = [C.POINTER(C.c_void_p), C.c_int]
+        L.fq_map_destroy.argtypes = [C.c_void_p]
+        L.fq_map_destroy.restype = None
+        L.fq_map_update.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
+        L.fq_map_update_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p]
+        L.fq_map_size.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         L.fq_create_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_void_p]
         L.fq_comm_unique_id.argtypes = [C.c_void_p]
         L.fq_comm_init.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
@@ -305,6 +320,61 @@ def hr_args(unk_ofs, unk, out_ptrs, drone_radius=HR_DEFAULTS["drone_radius"], de
     for k in HR_OUT_KEYS:
         setattr(s, k, out_ptrs.get(k) or None)
     return s
+
+
+def map_args(maps, map_index=None, max_local=4096):
+    """PairMap over a list of Map objects; map_index: None (every corridor uses maps[0]), an int32 array (host) or a
+    device address (for replan_pairs_map_dev).  The returned struct keeps what it points to alive."""
+    s = PairMap()
+    s.table = (C.c_void_p * len(maps))(*[m.handle for m in maps])
+    s.maps, s.n_maps, s.max_local = C.addressof(s.table), len(maps), int(max_local)
+    if map_index is None or isinstance(map_index, int):
+        s.map_index = map_index or None
+    else:
+        s.index = np.ascontiguousarray(map_index, np.int32)
+        s.map_index = s.index.ctypes.data
+    return s
+
+
+class Map:
+    """An indexed map on one GPU (fq_map_*): the occupied cloud O and the unknown cloud U of one mapper message, uploaded
+    and bucketed once, then read by every corridor and replan that names it (Solver.replan_pairs_map)."""
+
+    def __init__(self, device=0):
+        self._L = lib()
+        h = C.c_void_p()
+        rc = self._L.fq_map_create(C.byref(h), int(device))
+        if rc != 0:
+            raise FqError("fq_map_create failed (%d): %s" % (rc, self._L.fq_last_error(None).decode()))
+        self.handle = h.value
+
+    def update(self, occ, unk):
+        """Host clouds (m x 3 each, either may be empty); blocks until the map holds them."""
+        occ = np.ascontiguousarray(np.reshape(occ, (-1, 3)), np.float64)
+        unk = np.ascontiguousarray(np.reshape(unk, (-1, 3)), np.float64)
+        rc = self._L.fq_map_update(self.handle, occ.ctypes.data if len(occ) else None, len(occ),
+                                   unk.ctypes.data if len(unk) else None, len(unk))
+        if rc != 0:
+            raise FqError("fq_map_update failed (%d): %s" % (rc, self._L.fq_last_error(None).decode()))
+
+    def update_dev(self, d_occ, n_occ, d_unk, n_unk, stream=0):
+        """Device clouds (addresses of n x 3 doubles), stream-ordered."""
+        rc = self._L.fq_map_update_dev(self.handle, d_occ or None, int(n_occ), d_unk or None, int(n_unk), stream or None)
+        if rc != 0:
+            raise FqError("fq_map_update_dev failed (%d): %s" % (rc, self._L.fq_last_error(None).decode()))
+
+    def size(self):
+        """-> (n_occ, n_unk) of the last update."""
+        o, u = C.c_int(0), C.c_int(0)
+        self._L.fq_map_size(self.handle, C.byref(o), C.byref(u))
+        return o.value, u.value
+
+    def close(self):
+        if getattr(self, "handle", None):
+            self._L.fq_map_destroy(self.handle)
+            self.handle = None
+
+    __del__ = close
 
 
 def make_decomp_workload(pairs, max_faces=400, max_poly_faces=64):
@@ -660,10 +730,41 @@ class Solver:
         self._check(fn(self._h, *structs, C.byref(hr)))
         return out
 
+    def replan_pairs_map(self, w, maps, map_index=None, max_local=4096, hr=True, last_factor_safe=None,
+                         drone_radius=HR_DEFAULTS["drone_radius"], delta_a=HR_DEFAULTS["delta_a"], delta_H=HR_DEFAULTS["delta_H"],
+                         all_limit=0, windows=None, inc=1.0, gamma=20.0, exact=False, bbox=(2.0, 2.0, 1.0), inflate=0.42,
+                         z_ground=0.0, use_goal=True, want_candidates=False, want_coeffs=True, deferred=False):
+        """fq_replan_pairs_map on a make_decomp_workload dict (its clouds obs_* / unk are not used): every corridor reads the
+        Map maps[map_index[j]] (map_index None: maps[0]).  hr=True: as replan_pairs_hr, with corridor j's unknown cloud U
+        and occupied cloud O from its map (whole: O, safe: U ++ O); hr=False: as replan_pairs_decomp.  max_local caps the
+        points of one segment inside its local box.  -> the dict of replan_pairs_hr (hr=True) or replan_pairs_decomp."""
+        n = w["n_prob"]
+        extra = {}
+        if hr:
+            last = np.zeros(n) if last_factor_safe is None else np.array(last_factor_safe, np.float64).reshape(n)
+            extra = dict(last_factor_safe=last, index_H=np.zeros(n, np.int32), need_safe=np.zeros(n, np.uint8))
+        out, structs = self._decomp_structs(w, all_limit, windows, inc, gamma, exact, bbox, inflate, z_ground, use_goal,
+                                            want_candidates, want_coeffs, extra, clouds=False)
+        h = hr_args(None, None, {k: out[k].ctypes.data for k in HR_OUT_KEYS}, drone_radius, delta_a, delta_H) if hr else None
+        mp = map_args(maps, map_index, max_local)
+        fn = self._L.fq_replan_pairs_map_async if deferred else self._L.fq_replan_pairs_map
+        self._check(fn(self._h, *structs, C.byref(h) if h is not None else None, C.byref(mp)))
+        if deferred:
+            out["_keep"] = mp
+        return out
+
+    def replan_pairs_map_dev(self, a, s, win, ex, dc, hr, mp, results_all=0, stream=0):
+        """fq_replan_pairs_map_dev: as replan_pairs_hr_dev (hr may be None), with `mp` (PairMap, map_args) whose map_index is
+        a device address or None."""
+        self._check(self._L.fq_replan_pairs_map_dev(self._h, C.byref(a), C.byref(s), C.byref(win) if win is not None else None,
+                                                    C.byref(ex) if ex is not None else None, C.byref(dc),
+                                                    C.byref(hr) if hr is not None else None, C.byref(mp), results_all or None,
+                                                    stream or None))
+
     def _decomp_structs(self, w, all_limit, windows, inc, gamma, exact, bbox, inflate, z_ground, use_goal, want_candidates,
-                        want_coeffs, extra_out=()):
+                        want_coeffs, extra_out=(), clouds=True):
         """The returned arrays and the (PairArgs, PairAssign, PairWindow, PairExact, PairDecomp) arguments of
-        replan_pairs_decomp / replan_pairs_hr (ctypes references or None)."""
+        replan_pairs_decomp / replan_pairs_hr (ctypes references or None).  clouds=False: obs_* NULL (replan_pairs_map)."""
         n, Nw, Ns = w["n_prob"], w["N_whole"], w["N_safe"]
         extra = dict(face_ofs_whole=np.zeros(int(w["poly_ofs_whole"][-1]) + 1, np.int32), face_ofs_safe=np.zeros(int(w["poly_ofs_safe"][-1]) + 1, np.int32),
                      Ab_whole=np.zeros((n * w["max_faces_whole"], 4)), Ab_safe=np.zeros((n * w["max_faces_safe"], 4)),
@@ -685,7 +786,7 @@ class Solver:
         for k in ("max_faces_whole", "max_poly_faces_whole", "max_faces_safe", "max_poly_faces_safe"):
             setattr(a, k, int(w[k]))
         ex = exact_args({k: out[k].ctypes.data for k in EXACT_KEYS}) if exact else None
-        dc = decomp_args(lambda k: None if (k == "goal" and not use_goal) else w[k].ctypes.data,
+        dc = decomp_args(lambda k: None if (k == "goal" and not use_goal) or (not clouds and k.startswith("obs_")) else w[k].ctypes.data,
                          {k: out[k].ctypes.data for k in DECOMP_OUT_KEYS}, bbox, inflate, z_ground)
         return out, [C.byref(x) if x is not None else None for x in (a, s, wa, ex, dc)]
 

@@ -126,7 +126,13 @@ const char* fq_list_offsets(int n_prob, const int* poly_ofs, int N, long all_lim
 // (fq_replan_pairs_window*, host pointers); ex != NULL (with as): the exact stage (fq_replan_pairs_exact*, host pointers)
 int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results,
                             const fq_pair_assign* as = nullptr, const fq_pair_window* win = nullptr,
-                            const fq_pair_exact* ex = nullptr, const fq_pair_decomp* dc = nullptr, const fq_pair_hr* hr = nullptr);
+                            const fq_pair_exact* ex = nullptr, const fq_pair_decomp* dc = nullptr, const fq_pair_hr* hr = nullptr,
+                            const fq_pair_map* mp = nullptr);
+// fq_map.cu: the device address of a map's descriptor (fixed for the map's life, rewritten by every update), its device,
+// and whether its last update succeeded
+const FqMapDev* fq_map_descriptor(const fq_map* m);
+int fq_map_device(const fq_map* m);
+bool fq_map_valid(const fq_map* m);
 // fq_multi.cu
 void fq_comm_release(fq_ctx* ctx);
 // all-gather on one context's communicator (one process per GPU): `bytes` from every rank, rank order

@@ -789,3 +789,19 @@ cudaError_t fq_launch_decomp(const FqDecompArgs& a, cudaStream_t stream)
   fqd::fq_decomp_csr_kernel<<<1, 1024, 0, stream>>>(a);
   return cudaGetLastError();
 }
+
+namespace
+{
+__global__ void fq_map_table_kernel(const FqMapTableChunk c)
+{
+  const int i = threadIdx.x;
+  if (i < c.n) c.table[c.at + i] = c.m[i];
+}
+}  // namespace
+
+cudaError_t fq_launch_map_table(const FqMapTableChunk& c, cudaStream_t stream)
+{
+  if (c.n <= 0) return cudaSuccess;
+  fq_map_table_kernel<<<1, FqMapTableChunk::kCap, 0, stream>>>(c);
+  return cudaGetLastError();
+}

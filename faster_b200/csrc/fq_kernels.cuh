@@ -3,6 +3,7 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 #include "../../include/faster_b200.h"
+#include "fq_map.h"
 
 #define FQ_WARPS_PER_CTA 4
 #ifndef FQ_MIN_CTAS_PER_SM
@@ -220,6 +221,10 @@ struct FqPairHrArgs
   uint8_t* need;                        // out n_prob: needToComputeSafePath (0 without a whole winner)
   uint8_t* need_out;                    // out n_prob, or NULL: a copy for the caller
   int* index_H;                         // out n_prob, or NULL: indexH (-1 without a whole winner)
+  // fq_replan_pairs_map*: corridor j's unknown cloud is the U of maps[map_index[j]] (map_index NULL: maps[0]) in place of
+  // unk_ofs / unk, and only its cells near the sample are read
+  const FqMapDev* const* maps = nullptr;
+  const int* map_index = nullptr;
 };
 
 struct FqPairFinalArgs
@@ -297,6 +302,14 @@ struct FqDecompArgs
   double* xf;                           // out: n_prob x 9 final states (NaN rows for failed corridors)
   double* pos_out;                      // out n_prob x 3, or NULL
   int* status;                          // out n_prob, or NULL
+  // fq_replan_pairs_map*: an indexed map in place of obs_ofs / obs.  Corridor j reads maps[map_index[j]] (map_index NULL:
+  // maps[0]; outside 0 .. n_maps-1: FQ_DECOMP_CLOUD): its occupied cloud O (map_unk 0), or its unknown cloud U followed by
+  // O (map_unk 1, O's indices after U's), in the cells the segment's AABB overlaps.  max_obs then caps the survivors of one
+  // segment, and spill_idx (spill_n per slot) holds the spilled survivors' indices in the cloud.
+  const FqMapDev* const* maps = nullptr;
+  const int* map_index = nullptr;
+  int n_maps = 0, map_unk = 0;
+  int* spill_idx = nullptr;
 };
 size_t fq_decomp_spill_n(int max_obs);
 cudaError_t fq_launch_decomp(const FqDecompArgs& a, cudaStream_t stream);
@@ -324,4 +337,15 @@ cudaError_t fq_launch_pair_window(const FqPairWindowArgs& a, cudaStream_t stream
 cudaError_t fq_launch_select_multi(const FqSelectMultiArgs& a, cudaStream_t stream);
 cudaError_t fq_launch_pair_mid(const FqPairMidArgs& a, cudaStream_t stream);
 cudaError_t fq_launch_pair_hr(const FqPairHrArgs& a, cudaStream_t stream);
+// the map table of one submission: table[at + i] = m[i] for i < n, the device addresses of the maps' descriptors (they
+// pass through kernel parameters, so that the table needs no host copy and a CUDA graph can capture it; the descriptors
+// never move, so a replay reads each map's last update)
+struct FqMapTableChunk
+{
+  static constexpr int kCap = 64;
+  const FqMapDev* m[kCap];
+  int n, at;
+  const FqMapDev** table;
+};
+cudaError_t fq_launch_map_table(const FqMapTableChunk& c, cudaStream_t stream);
 cudaError_t fq_launch_pair_final(const FqPairFinalArgs& a, cudaStream_t stream);

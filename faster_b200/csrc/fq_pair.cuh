@@ -275,7 +275,10 @@ __global__ void fq_pair_mid_kernel(const FqPairMidArgs a)
 //      with pcl::PointXYZ's float coordinates and FLANN's float L2 order ((0 + dx^2) + dy^2) + dz^2; the first sample with
 //      sqrtf(d^2) < drone_radius (in double) sets needToComputeSafePath and indexH = (int)(delta_H i); none: indexH = n - 1.
 //      Since sqrtf is monotone, "the nearest point is that close" is "some point is that close": the CTA scans the cloud for
-//      any such point (__syncthreads_or), which neither thread count nor warp order can change.
+//      any such point (__syncthreads_or), which neither thread count nor warp order can change.  With an indexed map
+//      (fq_map.h) it scans only the cells within drone_radius of the sample, widened by a bound on the float rounding of
+//      the point and of the distance ((|q| + drone_radius) 2^-20, far above it) and by one cell: they hold every point that
+//      close, at any coordinate magnitude.
 //   R: the first i in 0 .. indexH whose braking distance sign(v (H - p)) v^2 / (2 delta_a a_max) exceeds |H - p| in x or y,
 //      else indexH.  Threads take strided samples, each walking its own sample clock; the first index is a block minimum.
 #if defined(__CUDA_ARCH__)
@@ -331,7 +334,8 @@ __global__ void __launch_bounds__(256) fq_pair_hr_kernel(const FqPairHrArgs a)
   const double dt = a.win_dt[j], DC = a.DC;
   const int N = a.N, n = fqdt::num_samples(N, dt, DC);
   const double* co = a.coeffs + (size_t)j * N * 12;
-  const int lo = a.unk_ofs[j], hi = a.unk_ofs[j + 1];
+  const FqMapDev* M = a.maps ? a.maps[a.map_index ? a.map_index[j] : 0] : nullptr;
+  const int lo = M ? 0 : a.unk_ofs[j], hi = M ? M->unk.n : a.unk_ofs[j + 1];
   SampleClock c0;                                                   // thread 0's clock through the H queries
   int hit_i = -1;
   for (int i = 0; i < n && hi > lo; i += 10)
@@ -345,8 +349,30 @@ __global__ void __launch_bounds__(256) fq_pair_hr_kernel(const FqPairHrArgs a)
     __syncthreads();
     const float q[3] = { s_q[0], s_q[1], s_q[2] };
     int near = 0;
-    for (int p = lo + tid; p < hi && !near; p += T)
-      near = (double)FQ_FSQRT(flann_l2(q, a.unk + 3 * (size_t)p)) < a.drone_radius;
+    if (!M)
+      for (int p = lo + tid; p < hi && !near; p += T)
+        near = (double)FQ_FSQRT(flann_l2(q, a.unk + 3 * (size_t)p)) < a.drone_radius;
+    else
+    {
+      const FqMapGrid& g = M->grid;
+      double qlo[3], qhi[3];
+      for (int k = 0; k < 3; k++)
+      {
+        const double r = a.drone_radius + (fabs((double)q[k]) + a.drone_radius) * 0x1p-20;
+        qlo[k] = (double)q[k] - r; qhi[k] = (double)q[k] + r;
+      }
+      int cl[3], ch[3];
+      fq_map_range(g, qlo, qhi, cl, ch);
+      for (int k = 0; k < 3; k++) { cl[k] = cl[k] > 0 ? cl[k] - 1 : 0; ch[k] = ch[k] < g.dims[k] - 1 ? ch[k] + 1 : g.dims[k] - 1; }
+      const int rows = (ch[1] - cl[1] + 1) * (ch[2] - cl[2] + 1);
+      for (int r = 0; r < rows && !near; r++)
+      {
+        int b, e;
+        fq_map_row(g, M->unk, cl, ch, r, &b, &e);
+        for (int p = b + tid; p < e && !near; p += T)
+          near = (double)FQ_FSQRT(flann_l2(q, M->unk.xyz + 3 * (size_t)p)) < a.drone_radius;
+      }
+    }
     if (__syncthreads_or(near)) { hit_i = i; break; }               // also the barrier before s_q is written again
   }
   if (hit_i < 0) { put(-1, 0, n - 1); return; }

@@ -108,7 +108,8 @@ void put_sweep(const Sweep& s, int side, fq_pair_args* a, fq_pair_assign* as, fq
 // the checks of one sweep that need no device memory.  as == NULL: one shared assignment list (sigmas); otherwise a list
 // per corridor, whose candidate counts the callers check.  win: per-corridor windows instead of the factor list.  dc: the
 // chain decomposes the corridors, so the sweep has no faces and no final states.
-const char* check_sweep(const Sweep& w, int n_prob, const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_decomp* dc)
+const char* check_sweep(const Sweep& w, int n_prob, const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_decomp* dc,
+                        const fq_pair_map* mp)
 {
   if (w.N < (w.force_final ? 3 : 2) || w.N > FQ_MAX_N) return "N out of range";
   if (!as)
@@ -135,7 +136,8 @@ const char* check_sweep(const Sweep& w, int n_prob, const fq_pair_assign* as, co
   }
   if (dc)
   {
-    if (!w.path || !w.obs_ofs || !w.obs) return "decomp: path_* / obs_ofs_* / obs_* must not be NULL";
+    if (!w.path || (!mp && (!w.obs_ofs || !w.obs))) return "decomp: path_* / obs_ofs_* / obs_* must not be NULL";
+    if (mp && (w.obs_ofs || w.obs)) return "map: obs_ofs_* and obs_* must be NULL (the maps hold the clouds)";
     if ((uintptr_t)w.Ab_out & 15) return "decomp: Ab_* must be 16-byte aligned";
   }
   return nullptr;
@@ -143,7 +145,7 @@ const char* check_sweep(const Sweep& w, int n_prob, const fq_pair_assign* as, co
 
 // the checks every entry makes, and the two sweeps of the call (see check_sweep)
 int check_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex,
-                const fq_pair_decomp* dc, Sweep* sw)
+                const fq_pair_decomp* dc, Sweep* sw, const fq_pair_map* mp = nullptr)
 {
   if (!a) return fq_fail(ctx, FQ_E_ARG, "args is NULL");
   if ((win || ex || dc) && !as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
@@ -160,21 +162,41 @@ int check_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, co
   for (int i = 0; i < 2; i++)
   {
     sw[i] = sweep_of(i, a, as, win, ex, dc);
-    if (const char* why = check_sweep(sw[i], a->n_prob, as, win, dc)) return fq_fail(ctx, FQ_E_ARG, why);
+    if (const char* why = check_sweep(sw[i], a->n_prob, as, win, dc, mp)) return fq_fail(ctx, FQ_E_ARG, why);
   }
   return 0;
 }
 
-// the checks of fq_pair_hr that need no device memory (the chain with H and R needs the decomposing chain's arguments)
-int check_hr(fq_ctx* ctx, const fq_pair_window* win, const fq_pair_decomp* dc, const fq_pair_hr* hr)
+// the checks of fq_pair_hr that need no device memory (the chain with H and R needs the decomposing chain's arguments).
+// map: the unknown clouds come from maps, so unk_ofs / unk must be NULL.
+int check_hr(fq_ctx* ctx, const fq_pair_window* win, const fq_pair_decomp* dc, const fq_pair_hr* hr, bool map = false)
 {
   if (!hr) return fq_fail(ctx, FQ_E_ARG, "hr is NULL");
   if (!dc) return fq_fail(ctx, FQ_E_ARG, "decomp is NULL");
   if (!std::isfinite(hr->drone_radius) || hr->drone_radius < 0) return fq_fail(ctx, FQ_E_ARG, "hr: drone_radius must be finite and >= 0");
   if (!std::isfinite(hr->delta_a) || !(hr->delta_a > 0)) return fq_fail(ctx, FQ_E_ARG, "hr: delta_a must be finite and > 0");
   if (!(hr->delta_H >= 0 && hr->delta_H <= 1)) return fq_fail(ctx, FQ_E_ARG, "hr: delta_H must be in [0, 1]");
-  if (!hr->unk_ofs || !hr->unk) return fq_fail(ctx, FQ_E_ARG, "hr: unk_ofs / unk must not be NULL");
+  if (map && (hr->unk_ofs || hr->unk)) return fq_fail(ctx, FQ_E_ARG, "map: hr->unk_ofs and hr->unk must be NULL (the maps hold the clouds)");
+  if (!map && (!hr->unk_ofs || !hr->unk)) return fq_fail(ctx, FQ_E_ARG, "hr: unk_ofs / unk must not be NULL");
   if (win && !hr->last_factor_safe) return fq_fail(ctx, FQ_E_ARG, "hr: last_factor_safe is required with a window");
+  return 0;
+}
+
+// the checks of fq_pair_map that need no device memory (map_index is checked by the host entries)
+int check_map(fq_ctx* ctx, const fq_pair_decomp* dc, const fq_pair_hr* hr, const fq_pair_window* win, const fq_pair_map* mp)
+{
+  if (!mp) return fq_fail(ctx, FQ_E_ARG, "map is NULL");
+  if (!dc) return fq_fail(ctx, FQ_E_ARG, "decomp is NULL");
+  if (hr)
+    if (int rc = check_hr(ctx, win, dc, hr, true)) return rc;
+  if (!mp->maps || mp->n_maps <= 0) return fq_fail(ctx, FQ_E_ARG, "map: no maps");
+  for (int i = 0; i < mp->n_maps; i++)
+  {
+    if (!mp->maps[i]) return fq_fail(ctx, FQ_E_ARG, "map: a NULL map");
+    if (fq_map_device(mp->maps[i]) != ctx->device) return fq_fail(ctx, FQ_E_ARG, "map: a map on another device");
+    if (!fq_map_valid(mp->maps[i])) return fq_fail(ctx, FQ_E_ARG, "map: a map whose last update failed");
+  }
+  if (mp->max_local < 0 || mp->max_local > (1 << 30)) return fq_fail(ctx, FQ_E_ARG, "map: max_local out of range (0..2^30)");
   return 0;
 }
 
@@ -190,6 +212,9 @@ struct Shared
   double *dc_stage, *dc_spill;
   int* dc_stage_n;
   uint8_t* dc_spill_flag;
+  // against maps: the spilled survivors' cloud indices, and the submission's map table
+  int* dc_spill_idx;
+  const FqMapDev** map_table;
 };
 struct SweepScratch
 {
@@ -302,7 +327,8 @@ long long longest_list(int N, int max_poly, long long all_limit)
 // the chain itself, every pointer a device pointer and every argument checked.  as == NULL: the shared lists of `a`;
 // sw: the two sweeps, their candidate counts set by the entry
 int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex,
-              const fq_pair_decomp* dc, const fq_pair_hr* hr, const Sweep* sw, fq_pair_result* results_all, cudaStream_t st)
+              const fq_pair_decomp* dc, const fq_pair_hr* hr, const fq_pair_map* mp, const Sweep* sw, fq_pair_result* results_all,
+              cudaStream_t st)
 {
   const int P = a->n_prob;
   // decomposing chain: staging slots of both sweeps (the larger), rows per slot, spilled survivors per slot
@@ -322,6 +348,7 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
     sh.hr_r = carve<int>(p, hr ? P : 0);  sh.hr_need = carve<uint8_t>(p, hr ? P : 0);
     sh.dc_stage = carve<double>(p, dslots * dcap * 4);    sh.dc_stage_n = carve<int>(p, dslots);
     sh.dc_spill = carve<double>(p, dslots * dspill * 4);  sh.dc_spill_flag = carve<uint8_t>(p, dslots * dspill);
+    sh.dc_spill_idx = carve<int>(p, mp ? dslots * dspill : 0);  sh.map_table = carve<const FqMapDev*>(p, mp ? mp->n_maps : 0);
     for (int i = 0; i < 2; i++)
     {
       const Sweep& w = sw[i];
@@ -340,6 +367,14 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
   };
   FQ_CUDA(ctx->d_pair.reserve(layout(nullptr)));   // grows only on the first call / a larger batch (synchronous cudaMalloc)
   layout((char*)ctx->d_pair.p);
+  if (mp)
+    for (int at = 0; at < mp->n_maps; at += FqMapTableChunk::kCap)
+    {
+      FqMapTableChunk c{};
+      c.n = std::min(FqMapTableChunk::kCap, mp->n_maps - at); c.at = at; c.table = sh.map_table;
+      for (int i = 0; i < c.n; i++) c.m[i] = fq_map_descriptor(mp->maps[at + i]);
+      FQ_CUDA(fq_launch_map_table(c, st));
+    }
   Tree tree{};
   const int stride = std::max(win ? std::max(sw[0].max_fac, sw[1].max_fac) : std::max(sw[0].n_fac, sw[1].n_fac), 1);
   if (ex)
@@ -354,7 +389,7 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
   // getDTInitial, the candidates, the batch solve, the selection, the exact stage (its tree flags to `changed`), and the
   // winners' coefficients into `coeffs` (NULL: not wanted).
   auto run_sweep = [&](const Sweep& w, SweepScratch& s, const double* x0, const double* first, double* coeffs,
-                       uint8_t* changed) -> int {
+                       uint8_t* changed, int side) -> int {
     FqKernelArgs corr{};                // the sweep's corridors; each launch adds its candidates and outputs
     corr.N = w.N; corr.force_final = w.force_final; corr.n_prob = P; corr.x0 = x0; corr.xf = w.xf; corr.lim = a->lim;
     corr.poly_ofs = w.poly_ofs; corr.face_ofs = w.face_ofs; corr.Ab = w.Ab; corr.max_faces = w.max_faces;
@@ -370,6 +405,10 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
       x.goal = dc->goal; x.face_cap = P * x.max_poly;
       x.face_ofs = w.face_ofs_out ? w.face_ofs_out : s.dc_face; x.Ab = w.Ab_out ? w.Ab_out : s.dc_Ab; x.xf = s.dc_xf;
       x.pos_out = w.pos_out; x.status = w.status;
+      if (mp)
+      { // the whole sweep reads O, the safe sweep U ++ O (faster.cpp:130-132)
+        x.maps = sh.map_table; x.map_index = mp->map_index; x.n_maps = mp->n_maps; x.map_unk = side; x.spill_idx = sh.dc_spill_idx;
+      }
       FQ_CUDA(fq_launch_decomp(x, st));
       corr.face_ofs = x.face_ofs; corr.Ab = x.Ab; corr.xf = x.xf;
     }
@@ -429,7 +468,7 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
       FQ_CUDA(fq_launch_window_factors(P, sw[i].max_fac, sw[i].init, sw[i].final_, sw[i].inc, ss[i].fac, ss[i].nf, st));
   // ---- whole sweep (faster.cpp:406-430); R needs its winners' coefficients
   double* coeffs_w = sw[0].coeffs ? sw[0].coeffs : ss[0].coeffs;
-  if (int rc = run_sweep(sw[0], ss[0], a->x0, nullptr, coeffs_w, tree.changed_w)) return rc;
+  if (int rc = run_sweep(sw[0], ss[0], a->x0, nullptr, coeffs_w, tree.changed_w, 0)) return rc;
   // ---- R (faster.cpp:474-475) and the safe sweep from it (faster.cpp:521-537), in corridors around R when the chain
   //      decomposes them; the exact stage re-solves its winners to confirm them, wanted or not.  With hr, H and R come
   //      from the unknown clouds (faster.cpp:452-475), and a corridor that needs no safe path gets a NaN R, so that the
@@ -443,12 +482,13 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
     h.n_prob = P; h.N = sw[0].N; h.DC = a->DC; h.drone_radius = hr->drone_radius; h.delta_a = hr->delta_a; h.delta_H = hr->delta_H;
     h.coeffs = coeffs_w; h.win_dt = ss[0].win_dt; h.win_idx = ss[0].win_idx; h.lim = a->lim; h.unk_ofs = hr->unk_ofs; h.unk = hr->unk;
     h.r_index = sh.hr_r; h.need = sh.hr_need; h.need_out = hr->need_safe; h.index_H = hr->index_H;
+    if (mp) { h.maps = sh.map_table; h.map_index = mp->map_index; }
     FQ_CUDA(fq_launch_pair_hr(h, st));
     m.r_index = sh.hr_r;
   }
   FQ_CUDA(fq_launch_pair_mid(m, st));
   double* coeffs_s = sw[1].coeffs ? sw[1].coeffs : ex ? ss[1].coeffs : nullptr;
-  if (int rc = run_sweep(sw[1], ss[1], sh.x0_safe, sh.x0_safe, coeffs_s, tree.changed_s)) return rc;
+  if (int rc = run_sweep(sw[1], ss[1], sh.x0_safe, sh.x0_safe, coeffs_s, tree.changed_s, 1)) return rc;
 
   FqPairFinalArgs f;
   f.n_prob = P; f.n_sig_w = sw[0].n_sig; f.n_sig_s = sw[1].n_sig; f.win_idx_w = ss[0].win_idx; f.win_idx_s = ss[1].win_idx;
@@ -497,18 +537,20 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
 // the chains with per-corridor lists (fq_replan_pairs_assign_dev, _window_dev, _exact_dev, _decomp_dev): every pointer
 // of the structs is a device pointer; the sweeps' sizes come from the hints of `as` (capacities) and `win` (factor rows)
 int chain_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex,
-              const fq_pair_decomp* dc, fq_pair_result* results_all, void* stream_v, const fq_pair_hr* hr = nullptr)
+              const fq_pair_decomp* dc, fq_pair_result* results_all, void* stream_v, const fq_pair_hr* hr = nullptr,
+              const fq_pair_map* mp = nullptr)
 {
   if (!ctx) return FQ_E_ARG;
   if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
   Sweep sw[2];
-  if (int rc = check_chain(ctx, a, as, win, ex, dc, sw)) return rc;
+  if (int rc = check_chain(ctx, a, as, win, ex, dc, sw, mp)) return rc;
   if (as->all_limit < 0) return fq_fail(ctx, FQ_E_ARG, "all_limit < 0");
   for (Sweep& w : sw)
   {
     if (win && (w.max_fac < 0 || w.max_fac > fqw::kMaxFactors)) return fq_fail(ctx, FQ_E_ARG, "max_fac_* out of range (0..4096)");
     if (w.max_poly < 0 || w.max_poly > FQ_MAX_POLY) return fq_fail(ctx, FQ_E_ARG, "max_poly_* out of range (0..FQ_MAX_POLY)");
     if (w.n_cand < 0 || w.n_cand > (1L << 30)) return fq_fail(ctx, FQ_E_ARG, "too many candidates (n_cand_* out of 0..2^30)");
+    if (mp) w.max_obs = mp->max_local;                   // the survivors of one segment, not a cloud
     if (dc && w.max_obs < 0) return fq_fail(ctx, FQ_E_ARG, "decomp: max_obs_* < 0");
     if ((uintptr_t)w.Ab & 15) return fq_fail(ctx, FQ_E_ARG, "Ab must be 16-byte aligned");
     // the longest list is the candidates per time allocation; with the factors, the most candidates of one corridor
@@ -520,7 +562,7 @@ int chain_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
     w.ee_width = (int)longest;
   }
   FQ_CUDA(cudaSetDevice(ctx->device));
-  return run_chain(ctx, a, as, win, ex, dc, hr, sw, results_all, stream_v ? (cudaStream_t)stream_v : ctx->stream);
+  return run_chain(ctx, a, as, win, ex, dc, hr, mp, sw, results_all, stream_v ? (cudaStream_t)stream_v : ctx->stream);
 }
 }  // namespace
 
@@ -538,7 +580,8 @@ extern "C" int fq_replan_pairs_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_r
     w.ee_width = w.n_sig;
   }
   FQ_CUDA(cudaSetDevice(ctx->device));
-  return run_chain(ctx, a, nullptr, nullptr, nullptr, nullptr, nullptr, sw, results_all, stream_v ? (cudaStream_t)stream_v : ctx->stream);
+  return run_chain(ctx, a, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, sw, results_all,
+                   stream_v ? (cudaStream_t)stream_v : ctx->stream);
 }
 
 extern "C" int fq_replan_pairs_assign_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, fq_pair_result* results_all,
@@ -578,6 +621,15 @@ extern "C" int fq_replan_pairs_hr_dev(fq_ctx* ctx, const fq_pair_args* a, const 
   if (!ctx) return FQ_E_ARG;
   if (int rc = check_hr(ctx, win, dc, hr)) return rc;
   return chain_dev(ctx, a, as, win, ex, dc, results_all, stream_v, hr);
+}
+
+extern "C" int fq_replan_pairs_map_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
+                                       const fq_pair_exact* ex, const fq_pair_decomp* dc, const fq_pair_hr* hr, const fq_pair_map* mp,
+                                       fq_pair_result* results_all, void* stream_v)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (int rc = check_map(ctx, dc, hr, win, mp)) return rc;
+  return chain_dev(ctx, a, as, win, ex, dc, results_all, stream_v, hr, mp);
 }
 
 const char* fq_list_offsets(int n_prob, const int* poly_ofs, int N, long all_limit, int n_fac, const double* init,
@@ -637,8 +689,9 @@ const char* scan_sweep(Sweep& w, int P, const fq_pair_assign* as, const fq_pair_
     int mp = 0;
     w.max_obs = 0;
     if (!scan_offsets(w.poly_ofs, P, FQ_MAX_POLY, &c->n_poly, &mp)) return "poly_ofs_* must start at 0 and step by 0..FQ_MAX_POLY";
-    if (!scan_offsets(w.obs_ofs, P, 1 << 30, n_obs, &w.max_obs)) return "decomp: obs_ofs_* must start at 0 and be non-decreasing";
-    if (!fq_scan_all_finite(w.path, 3 * (size_t)(c->n_poly + P)) || !fq_scan_all_finite(w.obs, 3 * (size_t)*n_obs))
+    if (w.obs_ofs && !scan_offsets(w.obs_ofs, P, 1 << 30, n_obs, &w.max_obs))   // (against maps there are no clouds here)
+      return "decomp: obs_ofs_* must start at 0 and be non-decreasing";
+    if (!fq_scan_all_finite(w.path, 3 * (size_t)(c->n_poly + P)) || (w.obs && !fq_scan_all_finite(w.obs, 3 * (size_t)*n_obs)))
       return "decomp: non-finite value in a path, a cloud or the goal";
   }
   if (!fq_scan_all_positive_finite(w.factors, (size_t)w.n_fac)) return "limits and factors must be finite and > 0";
@@ -667,19 +720,25 @@ const char* scan_sweep(Sweep& w, int P, const fq_pair_assign* as, const fq_pair_
 
 int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results,
                             const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex, const fq_pair_decomp* dc,
-                            const fq_pair_hr* hr)
+                            const fq_pair_hr* hr, const fq_pair_map* mp)
 {
   if (!ctx) return FQ_E_ARG;
   if (int rc = fq_settle(ctx)) return rc;
   Sweep sw[2];
-  if (int rc = check_chain(ctx, a, as, win, ex, dc, sw)) return rc;
+  if (int rc = check_chain(ctx, a, as, win, ex, dc, sw, mp)) return rc;
   const int P = a->n_prob;
   if (!fq_scan_all_finite(a->x0, 9 * (size_t)P)) return fq_fail(ctx, FQ_E_ARG, "non-finite value in x0/xf");
   if (!fq_scan_all_positive_finite(a->lim, 3 * (size_t)P)) return fq_fail(ctx, FQ_E_ARG, "limits and factors must be finite and > 0");
   if (dc && dc->goal && !fq_scan_all_finite(dc->goal, 3 * (size_t)P))
     return fq_fail(ctx, FQ_E_ARG, "decomp: non-finite value in a path, a cloud or the goal");
   int n_unk = 0, largest_unk = 0;
-  if (hr)
+  if (mp)
+  {
+    if (int rc = check_map(ctx, dc, hr, win, mp)) return rc;
+    for (int j = 0; mp->map_index && j < P; j++)
+      if (mp->map_index[j] < 0 || mp->map_index[j] >= mp->n_maps) return fq_fail(ctx, FQ_E_ARG, "map: map_index out of range");
+  }
+  else if (hr)
   {
     if (int rc = check_hr(ctx, win, dc, hr)) return rc;
     if (!scan_offsets(hr->unk_ofs, P, 1 << 30, &n_unk, &largest_unk)) return fq_fail(ctx, FQ_E_ARG, "hr: unk_ofs must start at 0 and be non-decreasing");
@@ -698,6 +757,7 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   fq_pair_exact dx{};
   fq_pair_decomp dd = dc ? *dc : fq_pair_decomp{};
   fq_pair_hr dh = hr ? *hr : fq_pair_hr{};
+  fq_pair_map dm = mp ? *mp : fq_pair_map{};
   if (as) da.all_limit = as->all_limit;
   Sweep dv[2];
   char *hi = nullptr, *din = nullptr, *dout = nullptr;
@@ -733,6 +793,7 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
     d.lim = in(a->lim, 3 * (size_t)P);
     d.results = out(a->results, P);
     if (dc) dd.goal = in(dc->goal, 3 * (size_t)P);
+    if (mp) dm.map_index = in(mp->map_index, P);
     if (hr)
     { // last_factor_safe is updated in its uploaded copy, which goes back to the caller's array
       dh.unk_ofs = in(hr->unk_ofs, P + 1);  dh.unk = in(hr->unk, 3 * (size_t)n_unk);
@@ -762,7 +823,8 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   cudaStream_t st = ctx->stream;
   FQ_CUDA(cudaMemcpyAsync(din, hi, in_bytes, cudaMemcpyHostToDevice, st));
   for (int i = 0; i < 2; i++) put_sweep(dv[i], i, &d, &da, &dw, &dx, &dd);
-  int rc = hr ? fq_replan_pairs_hr_dev(ctx, &d, &da, win ? &dw : nullptr, ex ? &dx : nullptr, &dd, &dh, nullptr, st)
+  int rc = mp ? fq_replan_pairs_map_dev(ctx, &d, &da, win ? &dw : nullptr, ex ? &dx : nullptr, &dd, hr ? &dh : nullptr, &dm, nullptr, st)
+         : hr ? fq_replan_pairs_hr_dev(ctx, &d, &da, win ? &dw : nullptr, ex ? &dx : nullptr, &dd, &dh, nullptr, st)
          : dc ? fq_replan_pairs_decomp_dev(ctx, &d, &da, win ? &dw : nullptr, ex ? &dx : nullptr, &dd, nullptr, st)
          : ex ? fq_replan_pairs_exact_dev(ctx, &d, &da, win ? &dw : nullptr, &dx, nullptr, st)
          : win ? fq_replan_pairs_window_dev(ctx, &d, &da, &dw, nullptr, st)
@@ -806,13 +868,14 @@ namespace
 // chains run on one GPU only, since gathering their per-corridor exact / nodes / corridor arrays would need a second
 // exchange besides the records'.
 int lists_host(fq_ctx* ctx, const fq_pair_args* a, bool deferred, const fq_pair_assign* as, const fq_pair_window* win,
-               const fq_pair_exact* ex = nullptr, const fq_pair_decomp* dc = nullptr, const fq_pair_hr* hr = nullptr)
+               const fq_pair_exact* ex = nullptr, const fq_pair_decomp* dc = nullptr, const fq_pair_hr* hr = nullptr,
+               const fq_pair_map* mp = nullptr)
 {
   if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
   if ((ex || dc) && (ctx->is_group || ctx->comm))
-    return fq_fail(ctx, FQ_E_ARG, "fq_replan_pairs_exact / _decomp / _hr: multi-GPU contexts are not supported (use the _dev entry)");
+    return fq_fail(ctx, FQ_E_ARG, "fq_replan_pairs_exact / _decomp / _hr / _map: multi-GPU contexts are not supported (use the _dev entry)");
   if (ctx->is_group || ctx->comm) return fq_replan_pairs_sharded(ctx, a, deferred, as, win);
-  return fq_replan_pairs_host_ex(ctx, a, deferred, nullptr, true, as, win, ex, dc, hr);
+  return fq_replan_pairs_host_ex(ctx, a, deferred, nullptr, true, as, win, ex, dc, hr, mp);
 }
 }  // namespace
 
@@ -875,4 +938,19 @@ extern "C" int fq_replan_pairs_hr_async(fq_ctx* ctx, const fq_pair_args* a, cons
   if (!ctx) return FQ_E_ARG;
   if (int rc = check_hr(ctx, win, dc, hr)) return rc;
   return lists_host(ctx, a, true, as, win, ex, dc, hr);
+}
+
+extern "C" int fq_replan_pairs_map(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
+                                   const fq_pair_exact* ex, const fq_pair_decomp* dc, const fq_pair_hr* hr, const fq_pair_map* mp)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (!mp) return fq_fail(ctx, FQ_E_ARG, "map is NULL");
+  return lists_host(ctx, a, false, as, win, ex, dc, hr, mp);
+}
+extern "C" int fq_replan_pairs_map_async(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
+                                         const fq_pair_exact* ex, const fq_pair_decomp* dc, const fq_pair_hr* hr, const fq_pair_map* mp)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (!mp) return fq_fail(ctx, FQ_E_ARG, "map is NULL");
+  return lists_host(ctx, a, true, as, win, ex, dc, hr, mp);
 }

@@ -47,7 +47,8 @@ typedef struct fq_ctx fq_ctx;     /* opaque: device, stream, plan tables, scratc
 
 int fq_abi_version(void);
 /* 1 if this build has the named feature: "sweep_early_exit", "replan_pairs", "multi_gpu", "row_tol", "certificates",
- * "replan_pairs_assign", "replan_pairs_window", "replan_pairs_exact", "replan_pairs_decomp", "replan_pairs_hr". */
+ * "replan_pairs_assign", "replan_pairs_window", "replan_pairs_exact", "replan_pairs_decomp", "replan_pairs_hr",
+ * "replan_pairs_map". */
 int fq_has_feature(const char* name);
 
 /* Threading: a context is used from one thread at a time, like a SolverGurobi instance in the reference (one replan
@@ -501,6 +502,82 @@ int fq_replan_pairs_hr_async(fq_ctx* ctx, const fq_pair_args* args, const fq_pai
 int fq_replan_pairs_hr_dev(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
                            const fq_pair_exact* exact, const fq_pair_decomp* decomp, const fq_pair_hr* hr, fq_pair_result* results_all,
                            void* stream);
+
+/* ---- an indexed map on the device, shared by every corridor and every later replan ---------------------------------
+ *
+ * Faster::updateMap (faster.cpp:99-137) keeps, per mapper message, the occupied cloud O (vec_o_), the unknown cloud U and
+ * U ++ O (vec_uo_: U with O appended, in that order), which every replan then queries.  An fq_map holds the same three
+ * clouds on one GPU, uploaded and indexed once: each of U and O is bucketed into a uniform grid of cells of edge
+ * FQ_MAP_CELL_EDGE (doubled until the grid has at most min(max(65536, 4 (|U| + |O|)), 2^26) cells), its points sorted by (cell, index)
+ * with a stable device radix sort.  The cell edge changes no answer, only how many points a query reads.  Feature
+ * "replan_pairs_map".
+ *
+ * An empty U is allowed: H/R then finds no unknown point and the safe cloud is O.  (The reference keeps its previous
+ * vec_uo_ when the unknown cloud is empty, faster.cpp:121-125; that is not modelled.)  A map must not be updated or
+ * destroyed while a submission that reads it is in flight.
+ *
+ * A submission reads a map through a descriptor that stays at one device address for the map's life and that every
+ * update rewrites in full on the update's stream: its grid, its counts and the addresses of its arrays.  So a
+ * fq_replan_pairs_map_dev call captured once in a CUDA graph and replayed after later updates -- with or without a grown
+ * capacity -- reads each map's last update, as a fresh call would.
+ *
+ * An update that fails (FQ_E_CUDA: an allocation or a launch) leaves the map empty, with a descriptor that reads no
+ * points, and fq_replan_pairs_map* refuse the map until an update succeeds. */
+#define FQ_MAP_CELL_EDGE 0.5
+typedef struct fq_map fq_map;
+/* Errors of fq_map_* are read with fq_last_error(NULL). */
+int fq_map_create(fq_map** out, int device);
+void fq_map_destroy(fq_map* map);
+/* HOST pointers (n x 3 doubles each; NULL with a count of 0); blocks until the map holds the new clouds.  FQ_E_ARG for a
+ * negative count, more than 2^30 points in all, a NULL cloud with a positive count or a non-finite coordinate. */
+int fq_map_update(fq_map* map, const double* occ, int n_occ, const double* unk, int n_unk);
+/* DEVICE pointers, stream-ordered on `stream` (NULL: the legacy default stream): copies the clouds and builds the index
+ * without synchronising, as long as the map's capacity holds n_occ + n_unk points.  A larger update first grows the
+ * capacity (cudaFree / cudaMalloc, which wait for the whole device); the capacity never shrinks.  The counts are checked
+ * as by fq_map_update; the coordinates cannot be checked without synchronising: a non-finite point is left out of the
+ * index, so no query ever sees it.  The input arrays may be reused once the stream has passed this call. */
+int fq_map_update_dev(fq_map* map, const double* d_occ, int n_occ, const double* d_unk, int n_unk, void* stream);
+/* the counts of the last update (either may be NULL) */
+int fq_map_size(const fq_map* map, int* n_occ, int* n_unk);
+
+/* ---- chained replan against indexed maps ------------------------------------------------------------------------
+ *
+ * fq_replan_pairs_hr* (or, with hr == NULL, fq_replan_pairs_decomp*, the r_fraction rule) with each corridor's clouds taken
+ * from a map: for corridor j, whose map holds O and U, the outputs are byte for byte those of fq_replan_pairs_hr called with
+ * obs_whole_j = O, obs_safe_j = U ++ O and unk_j = U -- records, per-candidate flags and costs, coefficients, corridors,
+ * E / M, statuses, index_H / need_safe, windows and exact / nodes -- as long as no segment has more than max_local points
+ * in its local box (below).  This holds at any coordinate magnitude: the cells H/R reads are widened by a bound on the
+ * float rounding of points, samples and distances.  decomp->obs_* and hr->unk* must be NULL, and decomp->max_obs_* are
+ * not used.  The decomposition reads only the cells the segment's local box overlaps, H/R only the cells near each
+ * sample.
+ *
+ * max_local caps the points of one segment's cloud that pass the local-box test; a segment above it gets FQ_DECOMP_CLOUD,
+ * and the rest of the batch is unaffected.  It sizes the decomposition's scratch, n_prob x max_poly x (max_local - 1024) x
+ * 37 bytes, whatever the maps' sizes. */
+typedef struct fq_pair_map
+{
+  const fq_map* const* maps;  /* n_maps maps, all on the context's device                                          */
+  int n_maps;
+  const int* map_index;       /* n_prob: corridor j uses maps[map_index[j]], or NULL: every corridor uses maps[0]  */
+  int max_local;              /* >= 0                                                                              */
+} fq_pair_map;
+
+/* HOST pointers everywhere (map_index included); blocks until every output is in the caller's arrays.  FQ_E_ARG: the
+ * refusals of fq_replan_pairs_hr (fq_replan_pairs_decomp when hr == NULL) other than those of the clouds, obs_* / unk*
+ * not NULL, map NULL, no maps or a NULL map, a map on another device, a map whose last update failed, a map_index
+ * entry outside 0 .. n_maps-1, max_local < 0 or above 2^30, and multi-GPU contexts. */
+int fq_replan_pairs_map(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
+                        const fq_pair_exact* exact, const fq_pair_decomp* decomp, const fq_pair_hr* hr, const fq_pair_map* map);
+/* The same, returning once everything is enqueued; outputs are valid after fq_wait(ctx).  Arrays must stay alive. */
+int fq_replan_pairs_map_async(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
+                              const fq_pair_exact* exact, const fq_pair_decomp* decomp, const fq_pair_hr* hr, const fq_pair_map* map);
+/* DEVICE pointers everywhere (the structs and the maps array live on the host; map_index is a device array), as
+ * fq_replan_pairs_hr_dev; never synchronises.  map_index is not read on the host: a corridor whose entry is out of range
+ * gets FQ_DECOMP_CLOUD for both sweeps.  On a rank context the records are all-gathered into results_all as
+ * fq_replan_pairs_dev does. */
+int fq_replan_pairs_map_dev(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
+                            const fq_pair_exact* exact, const fq_pair_decomp* decomp, const fq_pair_hr* hr, const fq_pair_map* map,
+                            fq_pair_result* results_all, void* stream);
 
 /* ---- several GPUs behind the boundary (SURVEY.md 8b/8e) ---------------------------------------------------------
  *
