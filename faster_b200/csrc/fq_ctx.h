@@ -114,30 +114,34 @@ int fq_solve_multi_host_ex(fq_ctx* ctx, int N, int force_final, int n_prob, cons
                            const int* poly_ofs, const int* face_ofs, const double* Ab, const int* cand_ofs, const double* dt,
                            const uint8_t* sigma, uint8_t* feasible, double* cost, double* coeffs, int32_t* iters, bool deferred,
                            int** d_win_idx, double** d_win_cost);
-// Candidate offsets of one sweep with per-corridor assignment lists (fq_pair_capi.cu): corridor j (P_j polytopes) has
-// |L(N, P_j, all_limit)| candidates per factor and n_fac factors, or the |F_j| of its window (init[j], final_[j], inc) when
-// init is not NULL.  Fills ofs[0 .. n_prob], *max_fac (largest |F_j|, 0 without windows) and *max_poly (largest P_j), and
-// returns why the sweep is refused, or nullptr.
-const char* fq_list_offsets(int n_prob, const int* poly_ofs, int N, long all_limit, int n_fac, const double* init,
-                            const double* final_, double inc, std::vector<long long>* ofs, int* max_fac, int* max_poly);
-// fq_pair_capi.cu.  d_results (may be NULL): receives the device address of the result records; copy_results = false
-// leaves the caller's `results` array untouched (the multi-GPU path reads the all-gathered table instead).  as != NULL:
-// per-corridor assignment lists (fq_replan_pairs_assign*, host pointers); win != NULL (with as): per-corridor windows
-// (fq_replan_pairs_window*, host pointers); ex != NULL (with as): the exact stage (fq_replan_pairs_exact*, host pointers)
-int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results,
-                            const fq_pair_assign* as = nullptr, const fq_pair_window* win = nullptr,
-                            const fq_pair_exact* ex = nullptr, const fq_pair_decomp* dc = nullptr, const fq_pair_hr* hr = nullptr,
-                            const fq_pair_map* mp = nullptr);
 // fq_map.cu: the device address of a map's descriptor (fixed for the map's life, rewritten by every update), its device,
 // and whether its last update succeeded
 const FqMapDev* fq_map_descriptor(const fq_map* m);
 int fq_map_device(const fq_map* m);
 bool fq_map_valid(const fq_map* m);
-// fq_multi.cu
+// ---- multi-GPU contexts (fq_multi.cu; the chained replan's sharding is in fq_pair_capi.cu).  A sharded host entry
+// checks the whole description and then every shard of the world on the host before it writes or enqueues anything, so
+// every rank of a communicator makes the same decision and none is left waiting in the all-gather.
 void fq_comm_release(fq_ctx* ctx);
 // all-gather on one context's communicator (one process per GPU): `bytes` from every rank, rank order
 int fq_comm_allgather(fq_ctx* ctx, const void* d_send, void* d_recv, size_t bytes, cudaStream_t stream);
-// fq_replan_pairs on a multi-GPU context (a group or a rank of a communicator)
-// (as != NULL: fq_replan_pairs_assign*, shards balanced by candidate count; win != NULL as well: fq_replan_pairs_window*)
-int fq_replan_pairs_sharded(fq_ctx* g, const fq_pair_args* a, bool deferred, const fq_pair_assign* as = nullptr,
-                            const fq_pair_window* win = nullptr);
+// member i of a single-process group (member 0 is the group's own context)
+inline fq_ctx* fq_member(fq_ctx* g, int i) { return i == 0 ? g : g->peers[i - 1]; }
+// the one exchange of a sharded call: local member i (one for a rank context) sends `bytes` from send[i] and receives
+// every rank's, in rank order, into recv[i].  Over the members of a single-process group, over a rank's communicator, or
+// a copy for a world of one.
+int fq_exchange(fq_ctx* g, const std::vector<void*>& send, const std::vector<void*>& recv, size_t bytes);
+struct FqSubCorridors
+{ // rebased CSR description of problems [lo, hi)
+  std::vector<int> poly_ofs, face_ofs;
+  const double* Ab;
+  void build(const int* po, const int* fo, const double* Ab_all, int lo, int hi)
+  {
+    poly_ofs.resize(hi - lo + 1);
+    for (int j = lo; j <= hi; j++) poly_ofs[j - lo] = po[j] - po[lo];
+    const int p0 = po[lo], p1 = po[hi];
+    face_ofs.resize(p1 - p0 + 1);
+    for (int p = p0; p <= p1; p++) face_ofs[p - p0] = fo[p] - fo[p0];
+    Ab = Ab_all ? Ab_all + 4 * (size_t)fo[p0] : nullptr;
+  }
+};

@@ -5,7 +5,8 @@
 //   * one process per GPU (torchrun-style): fq_create + fq_comm_init(id, rank, world) on every rank;
 //   * one process, several GPUs (what the reference's single planner process would do): fq_create_multi.
 // NCCL is loaded lazily with dlopen (libnccl.so.2; FQ_NCCL_LIB overrides), so the library has no link-time dependency
-// on it and single-GPU use needs no NCCL at all.
+// on it and single-GPU use needs no NCCL at all.  The chained replan's sharding lives beside its host entry and its sweep
+// descriptions (fq_pair_capi.cu); this file holds the communicators, the exchange and fq_solve_multi_sharded.
 #include "fq_ctx.h"
 
 #include <algorithm>
@@ -211,33 +212,9 @@ extern "C" int fq_shard_range(int n_prob, const int* cand_ofs, int rank, int wor
   return 0;
 }
 
-namespace
-{
-fq_ctx* member(fq_ctx* g, int i) { return i == 0 ? g : g->peers[i - 1]; }
-
-struct SubCorridors
-{ // rebased CSR description of problems [lo, hi)
-  std::vector<int> poly_ofs, face_ofs;
-  const double* Ab;
-  void build(const int* po, const int* fo, const double* Ab_all, int lo, int hi)
-  {
-    poly_ofs.resize(hi - lo + 1);
-    for (int j = lo; j <= hi; j++) poly_ofs[j - lo] = po[j] - po[lo];
-    const int p0 = po[lo], p1 = po[hi];
-    face_ofs.resize(p1 - p0 + 1);
-    for (int p = p0; p <= p1; p++) face_ofs[p - p0] = fo[p] - fo[p0];
-    Ab = Ab_all ? Ab_all + 4 * (size_t)fo[p0] : nullptr;
-  }
-};
-
-// the one exchange of a sharded call: local member i (one for a rank context) sends `count` records from send[i] and
-// receives every rank's, in rank order, into recv[i].  Over the members of a single-process group, over a rank's
-// communicator, or a copy for a world of one.
-template <class T>
-int exchange(fq_ctx* g, const std::vector<T*>& send, const std::vector<T*>& recv, size_t count)
+int fq_exchange(fq_ctx* g, const std::vector<void*>& send, const std::vector<void*>& recv, size_t bytes)
 {
   fq_ctx* ctx = g;
-  const size_t bytes = sizeof(T) * count;
   if (!g->is_group && g->comm) return fq_comm_allgather(g, send[0], recv[0], bytes, g->stream);
   // a context that is neither a group nor a communicator's rank keeps world == 1 (only fq_comm_init and fq_create_multi
   // set it), so past this point world > 1 means a group with world - 1 peers
@@ -250,147 +227,12 @@ int exchange(fq_ctx* g, const std::vector<T*>& send, const std::vector<T*>& recv
   FQ_NCCL(g_nccl.GroupStart());
   for (int i = 0; i < g->world; i++)
   {
-    fq_ctx* c = member(g, i);
+    fq_ctx* c = fq_member(g, i);
     cudaSetDevice(c->device);
     ncclResult_t r = g_nccl.AllGather(send[i], recv[i], bytes, ncclChar, c->comm->comm, c->stream);
     if (r != ncclSuccess) { g_nccl.GroupEnd(); return nccl_fail(g, r, "ncclAllGather"); }
   }
   FQ_NCCL(g_nccl.GroupEnd());
-  return 0;
-}
-}  // namespace
-
-// fq_replan_pairs on a multi-GPU context.  Group (one process): corridors [lo_i, hi_i) go to member i, every member runs
-// its chain, the result records are all-gathered (padded to the largest shard) and read back once from member 0; the
-// per-candidate arrays travel straight from each member into the caller's arrays.  Rank context (one process per GPU):
-// every rank passes the SAME full description and solves its own shard; after the all-gather every rank holds every
-// corridor's result record, while per-candidate outputs are filled for the rank's own corridors only.
-// Per-corridor assignment lists (as != NULL): the corridors' candidate counts differ, so the shards are balanced by
-// candidates -- fq_shard_range over the offsets of whole + safe candidates, computed here from poly_ofs -- and each shard's
-// per-candidate outputs start at the shard's first offset.  The caller's cand_ofs_* come from the same host offsets.
-// Per-corridor windows (win != NULL, with as): corridor j has |F_j| factors (fq_window.h) instead of n_fac_*, and every
-// shard gets its rows of the window arrays.
-int fq_replan_pairs_sharded(fq_ctx* g, const fq_pair_args* a, bool deferred, const fq_pair_assign* as, const fq_pair_window* win)
-{
-  fq_ctx* ctx = g;
-  if (!a || a->n_prob <= 0 || !a->results) return fq_fail(g, FQ_E_ARG, "bad arguments");
-  // the members' own check of N (fq_pair_capi.cu), here before the list lengths below use N and the offsets are written
-  if (a->N_whole < 3 || a->N_whole > FQ_MAX_N || a->N_safe < 2 || a->N_safe > FQ_MAX_N) return fq_fail(g, FQ_E_ARG, "N out of range");
-  // the shards' corridor descriptions are rebased on the host before the per-member validation runs: the arrays read
-  // here must exist (everything else is checked by the member's own call)
-  if (!a->x0 || !a->xf_whole || !a->xf_safe || !a->lim || !a->poly_ofs_whole || !a->face_ofs_whole || !a->poly_ofs_safe ||
-      !a->face_ofs_safe)
-    return fq_fail(g, FQ_E_ARG, "NULL argument");
-  if (win && (!win->init_whole || !win->final_whole || !win->init_safe || !win->final_safe))
-    return fq_fail(g, FQ_E_ARG, "window arrays must not be NULL");
-  if (!win && (a->n_fac_whole <= 0 || a->n_fac_safe <= 0 || (!as && (a->n_sig_whole <= 0 || a->n_sig_safe <= 0))))
-    return fq_fail(g, FQ_E_ARG, "empty factor / assignment grid");
-  if (as && (a->sigmas_whole || a->sigmas_safe || a->n_sig_whole != 0 || a->n_sig_safe != 0))
-    return fq_fail(g, FQ_E_ARG, "per-corridor assignment lists: sigmas_* must be NULL and n_sig_* 0");
-  for (int j = 0; j < a->n_prob; j++)
-    if (a->poly_ofs_whole[j + 1] < a->poly_ofs_whole[j] || a->poly_ofs_safe[j + 1] < a->poly_ofs_safe[j])
-      return fq_fail(g, FQ_E_ARG, "poly_ofs not monotone");
-  const int P = a->n_prob, world = g->world;
-  const bool group = g->is_group;
-  const int n_local = group ? world : 1;
-  const size_t ncw1 = (size_t)a->n_fac_whole * a->n_sig_whole, ncs1 = (size_t)a->n_fac_safe * a->n_sig_safe;
-  // per-corridor lists: candidate offsets of the two sweeps and of both together (the shards' weights)
-  std::vector<long long> ofw, ofs;
-  std::vector<int> ofb;
-  if (as)
-  {
-    int mf = 0, mp = 0;
-    const char* why = fq_list_offsets(P, a->poly_ofs_whole, a->N_whole, as->all_limit, a->n_fac_whole, win ? win->init_whole : nullptr,
-                                      win ? win->final_whole : nullptr, win ? win->inc_whole : 0, &ofw, &mf, &mp);
-    if (!why)
-      why = fq_list_offsets(P, a->poly_ofs_safe, a->N_safe, as->all_limit, a->n_fac_safe, win ? win->init_safe : nullptr,
-                            win ? win->final_safe : nullptr, win ? win->inc_safe : 0, &ofs, &mf, &mp);
-    if (why) return fq_fail(g, FQ_E_ARG, why);
-    ofb.assign(P + 1, 0);
-    for (int j = 1; j <= P; j++) ofb[j] = (int)std::min<long long>(ofw[j] + ofs[j], 0x7fffffffLL);
-  }
-  int pad = 0;
-  std::vector<int> lo(world), hi(world);
-  for (int r = 0; r < world; r++)
-  {
-    fq_shard_range(P, as ? ofb.data() : nullptr, r, world, &lo[r], &hi[r]);
-    pad = std::max(pad, hi[r] - lo[r]);
-  }
-  if (as)
-    for (int j = 0; j <= P; j++)
-    {
-      if (as->cand_ofs_whole) as->cand_ofs_whole[j] = (int)ofw[j];
-      if (as->cand_ofs_safe) as->cand_ofs_safe[j] = (int)ofs[j];
-    }
-  std::vector<fq_pair_result*> d_res(n_local, nullptr), d_all(n_local, nullptr);
-  for (int i = 0; i < n_local; i++)
-  {
-    fq_ctx* c = group ? member(g, i) : g;
-    const int r = group ? i : g->rank;
-    if (int rc = fq_settle(c)) return rc;
-    cudaSetDevice(c->device);
-    // gather buffers: [pad records to send | world x pad records received]
-    cudaError_t e = c->d_out.reserve(sizeof(fq_pair_result) * (size_t)pad * (world + 1));
-    if (e != cudaSuccess) return fq_cuda_fail(g, e, "gather buffer");
-    d_res[i] = (fq_pair_result*)c->d_out.p;
-    d_all[i] = d_res[i] + pad;
-    e = cudaMemsetAsync(d_res[i], 0xff, sizeof(fq_pair_result) * (size_t)pad, c->stream);
-    if (e != cudaSuccess) return fq_cuda_fail(g, e, "gather buffer");
-    const int n = hi[r] - lo[r];
-    if (n <= 0) continue;
-    fq_pair_args s = *a;
-    SubCorridors cw, cs;
-    cw.build(a->poly_ofs_whole, a->face_ofs_whole, a->Ab_whole, lo[r], hi[r]);
-    cs.build(a->poly_ofs_safe, a->face_ofs_safe, a->Ab_safe, lo[r], hi[r]);
-    s.n_prob = n;
-    s.x0 = a->x0 + 9 * (size_t)lo[r]; s.xf_whole = a->xf_whole + 9 * (size_t)lo[r]; s.xf_safe = a->xf_safe + 9 * (size_t)lo[r];
-    s.lim = a->lim + 3 * (size_t)lo[r];
-    s.poly_ofs_whole = cw.poly_ofs.data(); s.face_ofs_whole = cw.face_ofs.data(); s.Ab_whole = cw.Ab;
-    s.poly_ofs_safe = cs.poly_ofs.data(); s.face_ofs_safe = cs.face_ofs.data(); s.Ab_safe = cs.Ab;
-    // first candidate of the shard in the caller's per-candidate arrays
-    const size_t cw0 = as ? (size_t)ofw[lo[r]] : ncw1 * lo[r], cs0 = as ? (size_t)ofs[lo[r]] : ncs1 * lo[r];
-    if (a->feasible_whole) { s.feasible_whole = a->feasible_whole + cw0; s.cost_whole = a->cost_whole + cw0; }
-    if (a->feasible_safe) { s.feasible_safe = a->feasible_safe + cs0; s.cost_safe = a->cost_safe + cs0; }
-    if (a->coeffs_whole) s.coeffs_whole = a->coeffs_whole + 12 * (size_t)a->N_whole * lo[r];
-    if (a->coeffs_safe) s.coeffs_safe = a->coeffs_safe + 12 * (size_t)a->N_safe * lo[r];
-    s.results = a->results + lo[r];            // not copied back (copy_results = false): the gathered table is
-    fq_pair_assign sa{};
-    if (as)
-    { // the offsets were written above; the winners' assignments go straight into the caller's rows of the shard
-      sa.all_limit = as->all_limit;
-      sa.sigma_whole = as->sigma_whole ? as->sigma_whole + (size_t)a->N_whole * lo[r] : nullptr;
-      sa.sigma_safe = as->sigma_safe ? as->sigma_safe + (size_t)a->N_safe * lo[r] : nullptr;
-    }
-    fq_pair_window sw{};
-    if (win)
-    { // the shard's rows of every window array
-      const size_t o = (size_t)lo[r];
-      auto in = [o](const double* p) { return p + o; };
-      auto out = [o](auto* p) { return p ? p + o : p; };
-      sw = *win;
-      sw.init_whole = in(win->init_whole); sw.final_whole = in(win->final_whole); sw.init_safe = in(win->init_safe); sw.final_safe = in(win->final_safe);
-      sw.factor_whole = out(win->factor_whole); sw.factor_safe = out(win->factor_safe);
-      sw.trials_whole = out(win->trials_whole); sw.trials_safe = out(win->trials_safe);
-      sw.next_init_whole = out(win->next_init_whole); sw.next_final_whole = out(win->next_final_whole);
-      sw.next_init_safe = out(win->next_init_safe); sw.next_final_safe = out(win->next_final_safe);
-    }
-    fq_pair_result* dr = nullptr;
-    int rc = fq_replan_pairs_host_ex(c, &s, true, &dr, false, as ? &sa : nullptr, win ? &sw : nullptr);
-    if (rc) { if (c != g) g->err = c->err; return rc; }
-    e = cudaMemcpyAsync(d_res[i], dr, sizeof(fq_pair_result) * (size_t)n, cudaMemcpyDeviceToDevice, c->stream);
-    if (e != cudaSuccess) return fq_cuda_fail(g, e, "gather staging");
-  }
-  if (int rc = exchange(g, d_res, d_all, (size_t)pad)) return rc;
-  // ---- the gathered table, shard by shard, into the caller's results (from member 0 / this rank)
-  FQ_CUDA(cudaSetDevice(g->device));
-  for (int r = 0; r < world; r++)
-    if (hi[r] > lo[r])
-      FQ_CUDA(cudaMemcpyAsync(a->results + lo[r], d_all[0] + (size_t)r * pad, sizeof(fq_pair_result) * (size_t)(hi[r] - lo[r]),
-                              cudaMemcpyDeviceToHost, g->stream));
-  g->pending = true;
-  if (deferred) return 0;
-  for (int i = 0; i < n_local; i++)
-    if (int rc = fq_settle(group ? member(g, i) : g)) return rc;
   return 0;
 }
 
@@ -414,23 +256,24 @@ extern "C" int fq_solve_multi_sharded(fq_ctx* g, int N, int force_final, int n_p
   int pad = 0;
   std::vector<int> lo(world), hi(world);
   for (int r = 0; r < world; r++) { fq_shard_range(n_prob, cand_ofs, r, world, &lo[r], &hi[r]); pad = std::max(pad, hi[r] - lo[r]); }
-  std::vector<Rec*> d_res(n_local, nullptr), d_all(n_local, nullptr);
+  std::vector<void*> d_res(n_local, nullptr), d_all(n_local, nullptr);
   std::vector<FqArena*> arenas(n_local, nullptr);
   for (int i = 0; i < n_local; i++)
   {
-    fq_ctx* c = group ? member(g, i) : g;
+    fq_ctx* c = group ? fq_member(g, i) : g;
     const int r = group ? i : g->rank;
     if (int rc = fq_settle(c)) return rc;
     cudaSetDevice(c->device);
     cudaError_t e = c->d_bnb.reserve(sizeof(Rec) * (size_t)pad * (world + 1));      // d_in / d_out belong to the solve
     if (e != cudaSuccess) return fq_cuda_fail(g, e, "gather buffer");
-    d_res[i] = (Rec*)c->d_bnb.p;
-    d_all[i] = d_res[i] + pad;
-    e = cudaMemsetAsync(d_res[i], 0xff, sizeof(Rec) * (size_t)pad, c->stream);
+    Rec* res = (Rec*)c->d_bnb.p;
+    d_res[i] = res;
+    d_all[i] = res + pad;
+    e = cudaMemsetAsync(res, 0xff, sizeof(Rec) * (size_t)pad, c->stream);
     if (e != cudaSuccess) return fq_cuda_fail(g, e, "gather buffer");
     const int n = hi[r] - lo[r];
     if (n <= 0) continue;
-    SubCorridors sc;
+    FqSubCorridors sc;
     sc.build(poly_ofs, face_ofs, Ab, lo[r], hi[r]);
     std::vector<int> co(n + 1);
     for (int j = 0; j <= n; j++) co[j] = cand_ofs[lo[r] + j] - cand_ofs[lo[r]];
@@ -442,18 +285,18 @@ extern "C" int fq_solve_multi_sharded(fq_ctx* g, int N, int force_final, int n_p
                                     feasible + c0, cost + c0, nullptr, nullptr, true, &dwi, &dwc);
     if (rc) { if (c != g) g->err = c->err; return rc; }
     // pack (cost, idx) records: two strided copies on the device
-    e = cudaMemcpy2DAsync(&d_res[i][0].cost, sizeof(Rec), dwc, sizeof(double), sizeof(double), n, cudaMemcpyDeviceToDevice, c->stream);
+    e = cudaMemcpy2DAsync(&res[0].cost, sizeof(Rec), dwc, sizeof(double), sizeof(double), n, cudaMemcpyDeviceToDevice, c->stream);
     if (e == cudaSuccess)
-      e = cudaMemcpy2DAsync(&d_res[i][0].idx, sizeof(Rec), dwi, sizeof(int), sizeof(int), n, cudaMemcpyDeviceToDevice, c->stream);
+      e = cudaMemcpy2DAsync(&res[0].idx, sizeof(Rec), dwi, sizeof(int), sizeof(int), n, cudaMemcpyDeviceToDevice, c->stream);
     if (e != cudaSuccess) return fq_cuda_fail(g, e, "winner records");
   }
-  if (int rc = exchange(g, d_res, d_all, (size_t)pad)) return rc;
+  if (int rc = fq_exchange(g, d_res, d_all, sizeof(Rec) * (size_t)pad)) return rc;
   FQ_CUDA(cudaSetDevice(g->device));
   std::vector<Rec> all((size_t)pad * world);
   FQ_CUDA(cudaMemcpyAsync(all.data(), d_all[0], sizeof(Rec) * all.size(), cudaMemcpyDeviceToHost, g->stream));
   g->pending = true;
   for (int i = 0; i < n_local; i++)
-    if (int rc = fq_settle(group ? member(g, i) : g)) return rc;
+    if (int rc = fq_settle(group ? fq_member(g, i) : g)) return rc;
   for (int r = 0; r < world; r++)
     for (int j = lo[r]; j < hi[r]; j++)
     {

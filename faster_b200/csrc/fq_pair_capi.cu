@@ -632,6 +632,12 @@ extern "C" int fq_replan_pairs_map_dev(fq_ctx* ctx, const fq_pair_args* a, const
   return chain_dev(ctx, a, as, win, ex, dc, results_all, stream_v, hr, mp);
 }
 
+namespace
+{
+// Candidate offsets of one sweep with per-corridor assignment lists, the only code that counts them: corridor j (P_j
+// polytopes) has |L(N, P_j, all_limit)| candidates per factor and n_fac factors, or the |F_j| of its window (init[j],
+// final_[j], inc) when init is not NULL.  Fills ofs[0 .. n_prob], *max_fac (largest |F_j|, 0 without windows) and
+// *max_poly (largest P_j), and returns why the sweep is refused, or nullptr.
 const char* fq_list_offsets(int n_prob, const int* poly_ofs, int N, long all_limit, int n_fac, const double* init,
                             const double* final_, double inc, std::vector<long long>* ofs, int* max_fac, int* max_poly)
 {
@@ -654,8 +660,6 @@ const char* fq_list_offsets(int n_prob, const int* poly_ofs, int N, long all_lim
   return nullptr;
 }
 
-namespace
-{
 bool scan_offsets(const int* o, int n, int max_step, int* total, int* largest)
 { // o[0] = 0 and steps of 0 .. max_step
   if (o[0] != 0) return false;
@@ -671,8 +675,10 @@ bool scan_offsets(const int* o, int n, int max_step, int* total, int* largest)
 
 // The host-side checks of one sweep's arrays (host pointers), which also set the sizes the _dev entries take as hints:
 // max_faces / max_poly_faces (a decomposing chain keeps the caller's caps), max_obs, and with per-corridor lists n_cand,
-// max_fac and max_poly.  *c receives the corridors' sizes (a decomposing chain: n_poly only), *n_obs the clouds' points.
-const char* scan_sweep(Sweep& w, int P, const fq_pair_assign* as, const fq_pair_decomp* dc, FqCorridorSizes* c, int* n_obs)
+// max_fac and max_poly.  *c receives the corridors' sizes (a decomposing chain: n_poly only), *n_obs the clouds' points,
+// *ofs the candidate offsets of per-corridor lists (left empty with a shared list).
+const char* scan_sweep(Sweep& w, int P, const fq_pair_assign* as, const fq_pair_decomp* dc, FqCorridorSizes* c, int* n_obs,
+                       std::vector<long long>* ofs)
 {
   if (!dc)
   {
@@ -701,11 +707,10 @@ const char* scan_sweep(Sweep& w, int P, const fq_pair_assign* as, const fq_pair_
   if ((w.feasible == nullptr) != (w.cost == nullptr)) return "feasible_* and cost_* must be given (or omitted) together";
   if (as)
   {
-    std::vector<long long> ofs;
-    if (const char* why = fq_list_offsets(P, w.poly_ofs, w.N, as->all_limit, w.n_fac, w.init, w.final_, w.inc, &ofs, &w.max_fac,
+    if (const char* why = fq_list_offsets(P, w.poly_ofs, w.N, as->all_limit, w.n_fac, w.init, w.final_, w.inc, ofs, &w.max_fac,
                                           &w.max_poly))
       return why;
-    w.n_cand = (long)ofs[P];
+    w.n_cand = (long)(*ofs)[P];
     return nullptr;
   }
   if (c->n_poly > 0 && !w.sigmas) return "sigmas_* is NULL";
@@ -716,22 +721,29 @@ const char* scan_sweep(Sweep& w, int P, const fq_pair_assign* as, const fq_pair_
   w.n_cand = (long)P * w.n_fac * w.n_sig;
   return nullptr;
 }
-}  // namespace
 
-int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results,
-                            const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex, const fq_pair_decomp* dc,
-                            const fq_pair_hr* hr, const fq_pair_map* mp)
+// A submission checked against the caller's host arrays: its two sweeps, sized by scan_sweep, their corridors' sizes and
+// clouds' points, the unknown clouds' points, and with per-corridor lists each sweep's candidate offsets
+struct Checked
 {
-  if (!ctx) return FQ_E_ARG;
-  if (int rc = fq_settle(ctx)) return rc;
   Sweep sw[2];
-  if (int rc = check_chain(ctx, a, as, win, ex, dc, sw, mp)) return rc;
+  FqCorridorSizes cs[2];
+  int n_obs[2] = { 0, 0 };
+  int n_unk = 0;
+  std::vector<long long> cand_ofs[2];
+};
+
+// Every check of a host-pointer submission: everything that reads the caller's host memory and can refuse.  It writes
+// nothing but *k, so a refused submission leaves every output as it was.
+int check_host(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex,
+               const fq_pair_decomp* dc, const fq_pair_hr* hr, const fq_pair_map* mp, Checked* k)
+{
+  if (int rc = check_chain(ctx, a, as, win, ex, dc, k->sw, mp)) return rc;
   const int P = a->n_prob;
   if (!fq_scan_all_finite(a->x0, 9 * (size_t)P)) return fq_fail(ctx, FQ_E_ARG, "non-finite value in x0/xf");
   if (!fq_scan_all_positive_finite(a->lim, 3 * (size_t)P)) return fq_fail(ctx, FQ_E_ARG, "limits and factors must be finite and > 0");
   if (dc && dc->goal && !fq_scan_all_finite(dc->goal, 3 * (size_t)P))
     return fq_fail(ctx, FQ_E_ARG, "decomp: non-finite value in a path, a cloud or the goal");
-  int n_unk = 0, largest_unk = 0;
   if (mp)
   {
     if (int rc = check_map(ctx, dc, hr, win, mp)) return rc;
@@ -740,14 +752,27 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   }
   else if (hr)
   {
+    int largest_unk = 0;
     if (int rc = check_hr(ctx, win, dc, hr)) return rc;
-    if (!scan_offsets(hr->unk_ofs, P, 1 << 30, &n_unk, &largest_unk)) return fq_fail(ctx, FQ_E_ARG, "hr: unk_ofs must start at 0 and be non-decreasing");
-    if (!fq_scan_all_finite(hr->unk, 3 * (size_t)n_unk)) return fq_fail(ctx, FQ_E_ARG, "hr: non-finite value in an unknown cloud");
+    if (!scan_offsets(hr->unk_ofs, P, 1 << 30, &k->n_unk, &largest_unk)) return fq_fail(ctx, FQ_E_ARG, "hr: unk_ofs must start at 0 and be non-decreasing");
+    if (!fq_scan_all_finite(hr->unk, 3 * (size_t)k->n_unk)) return fq_fail(ctx, FQ_E_ARG, "hr: non-finite value in an unknown cloud");
   }
-  FqCorridorSizes cs[2];
-  int n_obs[2] = { 0, 0 };
   for (int i = 0; i < 2; i++)
-    if (const char* why = scan_sweep(sw[i], P, as, dc, &cs[i], &n_obs[i])) return fq_fail(ctx, FQ_E_ARG, why);
+    if (const char* why = scan_sweep(k->sw[i], P, as, dc, &k->cs[i], &k->n_obs[i], &k->cand_ofs[i])) return fq_fail(ctx, FQ_E_ARG, why);
+  return 0;
+}
+
+// A checked submission onto the device and back: one packed upload, the chain (through the _dev entry of its kind), the
+// outputs straight into the caller's arrays.  d_results (may be NULL) receives the device address of the result records;
+// copy_results = false leaves the caller's `results` untouched (the sharded chain reads the all-gathered table instead).
+int submit_host(fq_ctx* ctx, const Checked& k, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results,
+                const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex, const fq_pair_decomp* dc,
+                const fq_pair_hr* hr, const fq_pair_map* mp)
+{
+  const int P = a->n_prob, n_unk = k.n_unk;
+  const Sweep* sw = k.sw;
+  const FqCorridorSizes* cs = k.cs;
+  const int* n_obs = k.n_obs;
   FQ_CUDA(cudaSetDevice(ctx->device));
   // ---- one packed upload of the inputs and one block for the outputs.  stage() runs twice: to size them, then to copy
   //      the inputs into the pinned staging buffer and point the device copies of the structs at both
@@ -851,15 +876,142 @@ int fq_replan_pairs_host_ex(fq_ctx* ctx, const fq_pair_args* a, bool deferred, f
   return 0;
 }
 
+// a host-pointer chain on one GPU.  The context settles before the check: a deferred call may still be copying into
+// arrays this one reads (a window's next_* passed on as the next init_* / final_*).
+int host_chain(fq_ctx* ctx, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results,
+               const fq_pair_assign* as = nullptr, const fq_pair_window* win = nullptr, const fq_pair_exact* ex = nullptr,
+               const fq_pair_decomp* dc = nullptr, const fq_pair_hr* hr = nullptr, const fq_pair_map* mp = nullptr)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (int rc = fq_settle(ctx)) return rc;
+  Checked k;
+  if (int rc = check_host(ctx, a, as, win, ex, dc, hr, mp, &k)) return rc;
+  return submit_host(ctx, k, a, deferred, d_results, copy_results, as, win, ex, dc, hr, mp);
+}
+
+// checked sweep w cut to the corridors [lo, hi) (ofs: its candidate offsets, empty with a shared list): corridor offsets
+// rebased into *sub, per-corridor arrays from corridor lo, per-candidate outputs from the shard's first candidate.  The
+// candidate offsets are not the shard's to write.  The exact and decomposing fields are not cut: those chains are refused
+// on multi-GPU contexts (lists_host), so they are NULL here.
+Sweep cut_sweep(Sweep w, const std::vector<long long>& ofs, int lo, int hi, FqSubCorridors* sub)
+{
+  sub->build(w.poly_ofs, w.face_ofs, w.Ab, lo, hi);
+  w.poly_ofs = sub->poly_ofs.data();  w.face_ofs = sub->face_ofs.data();  w.Ab = sub->Ab;
+  const size_t j = (size_t)lo, NP = (size_t)w.N * lo, c0 = ofs.empty() ? (size_t)w.n_fac * w.n_sig * lo : (size_t)ofs[lo];
+  auto at = [](auto* p, size_t o) { return p ? p + o : p; };
+  w.xf = at(w.xf, 9 * j);  w.coeffs = at(w.coeffs, 12 * NP);  w.sigma_out = at(w.sigma_out, NP);
+  w.feasible = at(w.feasible, c0);  w.cost = at(w.cost, c0);
+  w.init = at(w.init, j);  w.final_ = at(w.final_, j);  w.factor = at(w.factor, j);  w.trials = at(w.trials, j);
+  w.next_init = at(w.next_init, j);  w.next_final = at(w.next_final, j);
+  w.cand_ofs_out = nullptr;
+  return w;
+}
+
+// one shard of a sharded call: its structs (pointing into the caller's arrays and the rebased offsets) and its check
+struct Shard
+{
+  fq_pair_args a{};
+  fq_pair_assign as{};
+  fq_pair_window win{};
+  FqSubCorridors sub[2];
+  Checked k;
+};
+
+// The chain on a multi-GPU context (fq_replan_pairs*, _assign*, _window*).  Group (one process): corridors [lo_i, hi_i) go
+// to member i, every member runs its chain, the result records are all-gathered (padded to the largest shard) and read
+// back once from member 0; the per-candidate arrays travel straight from each member into the caller's arrays.  Rank
+// context (one process per GPU): every rank passes the SAME full description and solves its own shard; after the
+// all-gather every rank holds every corridor's result record, while per-candidate outputs are filled for the rank's own
+// corridors only.
+// Nothing is written or enqueued before two checks pass, on every rank alike.  The whole description is checked as a
+// plain context checks it, so what a plain context refuses is refused with the same message.  Then every shard of the
+// world is cut and checked, which also sizes it as the same batch on one GPU.  A shard's check is not always implied by
+// the whole one: a shared list may name a polytope a corridor lacks when some corridor of the batch has none (the bound
+// is then skipped), so corridors with P = {0, 1} and the entry 1 pass as a whole but not as the shard [1, 2).  Checking
+// every shard on every rank keeps the ranks' decisions equal even then.
+// Shared lists: equal corridor counts per shard.  Per-corridor lists: the shards are balanced by candidates (fq_shard_range
+// over the summed whole + safe offsets), and each shard's per-candidate outputs start at its first offset.
+int sharded_chain(fq_ctx* g, const fq_pair_args* a, bool deferred, const fq_pair_assign* as, const fq_pair_window* win)
+{
+  fq_ctx* ctx = g;
+  if (int rc = fq_settle(g)) return rc;            // every member (see host_chain)
+  Checked k;
+  if (int rc = check_host(g, a, as, win, nullptr, nullptr, nullptr, nullptr, &k)) return rc;
+  const int P = a->n_prob, world = g->world;
+  const bool group = g->is_group;
+  const int n_local = group ? world : 1;
+  std::vector<int> weight;
+  if (as)
+  {
+    weight.assign(P + 1, 0);
+    for (int j = 1; j <= P; j++) weight[j] = (int)std::min<long long>(k.cand_ofs[0][j] + k.cand_ofs[1][j], 0x7fffffffLL);
+  }
+  int pad = 0;
+  std::vector<int> lo(world), hi(world);
+  std::vector<Shard> shard(world);
+  for (int r = 0; r < world; r++)
+  {
+    fq_shard_range(P, as ? weight.data() : nullptr, r, world, &lo[r], &hi[r]);
+    pad = std::max(pad, hi[r] - lo[r]);
+    if (hi[r] <= lo[r]) continue;
+    Shard& s = shard[r];
+    s.a = *a;
+    s.a.n_prob = hi[r] - lo[r];  s.a.x0 = a->x0 + 9 * (size_t)lo[r];  s.a.lim = a->lim + 3 * (size_t)lo[r];
+    s.a.results = a->results + lo[r];           // not copied back (copy_results = false): the gathered table is
+    if (as) s.as = *as;
+    if (win) s.win = *win;
+    for (int h = 0; h < 2; h++)
+      put_sweep(cut_sweep(k.sw[h], k.cand_ofs[h], lo[r], hi[r], &s.sub[h]), h, &s.a, as ? &s.as : nullptr, win ? &s.win : nullptr,
+                nullptr, nullptr);
+    if (int rc = check_host(g, &s.a, as ? &s.as : nullptr, win ? &s.win : nullptr, nullptr, nullptr, nullptr, nullptr, &s.k)) return rc;
+  }
+  for (int i = 0; as && i < 2; i++)
+    for (int j = 0; k.sw[i].cand_ofs_out && j <= P; j++) k.sw[i].cand_ofs_out[j] = (int)k.cand_ofs[i][j];
+  std::vector<void*> d_res(n_local, nullptr), d_all(n_local, nullptr);
+  for (int i = 0; i < n_local; i++)
+  {
+    fq_ctx* c = group ? fq_member(g, i) : g;
+    const int r = group ? i : g->rank;
+    cudaSetDevice(c->device);
+    // gather buffers: [pad records to send | world x pad records received]
+    cudaError_t e = c->d_out.reserve(sizeof(fq_pair_result) * (size_t)pad * (world + 1));
+    if (e != cudaSuccess) return fq_cuda_fail(g, e, "gather buffer");
+    fq_pair_result* res = (fq_pair_result*)c->d_out.p;
+    d_res[i] = res;
+    d_all[i] = res + pad;
+    e = cudaMemsetAsync(res, 0xff, sizeof(fq_pair_result) * (size_t)pad, c->stream);
+    if (e != cudaSuccess) return fq_cuda_fail(g, e, "gather buffer");
+    if (hi[r] <= lo[r]) continue;
+    Shard& s = shard[r];
+    fq_pair_result* dr = nullptr;
+    int rc = submit_host(c, s.k, &s.a, true, &dr, false, as ? &s.as : nullptr, win ? &s.win : nullptr, nullptr, nullptr, nullptr, nullptr);
+    if (rc) { if (c != g) g->err = c->err; return rc; }
+    e = cudaMemcpyAsync(res, dr, sizeof(fq_pair_result) * (size_t)s.a.n_prob, cudaMemcpyDeviceToDevice, c->stream);
+    if (e != cudaSuccess) return fq_cuda_fail(g, e, "gather staging");
+  }
+  if (int rc = fq_exchange(g, d_res, d_all, sizeof(fq_pair_result) * (size_t)pad)) return rc;
+  // ---- the gathered table, shard by shard, into the caller's results (from member 0 / this rank)
+  FQ_CUDA(cudaSetDevice(g->device));
+  const fq_pair_result* all = (const fq_pair_result*)d_all[0];
+  for (int r = 0; r < world; r++)
+    if (hi[r] > lo[r])
+      FQ_CUDA(cudaMemcpyAsync(a->results + lo[r], all + (size_t)r * pad, sizeof(fq_pair_result) * (size_t)(hi[r] - lo[r]),
+                              cudaMemcpyDeviceToHost, g->stream));
+  g->pending = true;
+  if (deferred) return 0;
+  return fq_settle(g);
+}
+}  // namespace
+
 extern "C" int fq_replan_pairs(fq_ctx* ctx, const fq_pair_args* a)
 {
-  if (ctx && (ctx->is_group || ctx->comm)) return fq_replan_pairs_sharded(ctx, a, false);
-  return fq_replan_pairs_host_ex(ctx, a, false, nullptr, true);
+  if (ctx && (ctx->is_group || ctx->comm)) return sharded_chain(ctx, a, false, nullptr, nullptr);
+  return host_chain(ctx, a, false, nullptr, true);
 }
 extern "C" int fq_replan_pairs_async(fq_ctx* ctx, const fq_pair_args* a)
 {
-  if (ctx && (ctx->is_group || ctx->comm)) return fq_replan_pairs_sharded(ctx, a, true);
-  return fq_replan_pairs_host_ex(ctx, a, true, nullptr, true);
+  if (ctx && (ctx->is_group || ctx->comm)) return sharded_chain(ctx, a, true, nullptr, nullptr);
+  return host_chain(ctx, a, true, nullptr, true);
 }
 
 namespace
@@ -874,8 +1026,8 @@ int lists_host(fq_ctx* ctx, const fq_pair_args* a, bool deferred, const fq_pair_
   if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
   if ((ex || dc) && (ctx->is_group || ctx->comm))
     return fq_fail(ctx, FQ_E_ARG, "fq_replan_pairs_exact / _decomp / _hr / _map: multi-GPU contexts are not supported (use the _dev entry)");
-  if (ctx->is_group || ctx->comm) return fq_replan_pairs_sharded(ctx, a, deferred, as, win);
-  return fq_replan_pairs_host_ex(ctx, a, deferred, nullptr, true, as, win, ex, dc, hr, mp);
+  if (ctx->is_group || ctx->comm) return sharded_chain(ctx, a, deferred, as, win);
+  return host_chain(ctx, a, deferred, nullptr, true, as, win, ex, dc, hr, mp);
 }
 }  // namespace
 

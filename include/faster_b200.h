@@ -590,8 +590,16 @@ int fq_replan_pairs_map_dev(fq_ctx* ctx, const fq_pair_args* args, const fq_pair
  * environment variable FQ_NCCL_LIB overrides); single-GPU use never touches it.
  *
  * One process, n_gpus devices (devices == NULL: 0..n_gpus-1).  The returned context is the context of devices[0] for
- * every single-GPU entry point, and a GROUP for fq_replan_pairs / fq_replan_pairs_async / fq_solve_multi_sharded, which
- * spread the corridors over all its devices. */
+ * every single-GPU entry point, and a GROUP for fq_replan_pairs, fq_replan_pairs_assign and fq_replan_pairs_window (sync
+ * and async) and fq_solve_multi_sharded, which spread the corridors over all its devices.
+ *
+ * Those chained-replan entries check the whole description on a multi-GPU context (group or rank) exactly as on a plain
+ * context: what a plain context refuses, they refuse with the same code and fq_last_error text.  They then check every
+ * shard as a one-GPU call of its own.  Both checks run before any output is written (cand_ofs_* included) or any work is
+ * enqueued, and every rank checks every shard, not only its own, so the ranks of a communicator accept or refuse a
+ * description together.  One description passes the first check and not the second: a shared list (sigmas_*) whose
+ * entry names a polytope that a corridor lacks.  A plain context lets that entry through when some corridor of the batch
+ * has no polytope, but a shard without such a corridor refuses it ("sigmas_* entry >= number of polytopes"). */
 int fq_create_multi(fq_ctx** out, int n_gpus, const int* devices);
 /* One process per GPU: rank 0 obtains an id (128 bytes), the launcher distributes it (torch.distributed, MPI, a file),
  * every rank attaches its own context.  Afterwards fq_replan_pairs / fq_solve_multi_sharded on that context solve the
