@@ -20,7 +20,8 @@ EXPORTS = ["fq_abi_version", "fq_create", "fq_destroy", "fq_last_error", "fq_set
            "fq_replan_pairs_exact", "fq_replan_pairs_exact_async", "fq_replan_pairs_exact_dev", "fq_replan_pairs_decomp",
            "fq_replan_pairs_decomp_async", "fq_replan_pairs_decomp_dev", "fq_replan_pairs_hr", "fq_replan_pairs_hr_async",
            "fq_replan_pairs_hr_dev", "fq_map_create", "fq_map_destroy", "fq_map_update", "fq_map_update_dev", "fq_map_size",
-           "fq_replan_pairs_map", "fq_replan_pairs_map_async", "fq_replan_pairs_map_dev"]
+           "fq_replan_pairs_map", "fq_replan_pairs_map_async", "fq_replan_pairs_map_dev", "fq_replan_pairs_plan",
+           "fq_replan_pairs_plan_async", "fq_replan_pairs_plan_dev"]
 
 
 class FqError(RuntimeError):
@@ -97,6 +98,15 @@ class PairHR(C.Structure):
 class PairMap(C.Structure):
     """fq_pair_map of include/faster_b200.h: the indexed maps the corridors of a submission read."""
     _fields_ = [("maps", C.c_void_p), ("n_maps", C.c_int), ("map_index", C.c_void_p), ("max_local", C.c_int)]
+
+
+class PairPlan(C.Structure):
+    """fq_pair_plan of include/faster_b200.h: every corridor's committed plan piece, sampled on the device."""
+    _fields_ = [("cap_states", C.c_longlong), ("states", C.c_void_p), ("plan_ofs", C.c_void_p), ("status", C.c_void_p)]
+
+
+PLAN_OK, PLAN_NONE, PLAN_CAPACITY = 0, 1, 2                             # FQ_PLAN_*
+PLAN_KEYS = ["states", "plan_ofs", "status"]
 
 
 HR_OUT_KEYS = ["last_factor_safe", "index_H", "need_safe"]
@@ -178,6 +188,9 @@ def lib():
         L.fq_replan_pairs_map.argtypes = L.fq_replan_pairs_hr.argtypes + [C.POINTER(PairMap)]
         L.fq_replan_pairs_map_async.argtypes = L.fq_replan_pairs_map.argtypes
         L.fq_replan_pairs_map_dev.argtypes = L.fq_replan_pairs_map.argtypes + [C.c_void_p, C.c_void_p]
+        L.fq_replan_pairs_plan.argtypes = L.fq_replan_pairs_map.argtypes + [C.POINTER(PairPlan)]
+        L.fq_replan_pairs_plan_async.argtypes = L.fq_replan_pairs_plan.argtypes
+        L.fq_replan_pairs_plan_dev.argtypes = L.fq_replan_pairs_plan.argtypes + [C.c_void_p, C.c_void_p]
         L.fq_map_create.argtypes = [C.POINTER(C.c_void_p), C.c_int]
         L.fq_map_destroy.argtypes = [C.c_void_p]
         L.fq_map_destroy.restype = None
@@ -318,6 +331,15 @@ def hr_args(unk_ofs, unk, out_ptrs, drone_radius=HR_DEFAULTS["drone_radius"], de
     s.unk_ofs, s.unk = unk_ofs, unk
     s.drone_radius, s.delta_a, s.delta_H = float(drone_radius), float(delta_a), float(delta_H)
     for k in HR_OUT_KEYS:
+        setattr(s, k, out_ptrs.get(k) or None)
+    return s
+
+
+def plan_args(cap_states, out_ptrs):
+    """PairPlan; out_ptrs: addresses of PLAN_KEYS (status may be 0/None/missing = NULL)."""
+    s = PairPlan()
+    s.cap_states = int(cap_states)
+    for k in PLAN_KEYS:
         setattr(s, k, out_ptrs.get(k) or None)
     return s
 
@@ -603,10 +625,11 @@ class Solver:
     def allgather_dev(self, d_send, d_recv, nbytes, stream=0):
         self._check(self._L.fq_allgather_dev(self._h, d_send, d_recv, int(nbytes), stream or None))
 
-    def replan_pairs(self, w, want_candidates=True, want_coeffs=True, deferred=False, out=None):
+    def replan_pairs(self, w, want_candidates=True, want_coeffs=True, deferred=False, out=None, plan=None):
         """fq_replan_pairs on a make_pair_workload dict (host arrays).  -> dict(results (structured array), feasible_whole,
         cost_whole, feasible_safe, cost_safe, coeffs_whole, coeffs_safe).  deferred: valid after wait(); `out` reuses a
-        previous return value's arrays (keep it and `w` alive until then)."""
+        previous return value's arrays (keep it and `w` alive until then).  plan: a PairPlan (plan_args) for
+        fq_replan_pairs_plan (replan_pairs_plan)."""
         n = w["n_prob"]
         ncw = n * len(w["factors_whole"]) * len(w["sigmas_whole"])
         ncs = n * len(w["factors_safe"]) * len(w["sigmas_safe"])
@@ -618,9 +641,39 @@ class Solver:
             if want_coeffs:
                 out.update(coeffs_whole=np.zeros((n, w["N_whole"], 12)), coeffs_safe=np.zeros((n, w["N_safe"], 12)))
         a = pair_args(w, lambda k: w[k].ctypes.data, {k: v.ctypes.data for k, v in out.items()})
-        fn = self._L.fq_replan_pairs_async if deferred else self._L.fq_replan_pairs
-        self._check(fn(self._h, C.byref(a)))
+        self._submit("", deferred, [C.byref(a)], plan)
         return out
+
+    def _submit(self, family, deferred, structs, plan):
+        """The host entry fq_replan_pairs<family> (sync or async) with `structs` (ctypes references or None, in its argument
+        order), or, given a PairPlan, fq_replan_pairs_plan with the same structs and the plan."""
+        if plan is None:
+            fn = getattr(self._L, "fq_replan_pairs" + family + ("_async" if deferred else ""))
+            self._check(fn(self._h, *structs))
+        else:
+            fn = self._L.fq_replan_pairs_plan_async if deferred else self._L.fq_replan_pairs_plan
+            self._check(fn(self._h, *(list(structs) + [None] * (7 - len(structs))), C.byref(plan)))
+
+    def replan_pairs_plan(self, w, cap_states, chain="assign", *args, **kw):
+        """fq_replan_pairs_plan: the chained replan `chain` -- "shared" (replan_pairs), "assign", "window", "exact", "decomp",
+        "hr" or "map" (replan_pairs_<chain>) -- called with `args` / `kw` as that method takes them, which also returns every
+        corridor's committed plan piece.  -> that method's dict plus states (cap_states x 12), plan_ofs (int64, n_prob + 1:
+        corridor j is rows plan_ofs[j] .. plan_ofs[j+1]-1; plan_ofs[-1] = the rows the batch needs) and status (int32,
+        PLAN_*).  With deferred=True they are valid after wait()."""
+        n, cap = w["n_prob"], int(cap_states)
+        po = dict(states=np.zeros((max(cap, 1), 12))[:cap], plan_ofs=np.zeros(n + 1, np.int64), status=np.zeros(n, np.int32))
+        pl = plan_args(cap, {k: v.ctypes.data for k, v in po.items()})
+        fam = self.replan_pairs if chain == "shared" else getattr(self, "replan_pairs_" + chain)
+        out = fam(w, *args, plan=pl, **kw)
+        out.update(po)
+        return out
+
+    def replan_pairs_plan_dev(self, a, s, win, ex, dc, hr, mp, plan, results_all=0, stream=0):
+        """fq_replan_pairs_plan_dev: the structs of the selected family's _dev entry (s None: the shared lists; any of win,
+        ex, dc, hr, mp None), with `plan` (PairPlan) holding device addresses."""
+        B = lambda x: C.byref(x) if x is not None else None  # noqa: E731
+        self._check(self._L.fq_replan_pairs_plan_dev(self._h, C.byref(a), B(s), B(win), B(ex), B(dc), B(hr), B(mp), C.byref(plan),
+                                                     results_all or None, stream or None))
 
     def _list_outputs(self, w, all_limit, windows, inc, gamma, want_candidates, want_coeffs, extra=()):
         """What the per-corridor-list entries share: each sweep's candidate offsets, from the factors_* of `w` or from
@@ -654,7 +707,7 @@ class Solver:
         wa.arrays = wins                        # keeps the window arrays wa points to alive as long as wa
         return out, s, wa
 
-    def replan_pairs_assign(self, w, all_limit=0, want_candidates=True, want_coeffs=True, deferred=False):
+    def replan_pairs_assign(self, w, all_limit=0, want_candidates=True, want_coeffs=True, deferred=False, plan=None):
         """fq_replan_pairs_assign on a make_pair_workload dict (host arrays; its sigmas_* are not used: every corridor
         gets its own list L(N, P_j, all_limit)).  -> dict(results, feasible_*/cost_* (per candidate, corridor j at
         cand_ofs_*[j] .. cand_ofs_*[j+1]), coeffs_*, cand_ofs_whole, cand_ofs_safe, sigma_whole, sigma_safe (the winners'
@@ -662,11 +715,11 @@ class Solver:
         out, s, _ = self._list_outputs(w, all_limit, None, 1.0, 20.0, want_candidates, want_coeffs)
         a = pair_args(w, lambda k: None if k.startswith("sigmas_") else w[k].ctypes.data, {k: v.ctypes.data for k, v in out.items()})
         a.n_sig_whole = a.n_sig_safe = 0
-        fn = self._L.fq_replan_pairs_assign_async if deferred else self._L.fq_replan_pairs_assign
-        self._check(fn(self._h, C.byref(a), C.byref(s)))
+        self._submit("_assign", deferred, [C.byref(a), C.byref(s)], plan)
         return out
 
-    def replan_pairs_window(self, w, windows, all_limit=0, inc=1.0, gamma=20.0, want_candidates=True, want_coeffs=True, deferred=False):
+    def replan_pairs_window(self, w, windows, all_limit=0, inc=1.0, gamma=20.0, want_candidates=True, want_coeffs=True, deferred=False,
+                            plan=None):
         """fq_replan_pairs_window on a make_pair_workload dict (host arrays; its factors_* and sigmas_* are not used: corridor
         j sweeps its own window F_j and list L_j).  windows: dict of n_prob-arrays init_whole, final_whole, init_safe,
         final_safe; inc / gamma as window_args.  -> the dict of replan_pairs_assign plus factor_*, trials_* and the next
@@ -675,12 +728,11 @@ class Solver:
         a = pair_args(w, lambda k: None if k.startswith(("sigmas_", "factors_")) else w[k].ctypes.data,
                       {k: v.ctypes.data for k, v in out.items()})
         a.n_sig_whole = a.n_sig_safe = a.n_fac_whole = a.n_fac_safe = 0
-        fn = self._L.fq_replan_pairs_window_async if deferred else self._L.fq_replan_pairs_window
-        self._check(fn(self._h, C.byref(a), C.byref(s), C.byref(wa)))
+        self._submit("_window", deferred, [C.byref(a), C.byref(s), C.byref(wa)], plan)
         return out
 
     def replan_pairs_exact(self, w, all_limit=0, windows=None, inc=1.0, gamma=20.0, want_candidates=True, want_coeffs=True,
-                           deferred=False):
+                           deferred=False, plan=None):
         """fq_replan_pairs_exact on a make_pair_workload dict (host arrays; its sigmas_* are not used).  windows=None: the shared
         factor lists factors_* of `w`, as replan_pairs_assign; otherwise per-corridor windows as replan_pairs_window.  -> the
         dict of replan_pairs_assign (or _window) plus exact_whole, exact_safe (int32: 1 = the minimum over all assignments)
@@ -695,26 +747,25 @@ class Solver:
         if windows is not None:
             a.n_fac_whole = a.n_fac_safe = 0
         ex = exact_args({k: out[k].ctypes.data for k in EXACT_KEYS})
-        fn = self._L.fq_replan_pairs_exact_async if deferred else self._L.fq_replan_pairs_exact
-        self._check(fn(self._h, C.byref(a), C.byref(s), C.byref(wa) if wa is not None else None, C.byref(ex)))
+        self._submit("_exact", deferred, [C.byref(a), C.byref(s), C.byref(wa) if wa is not None else None, C.byref(ex)], plan)
         return out
 
     def replan_pairs_decomp(self, w, all_limit=0, windows=None, inc=1.0, gamma=20.0, exact=False, bbox=(2.0, 2.0, 1.0),
-                            inflate=0.42, z_ground=0.0, use_goal=True, want_candidates=False, want_coeffs=True, deferred=False):
+                            inflate=0.42, z_ground=0.0, use_goal=True, want_candidates=False, want_coeffs=True, deferred=False,
+                            plan=None):
         """fq_replan_pairs_decomp on a make_decomp_workload dict (host arrays) with its factors_whole / factors_safe (shared
         factor lists) or `windows` (per-corridor windows, as replan_pairs_window); exact=True adds the exact stage.  -> the
         dict of replan_pairs_assign (plus the window / exact outputs when asked for) and the corridors the sweeps used:
         face_ofs_* / Ab_* (CSR), E, M (n_prob x 3) and status_whole / status_safe (FQ_DECOMP_*).  deferred: valid after wait()."""
         out, structs = self._decomp_structs(w, all_limit, windows, inc, gamma, exact, bbox, inflate, z_ground, use_goal,
                                             want_candidates, want_coeffs)
-        fn = self._L.fq_replan_pairs_decomp_async if deferred else self._L.fq_replan_pairs_decomp
-        self._check(fn(self._h, *structs))
+        self._submit("_decomp", deferred, structs, plan)
         return out
 
     def replan_pairs_hr(self, w, last_factor_safe=None, drone_radius=HR_DEFAULTS["drone_radius"], delta_a=HR_DEFAULTS["delta_a"],
                         delta_H=HR_DEFAULTS["delta_H"], all_limit=0, windows=None, inc=1.0, gamma=20.0, exact=False,
                         bbox=(2.0, 2.0, 1.0), inflate=0.42, z_ground=0.0, use_goal=True, want_candidates=False, want_coeffs=True,
-                        deferred=False):
+                        deferred=False, plan=None):
         """fq_replan_pairs_hr on a make_decomp_workload dict with unknown clouds (unk_ofs, unk): replan_pairs_decomp with H and
         R chosen from the clouds.  last_factor_safe: n_prob factors (default 0, the start-up value; required in effect with
         `windows`).  -> the dict of replan_pairs_decomp plus index_H (int32), need_safe (uint8) and last_factor_safe (the
@@ -726,14 +777,13 @@ class Solver:
                                             want_candidates, want_coeffs, extra)
         hr = hr_args(w["unk_ofs"].ctypes.data, w["unk"].ctypes.data, {k: out[k].ctypes.data for k in HR_OUT_KEYS}, drone_radius,
                      delta_a, delta_H)
-        fn = self._L.fq_replan_pairs_hr_async if deferred else self._L.fq_replan_pairs_hr
-        self._check(fn(self._h, *structs, C.byref(hr)))
+        self._submit("_hr", deferred, structs + [C.byref(hr)], plan)
         return out
 
     def replan_pairs_map(self, w, maps, map_index=None, max_local=4096, hr=True, last_factor_safe=None,
                          drone_radius=HR_DEFAULTS["drone_radius"], delta_a=HR_DEFAULTS["delta_a"], delta_H=HR_DEFAULTS["delta_H"],
                          all_limit=0, windows=None, inc=1.0, gamma=20.0, exact=False, bbox=(2.0, 2.0, 1.0), inflate=0.42,
-                         z_ground=0.0, use_goal=True, want_candidates=False, want_coeffs=True, deferred=False):
+                         z_ground=0.0, use_goal=True, want_candidates=False, want_coeffs=True, deferred=False, plan=None):
         """fq_replan_pairs_map on a make_decomp_workload dict (its clouds obs_* / unk are not used): every corridor reads the
         Map maps[map_index[j]] (map_index None: maps[0]).  hr=True: as replan_pairs_hr, with corridor j's unknown cloud U
         and occupied cloud O from its map (whole: O, safe: U ++ O); hr=False: as replan_pairs_decomp.  max_local caps the
@@ -747,8 +797,7 @@ class Solver:
                                             want_candidates, want_coeffs, extra, clouds=False)
         h = hr_args(None, None, {k: out[k].ctypes.data for k in HR_OUT_KEYS}, drone_radius, delta_a, delta_H) if hr else None
         mp = map_args(maps, map_index, max_local)
-        fn = self._L.fq_replan_pairs_map_async if deferred else self._L.fq_replan_pairs_map
-        self._check(fn(self._h, *structs, C.byref(h) if h is not None else None, C.byref(mp)))
+        self._submit("_map", deferred, structs + [C.byref(h) if h is not None else None, C.byref(mp)], plan)
         if deferred:
             out["_keep"] = mp
         return out

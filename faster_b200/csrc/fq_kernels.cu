@@ -780,6 +780,14 @@ cudaError_t fq_launch_pair_final(const FqPairFinalArgs& a, cudaStream_t stream)
   return cudaGetLastError();
 }
 
+cudaError_t fq_launch_pair_plan(const FqPairPlanArgs& a, cudaStream_t stream)
+{
+  if (a.n_prob <= 0) return cudaSuccess;
+  fqp::fq_pair_plan_offsets_kernel<<<1, 1024, 0, stream>>>(a);
+  fqp::fq_pair_plan_sample_kernel<<<a.n_prob, 128, 0, stream>>>(a);
+  return cudaGetLastError();
+}
+
 size_t fq_decomp_spill_n(int max_obs) { return max_obs > fqd::kFitPts ? (size_t)(max_obs - fqd::kFitPts) : 0; }
 
 cudaError_t fq_launch_decomp(const FqDecompArgs& a, cudaStream_t stream)

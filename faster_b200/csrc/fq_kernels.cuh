@@ -275,6 +275,24 @@ struct FqPairWindowArgs
   double* last_factor_safe = nullptr;
 };
 
+// the plan piece of every corridor (fq_replan_pairs_plan*, fq_pair.cuh): whole samples 0 .. k_safe, then every safe sample,
+// each as fq_fill_x writes it with the winner's full sample count
+struct FqPairPlanArgs
+{
+  int n_prob, N_w, N_s;
+  double DC;
+  const int *win_idx_w, *win_idx_s;     // n_prob: the sweeps' winners (-1: none)
+  const double *win_dt_w, *win_dt_s;    // n_prob
+  const int *n_samples, *k_safe;        // n_prob: fq_pair_mid_kernel's
+  const uint8_t* need;                  // n_prob: needToComputeSafePath (fq_pair_hr_kernel), or NULL: a safe path is always needed
+  const double *coeffs_w, *coeffs_s;    // n_prob x N x 12: the winners' coefficients
+  long long cap;                        // rows of states
+  double* states;                       // out: cap x 12
+  long long* plan_ofs;                  // out: n_prob + 1, the exclusive scan of every succeeding corridor's rows
+  int* status;                          // out n_prob (FQ_PLAN_*), or NULL
+};
+cudaError_t fq_launch_pair_plan(const FqPairPlanArgs& a, cudaStream_t stream);
+
 // the device decomposition of one sweep's corridors (fq_decomp.cuh): fq_decomp_kernel stages every polytope's rows in a slot
 // of cap_pf rows (slot j * max_poly + s), fq_decomp_csr_kernel packs them into the sweep's CSR and sets the final states
 struct FqDecompArgs

@@ -469,4 +469,79 @@ __global__ void fq_pair_window_kernel(const FqPairWindowArgs a)
   if (a.next_init_s) a.next_init_s[j] = ni;
   if (a.next_final_s) a.next_final_s[j] = nf;
 }
+
+// ---- the plan piece of every corridor (fq_replan_pairs_plan*): what appendToPlan pushes (faster.cpp:606-648), whole
+//      X_temp_[0 .. k_safe] followed by the whole safe X_temp_, each sampled as fillX does with the winner's full count
+
+// corridor j's rows: 0 when the replan returns early (no whole winner, or a needed safe path without a safe winner:
+// faster.cpp:420-424, :529-533), else k_safe + 1 + n_s (n_s = 0 when no safe path is needed; then k_safe = n_w - 1).
+// *k and *n_s receive k_safe and the safe sample count.
+FQ_HD long long plan_rows(const FqPairPlanArgs& a, int j, int* k, int* n_s)
+{
+  *k = -1; *n_s = 0;
+  if (a.win_idx_w[j] < 0) return 0;
+  const bool need = !a.need || a.need[j];
+  if (need && a.win_idx_s[j] < 0) return 0;
+  *k = a.k_safe[j];
+  *n_s = need ? fqdt::num_samples(a.N_s, a.win_dt_s[j], a.DC) : 0;
+  return (long long)*k + 1 + *n_s;
+}
+
+// plan_ofs = the exclusive scan of every corridor's rows (64 bits: nothing bounds the sum), and the statuses: a corridor
+// whose rows end past cap is FQ_PLAN_CAPACITY.  One CTA (any size up to 1024): every thread takes a contiguous run of
+// corridors, thread 0 scans the runs' sums.
+__global__ void __launch_bounds__(1024) fq_pair_plan_offsets_kernel(const FqPairPlanArgs a)
+{
+  __shared__ long long s_run[1024];
+  const int T = blockDim.x, tid = threadIdx.x;
+  const int per = (a.n_prob + T - 1) / T;
+  const int j0 = min(a.n_prob, tid * per), j1 = min(a.n_prob, j0 + per);
+  int k, ns;
+  long long sum = 0;
+  for (int j = j0; j < j1; j++) sum += plan_rows(a, j, &k, &ns);
+  s_run[tid] = sum;
+  __syncthreads();
+  if (tid == 0)
+  {
+    long long run = 0;
+    for (int i = 0; i < T; i++) { const long long x = s_run[i]; s_run[i] = run; run += x; }
+    a.plan_ofs[a.n_prob] = run;
+  }
+  __syncthreads();
+  long long run = s_run[tid];
+  for (int j = j0; j < j1; j++)
+  {
+    const long long r = plan_rows(a, j, &k, &ns);
+    a.plan_ofs[j] = run;
+    if (a.status) a.status[j] = r == 0 ? FQ_PLAN_NONE : (run + r > a.cap ? FQ_PLAN_CAPACITY : FQ_PLAN_OK);
+    run += r;
+  }
+}
+
+// the rows of every corridor that fits, after fq_pair_plan_offsets_kernel.  One CTA per corridor (any block size): each
+// thread takes a contiguous run of the piece's rows, replays the sample clock of its side to the run's first sample and
+// walks on from there, so a corridor costs O(threads x rows) clock steps, not O(rows^2).
+__global__ void __launch_bounds__(128) fq_pair_plan_sample_kernel(const FqPairPlanArgs a)
+{
+  const int j = blockIdx.x;
+  if (j >= a.n_prob) return;
+  const long long base = a.plan_ofs[j], rows = a.plan_ofs[j + 1] - base;
+  if (rows <= 0 || base + rows > a.cap) return;          // nothing to append, or past the capacity (FQ_PLAN_CAPACITY)
+  int k, ns;
+  plan_rows(a, j, &k, &ns);
+  const int nw = a.n_samples[j];
+  const long long per = (rows + blockDim.x - 1) / blockDim.x, r0 = per * threadIdx.x;
+  const long long r1 = r0 + per < rows ? r0 + per : rows;
+  const double* cw = a.coeffs_w + (size_t)j * a.N_w * 12;
+  const double* cs = a.coeffs_s + (size_t)j * a.N_s * 12;
+  SampleClock clock_w, clock_s;
+  for (long long r = r0; r < r1; r++)
+  {
+    double o[12];
+    if (r <= k) sample_at(clock_w, (int)r, cw, a.N_w, a.win_dt_w[j], a.DC, nw, o);
+    else sample_at(clock_s, (int)(r - k - 1), cs, a.N_s, a.win_dt_s[j], a.DC, ns, o);
+    double* out = a.states + 12 * (size_t)(base + r);
+    for (int q = 0; q < 12; q++) out[q] = o[q];
+  }
+}
 }  // namespace fqp

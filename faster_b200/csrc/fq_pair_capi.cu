@@ -327,8 +327,8 @@ long long longest_list(int N, int max_poly, long long all_limit)
 // the chain itself, every pointer a device pointer and every argument checked.  as == NULL: the shared lists of `a`;
 // sw: the two sweeps, their candidate counts set by the entry
 int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex,
-              const fq_pair_decomp* dc, const fq_pair_hr* hr, const fq_pair_map* mp, const Sweep* sw, fq_pair_result* results_all,
-              cudaStream_t st)
+              const fq_pair_decomp* dc, const fq_pair_hr* hr, const fq_pair_map* mp, const fq_pair_plan* pl, const Sweep* sw,
+              fq_pair_result* results_all, cudaStream_t st)
 {
   const int P = a->n_prob;
   // decomposing chain: staging slots of both sweeps (the larger), rows per slot, spilled survivors per slot
@@ -487,7 +487,8 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
     m.r_index = sh.hr_r;
   }
   FQ_CUDA(fq_launch_pair_mid(m, st));
-  double* coeffs_s = sw[1].coeffs ? sw[1].coeffs : ex ? ss[1].coeffs : nullptr;
+  // the safe winners' coefficients: wanted, or needed by the exact stage's confirmation or by the plan
+  double* coeffs_s = sw[1].coeffs ? sw[1].coeffs : ex || pl ? ss[1].coeffs : nullptr;
   if (int rc = run_sweep(sw[1], ss[1], sh.x0_safe, sh.x0_safe, coeffs_s, tree.changed_s, 1)) return rc;
 
   FqPairFinalArgs f;
@@ -525,6 +526,16 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
     if (hr) { wa.need_safe = sh.hr_need; wa.last_factor_safe = hr->last_factor_safe; }
     FQ_CUDA(fq_launch_pair_window(wa, st));
   }
+  if (pl)
+  { // ---- the plan pieces (appendToPlan, faster.cpp:606-648) from the winners and k_safe
+    FqPairPlanArgs q;
+    q.n_prob = P; q.N_w = sw[0].N; q.N_s = sw[1].N; q.DC = a->DC;
+    q.win_idx_w = ss[0].win_idx; q.win_idx_s = ss[1].win_idx; q.win_dt_w = ss[0].win_dt; q.win_dt_s = ss[1].win_dt;
+    q.n_samples = sh.n_samples; q.k_safe = sh.k_safe; q.need = hr ? sh.hr_need : nullptr;
+    q.coeffs_w = coeffs_w; q.coeffs_s = coeffs_s;
+    q.cap = pl->cap_states; q.states = pl->states; q.plan_ofs = pl->plan_ofs; q.status = pl->status;
+    FQ_CUDA(fq_launch_pair_plan(q, st));
+  }
   // ---- the path's one exchange: every rank's result records to every rank (north_star: one all-gather, only when the
   //      batch is spread over several GPUs)
   if (results_all && ctx->comm)
@@ -538,7 +549,7 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
 // of the structs is a device pointer; the sweeps' sizes come from the hints of `as` (capacities) and `win` (factor rows)
 int chain_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex,
               const fq_pair_decomp* dc, fq_pair_result* results_all, void* stream_v, const fq_pair_hr* hr = nullptr,
-              const fq_pair_map* mp = nullptr)
+              const fq_pair_map* mp = nullptr, const fq_pair_plan* pl = nullptr)
 {
   if (!ctx) return FQ_E_ARG;
   if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
@@ -562,12 +573,11 @@ int chain_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
     w.ee_width = (int)longest;
   }
   FQ_CUDA(cudaSetDevice(ctx->device));
-  return run_chain(ctx, a, as, win, ex, dc, hr, mp, sw, results_all, stream_v ? (cudaStream_t)stream_v : ctx->stream);
+  return run_chain(ctx, a, as, win, ex, dc, hr, mp, pl, sw, results_all, stream_v ? (cudaStream_t)stream_v : ctx->stream);
 }
-}  // namespace
 
-// every pointer of `a` is a device pointer
-extern "C" int fq_replan_pairs_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_result* results_all, void* stream_v)
+// the chain with the shared lists of `a` (fq_replan_pairs_dev): every pointer of `a` is a device pointer
+int shared_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_result* results_all, void* stream_v, const fq_pair_plan* pl = nullptr)
 {
   if (!ctx) return FQ_E_ARG;
   Sweep sw[2];
@@ -580,8 +590,56 @@ extern "C" int fq_replan_pairs_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_r
     w.ee_width = w.n_sig;
   }
   FQ_CUDA(cudaSetDevice(ctx->device));
-  return run_chain(ctx, a, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, sw, results_all,
+  return run_chain(ctx, a, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, pl, sw, results_all,
                    stream_v ? (cudaStream_t)stream_v : ctx->stream);
+}
+
+// the plan's own refusals (fq_replan_pairs_plan*)
+int check_plan(fq_ctx* ctx, const fq_pair_plan* pl)
+{
+  if (!pl) return fq_fail(ctx, FQ_E_ARG, "plan is NULL");
+  if (!pl->states || !pl->plan_ofs) return fq_fail(ctx, FQ_E_ARG, "plan: states and plan_ofs must not be NULL");
+  if (pl->cap_states < 0) return fq_fail(ctx, FQ_E_ARG, "plan: cap_states < 0");
+  if (ctx->is_group || ctx->comm)
+    return fq_fail(ctx, FQ_E_ARG, "fq_replan_pairs_plan: multi-GPU contexts are not supported (plans are variable-length per corridor)");
+  return 0;
+}
+
+// The device chain the non-NULL structs select (fq_replan_pairs_plan*; the same dispatch as the host entries): the shared
+// lists without assign, else _map, _hr, _decomp, _exact, _window or _assign, each with its own family's checks.
+int family_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex,
+               const fq_pair_decomp* dc, const fq_pair_hr* hr, const fq_pair_map* mp, const fq_pair_plan* pl,
+               fq_pair_result* results_all, void* stream_v)
+{
+  if (!as)
+  {
+    if (win || ex || dc || hr || mp) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
+    return shared_dev(ctx, a, results_all, stream_v, pl);
+  }
+  if (mp)
+  {
+    if (int rc = check_map(ctx, dc, hr, win, mp)) return rc;
+  }
+  else if (hr)
+  {
+    if (int rc = check_hr(ctx, win, dc, hr)) return rc;
+  }
+  return chain_dev(ctx, a, as, win, ex, dc, results_all, stream_v, hr, mp, pl);
+}
+}  // namespace
+
+extern "C" int fq_replan_pairs_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_result* results_all, void* stream_v)
+{
+  return shared_dev(ctx, a, results_all, stream_v);
+}
+
+extern "C" int fq_replan_pairs_plan_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
+                                        const fq_pair_exact* ex, const fq_pair_decomp* dc, const fq_pair_hr* hr, const fq_pair_map* mp,
+                                        const fq_pair_plan* pl, fq_pair_result* results_all, void* stream_v)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (int rc = check_plan(ctx, pl)) return rc;
+  return family_dev(ctx, a, as, win, ex, dc, hr, mp, pl, results_all, stream_v);
 }
 
 extern "C" int fq_replan_pairs_assign_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, fq_pair_result* results_all,
@@ -767,7 +825,7 @@ int check_host(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, con
 // copy_results = false leaves the caller's `results` untouched (the sharded chain reads the all-gathered table instead).
 int submit_host(fq_ctx* ctx, const Checked& k, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results,
                 const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex, const fq_pair_decomp* dc,
-                const fq_pair_hr* hr, const fq_pair_map* mp)
+                const fq_pair_hr* hr, const fq_pair_map* mp, const fq_pair_plan* pl = nullptr)
 {
   const int P = a->n_prob, n_unk = k.n_unk;
   const Sweep* sw = k.sw;
@@ -783,6 +841,7 @@ int submit_host(fq_ctx* ctx, const Checked& k, const fq_pair_args* a, bool defer
   fq_pair_decomp dd = dc ? *dc : fq_pair_decomp{};
   fq_pair_hr dh = hr ? *hr : fq_pair_hr{};
   fq_pair_map dm = mp ? *mp : fq_pair_map{};
+  fq_pair_plan dp = pl ? *pl : fq_pair_plan{};
   if (as) da.all_limit = as->all_limit;
   Sweep dv[2];
   char *hi = nullptr, *din = nullptr, *dout = nullptr;
@@ -825,6 +884,11 @@ int submit_host(fq_ctx* ctx, const Checked& k, const fq_pair_args* a, bool defer
       dh.last_factor_safe = in(hr->last_factor_safe, P);
       dh.index_H = out(hr->index_H, P);  dh.need_safe = out(hr->need_safe, P);
     }
+    if (pl)
+    {
+      dp.states = out(pl->states, 12 * (size_t)pl->cap_states);
+      dp.plan_ofs = out(pl->plan_ofs, P + 1);  dp.status = out(pl->status, P);
+    }
     for (int i = 0; i < 2; i++)
     {
       const Sweep& w = sw[i];
@@ -848,12 +912,8 @@ int submit_host(fq_ctx* ctx, const Checked& k, const fq_pair_args* a, bool defer
   cudaStream_t st = ctx->stream;
   FQ_CUDA(cudaMemcpyAsync(din, hi, in_bytes, cudaMemcpyHostToDevice, st));
   for (int i = 0; i < 2; i++) put_sweep(dv[i], i, &d, &da, &dw, &dx, &dd);
-  int rc = mp ? fq_replan_pairs_map_dev(ctx, &d, &da, win ? &dw : nullptr, ex ? &dx : nullptr, &dd, hr ? &dh : nullptr, &dm, nullptr, st)
-         : hr ? fq_replan_pairs_hr_dev(ctx, &d, &da, win ? &dw : nullptr, ex ? &dx : nullptr, &dd, &dh, nullptr, st)
-         : dc ? fq_replan_pairs_decomp_dev(ctx, &d, &da, win ? &dw : nullptr, ex ? &dx : nullptr, &dd, nullptr, st)
-         : ex ? fq_replan_pairs_exact_dev(ctx, &d, &da, win ? &dw : nullptr, &dx, nullptr, st)
-         : win ? fq_replan_pairs_window_dev(ctx, &d, &da, &dw, nullptr, st)
-         : as ? fq_replan_pairs_assign_dev(ctx, &d, &da, nullptr, st) : fq_replan_pairs_dev(ctx, &d, nullptr, st);
+  int rc = family_dev(ctx, &d, as ? &da : nullptr, win ? &dw : nullptr, ex ? &dx : nullptr, dc ? &dd : nullptr, hr ? &dh : nullptr,
+                      mp ? &dm : nullptr, pl ? &dp : nullptr, nullptr, st);
   if (rc) return rc;
   // ---- results straight into the caller's arrays (asynchronous when they are pinned).  The caller's window arrays were
   //      copied into the upload above, so the next_* outputs may alias them.
@@ -871,8 +931,26 @@ int submit_host(fq_ctx* ctx, const Checked& k, const fq_pair_args* a, bool defer
     if (hr->index_H) FQ_CUDA(cudaMemcpyAsync(hr->index_H, dh.index_H, sizeof(int) * P, cudaMemcpyDeviceToHost, st));
     if (hr->need_safe) FQ_CUDA(cudaMemcpyAsync(hr->need_safe, dh.need_safe, P, cudaMemcpyDeviceToHost, st));
   }
+  if (pl)
+  {
+    FQ_CUDA(cudaMemcpyAsync(pl->plan_ofs, dp.plan_ofs, sizeof(long long) * (size_t)(P + 1), cudaMemcpyDeviceToHost, st));
+    if (pl->status) FQ_CUDA(cudaMemcpyAsync(pl->status, dp.status, sizeof(int) * (size_t)P, cudaMemcpyDeviceToHost, st));
+    if (deferred && pl->cap_states > 0)      // the rows' total is not known yet: all cap_states rows
+      FQ_CUDA(cudaMemcpyAsync(pl->states, dp.states, sizeof(double) * 12 * (size_t)pl->cap_states, cudaMemcpyDeviceToHost, st));
+  }
   if (deferred) { ctx->pending = true; return 0; }
   FQ_CUDA(cudaStreamSynchronize(st));
+  if (pl)
+  { // only the rows of the corridors that fit: those before the first FQ_PLAN_CAPACITY corridor
+    long long rows = 0;
+    for (int j = 0; j <= P; j++)
+      if (pl->plan_ofs[j] <= pl->cap_states) rows = pl->plan_ofs[j];
+    if (rows > 0)
+    {
+      FQ_CUDA(cudaMemcpyAsync(pl->states, dp.states, sizeof(double) * 12 * (size_t)rows, cudaMemcpyDeviceToHost, st));
+      FQ_CUDA(cudaStreamSynchronize(st));
+    }
+  }
   return 0;
 }
 
@@ -880,13 +958,14 @@ int submit_host(fq_ctx* ctx, const Checked& k, const fq_pair_args* a, bool defer
 // arrays this one reads (a window's next_* passed on as the next init_* / final_*).
 int host_chain(fq_ctx* ctx, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results,
                const fq_pair_assign* as = nullptr, const fq_pair_window* win = nullptr, const fq_pair_exact* ex = nullptr,
-               const fq_pair_decomp* dc = nullptr, const fq_pair_hr* hr = nullptr, const fq_pair_map* mp = nullptr)
+               const fq_pair_decomp* dc = nullptr, const fq_pair_hr* hr = nullptr, const fq_pair_map* mp = nullptr,
+               const fq_pair_plan* pl = nullptr)
 {
   if (!ctx) return FQ_E_ARG;
   if (int rc = fq_settle(ctx)) return rc;
   Checked k;
   if (int rc = check_host(ctx, a, as, win, ex, dc, hr, mp, &k)) return rc;
-  return submit_host(ctx, k, a, deferred, d_results, copy_results, as, win, ex, dc, hr, mp);
+  return submit_host(ctx, k, a, deferred, d_results, copy_results, as, win, ex, dc, hr, mp, pl);
 }
 
 // checked sweep w cut to the corridors [lo, hi) (ofs: its candidate offsets, empty with a shared list): corridor offsets
@@ -1021,15 +1100,45 @@ namespace
 // exchange besides the records'.
 int lists_host(fq_ctx* ctx, const fq_pair_args* a, bool deferred, const fq_pair_assign* as, const fq_pair_window* win,
                const fq_pair_exact* ex = nullptr, const fq_pair_decomp* dc = nullptr, const fq_pair_hr* hr = nullptr,
-               const fq_pair_map* mp = nullptr)
+               const fq_pair_map* mp = nullptr, const fq_pair_plan* pl = nullptr)
 {
   if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
   if ((ex || dc) && (ctx->is_group || ctx->comm))
     return fq_fail(ctx, FQ_E_ARG, "fq_replan_pairs_exact / _decomp / _hr / _map: multi-GPU contexts are not supported (use the _dev entry)");
   if (ctx->is_group || ctx->comm) return sharded_chain(ctx, a, deferred, as, win);
-  return host_chain(ctx, a, deferred, nullptr, true, as, win, ex, dc, hr, mp);
+  return host_chain(ctx, a, deferred, nullptr, true, as, win, ex, dc, hr, mp, pl);
+}
+
+// fq_replan_pairs_plan / _async: the plan's refusals (multi-GPU contexts among them, so nothing here is sharded), then the
+// host entry of the family the structs select, with its own checks in its own order
+int plan_host(fq_ctx* ctx, const fq_pair_args* a, bool deferred, const fq_pair_assign* as, const fq_pair_window* win,
+              const fq_pair_exact* ex, const fq_pair_decomp* dc, const fq_pair_hr* hr, const fq_pair_map* mp, const fq_pair_plan* pl)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (int rc = check_plan(ctx, pl)) return rc;
+  if (!as)
+  {
+    if (win || ex || dc || hr || mp) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
+    return host_chain(ctx, a, deferred, nullptr, true, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, pl);
+  }
+  if (hr && !mp)
+    if (int rc = check_hr(ctx, win, dc, hr)) return rc;
+  return lists_host(ctx, a, deferred, as, win, ex, dc, hr, mp, pl);
 }
 }  // namespace
+
+extern "C" int fq_replan_pairs_plan(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
+                                    const fq_pair_exact* ex, const fq_pair_decomp* dc, const fq_pair_hr* hr, const fq_pair_map* mp,
+                                    const fq_pair_plan* pl)
+{
+  return plan_host(ctx, a, false, as, win, ex, dc, hr, mp, pl);
+}
+extern "C" int fq_replan_pairs_plan_async(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
+                                          const fq_pair_exact* ex, const fq_pair_decomp* dc, const fq_pair_hr* hr,
+                                          const fq_pair_map* mp, const fq_pair_plan* pl)
+{
+  return plan_host(ctx, a, true, as, win, ex, dc, hr, mp, pl);
+}
 
 extern "C" int fq_replan_pairs_assign(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as)
 {

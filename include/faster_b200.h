@@ -48,7 +48,7 @@ typedef struct fq_ctx fq_ctx;     /* opaque: device, stream, plan tables, scratc
 int fq_abi_version(void);
 /* 1 if this build has the named feature: "sweep_early_exit", "replan_pairs", "multi_gpu", "row_tol", "certificates",
  * "replan_pairs_assign", "replan_pairs_window", "replan_pairs_exact", "replan_pairs_decomp", "replan_pairs_hr",
- * "replan_pairs_map". */
+ * "replan_pairs_map", "replan_pairs_plan". */
 int fq_has_feature(const char* name);
 
 /* Threading: a context is used from one thread at a time, like a SolverGurobi instance in the reference (one replan
@@ -302,7 +302,8 @@ int fq_replan_pairs_assign_dev(fq_ctx* ctx, const fq_pair_args* args, const fq_p
  *                after a whole sweep without winner; an emptied sweep of the _dev variant)
  *   next_*[j]    the window of the next replan: if both sweeps won, max(f*_w - gamma_whole, 1.0) and f*_w + gammap_whole
  *                (and likewise for safe); otherwise the input window unchanged, since replan() returns before its update
- *                (faster.cpp:420-424, :529-533).  appendToPlan's early return (:548) is planner state and not modelled.
+ *                (faster.cpp:420-424, :529-533).  appendToPlan's early return (:548) depends on the planner's plan_ deque
+ *                and is not modelled; the states appendToPlan pushes are (fq_replan_pairs_plan below).
  * fq_pair_args is used as for fq_replan_pairs_assign except that factors_* must be NULL and n_fac_* 0 (FQ_E_ARG otherwise);
  * `assign` is required.  Feature "replan_pairs_window". */
 typedef struct fq_pair_window
@@ -578,6 +579,63 @@ int fq_replan_pairs_map_async(fq_ctx* ctx, const fq_pair_args* args, const fq_pa
 int fq_replan_pairs_map_dev(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
                             const fq_pair_exact* exact, const fq_pair_decomp* decomp, const fq_pair_hr* hr, const fq_pair_map* map,
                             fq_pair_result* results_all, void* stream);
+
+/* ---- chained replan that returns each corridor's committed plan --------------------------------------------------------
+ *
+ * What a replan commits is not its coefficients but the states appendToPlan pushes onto the plan (faster.cpp:548,
+ * :606-648): the whole winner's fillX samples X_temp_[0 .. k_safe] followed by every sample of the safe winner.  The entry
+ * points below run one of the chains above and also return that piece for every corridor, sampled on the device.  Feature
+ * "replan_pairs_plan".
+ *
+ * The chain is chosen by the structs given, with the rules of its own family: assign == NULL is fq_replan_pairs (window,
+ * exact, decomp, hr and map must then be NULL); otherwise map != NULL is _map, hr != NULL _hr, decomp != NULL _decomp,
+ * exact != NULL _exact, window != NULL _window, else _assign.  Every output other than the plan is byte for byte that
+ * family's, and every refusal of that family is refused alike (FQ_E_ARG, same fq_last_error text).
+ *
+ * Per corridor j, with n_w = n_samples_whole and n_s = max(2, (int)(N_safe safe_dt / DC)) (resetX's count):
+ *   the replan succeeds when it has a whole winner and, unless no safe path is needed (need_safe = 0, only with hr), a
+ *   safe winner; otherwise status FQ_PLAN_NONE and no rows (faster.cpp:420-424, :529-533);
+ *   piece = whole samples 0 .. k_safe, then safe samples 0 .. n_s - 1 (none when no safe path is needed, where k_safe =
+ *   n_w - 1): k_safe + 1 + n_s rows of 12 doubles, pos vel accel jerk, the layout of fq_fill_x;
+ *   every row is bit-equal to fq_fill_x(N, coeffs_*[j], dt, DC, n, .) called with the FULL count n (n_w or n_s) on the
+ *   coefficients the call returns in coeffs_* (for _exact after its fallback).  So whole row k_safe keeps its velocity
+ *   unless k_safe = n_w - 1, its first 9 doubles are the record's R bit for bit, and the last safe row is at rest.
+ * coeffs_* may be NULL: the chain keeps the winners' coefficients in its own scratch.
+ *
+ * Capacity: n_s depends on R, so the caller cannot size the plan in advance.  plan_ofs[0 .. n_prob] is the exclusive scan
+ * of every succeeding corridor's rows (64 bits), and plan_ofs[n_prob] is the capacity the whole batch needs.  A corridor
+ * whose rows would end past cap_states gets FQ_PLAN_CAPACITY and none of its rows are written; those corridors are the
+ * succeeding corridors of a suffix of the batch.  Nothing is written past cap_states rows, and the call still returns 0.
+ * Refused (FQ_E_ARG) besides the family's refusals: plan NULL, states or plan_ofs NULL, cap_states < 0, and multi-GPU
+ * contexts (group or rank): gathering variable-length plans would need a second exchange besides the records'. */
+#define FQ_PLAN_OK 0
+#define FQ_PLAN_NONE 1      /* the replan appends nothing (above)                                                   */
+#define FQ_PLAN_CAPACITY 2  /* the piece does not fit in cap_states rows                                            */
+typedef struct fq_pair_plan
+{
+  long long cap_states;     /* rows of `states`                                                                     */
+  double* states;           /* out: cap_states x 12                                                                 */
+  long long* plan_ofs;      /* out: n_prob + 1; corridor j is rows plan_ofs[j] .. plan_ofs[j+1]-1                   */
+  int* status;              /* out: n_prob (FQ_PLAN_*), or NULL                                                     */
+} fq_pair_plan;
+
+/* HOST pointers everywhere; blocks until every output is in the caller's arrays.  Of `states` only the rows of the
+ * corridors that fit are copied back (at most min(plan_ofs[n_prob], cap_states)); the rest of the array is untouched. */
+int fq_replan_pairs_plan(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
+                         const fq_pair_exact* exact, const fq_pair_decomp* decomp, const fq_pair_hr* hr, const fq_pair_map* map,
+                         const fq_pair_plan* plan);
+/* The same, returning once everything is enqueued; outputs are valid after fq_wait(ctx).  Arrays must stay alive.  The
+ * plan_ofs total is not known when the copies are enqueued, so all cap_states rows of `states` are copied back; rows past
+ * plan_ofs[n_prob] hold whatever the library's staging buffer held. */
+int fq_replan_pairs_plan_async(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
+                               const fq_pair_exact* exact, const fq_pair_decomp* decomp, const fq_pair_hr* hr, const fq_pair_map* map,
+                               const fq_pair_plan* plan);
+/* DEVICE pointers everywhere (the structs live on the host; plan's arrays are device arrays), with the hint rules of the
+ * selected family's _dev entry.  Never synchronises: the offsets and the rows are computed on the device after the
+ * records, so a CUDA graph can capture the call. */
+int fq_replan_pairs_plan_dev(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
+                             const fq_pair_exact* exact, const fq_pair_decomp* decomp, const fq_pair_hr* hr, const fq_pair_map* map,
+                             const fq_pair_plan* plan, fq_pair_result* results_all, void* stream);
 
 /* ---- several GPUs behind the boundary (SURVEY.md 8b/8e) ---------------------------------------------------------
  *
