@@ -148,7 +148,6 @@ __global__ void __launch_bounds__(W * 32, (N_ <= 10 ? 4 : (N_ <= 15 ? 3 : 2))) f
   const unsigned char* closed_row = b.keep_ties && b.closed ? b.closed + (size_t)c * b.n_dt : nullptr;
 
   WarpState<D> m;
-  int* seg_ofs;
   {
     double* p = reinterpret_cast<double*>(wraw + (size_t)warp * pwb);
     m.J = p;   p += NW * LD;
@@ -158,7 +157,6 @@ __global__ void __launch_bounds__(W * 32, (N_ <= 10 ? 4 : (N_ <= 15 ? 3 : 2))) f
     m.d = p;   p += NW + 2;
     m.zb = p;  p += NW;
     m.items = reinterpret_cast<unsigned short*>(p);
-    seg_ofs = sfo + 40 + warp * 32;
   }
   const long long n_child = (long long)n_par * P;
   for (long long child = (long long)sub * W + warp; child < n_child; child += (long long)b.cpc * W)
@@ -224,7 +222,7 @@ __global__ void __launch_bounds__(W * 32, (N_ <= 10 ? 4 : (N_ <= 15 ? 3 : 2))) f
 #pragma unroll
       for (int t = 1; t < 16; t++)
         if (lane == t && t <= k) p = sig[t];
-      total_rows = build_items<D>(m, sfo, seg_ofs, lane, k + 1, p, a.item_cap);
+      total_rows = build_items<D>(m, sfo, lane, k + 1, p, a.item_cap);
       if (total_rows < 0) { if (lane == 0) flg[0] = 1; continue; }
     }
     int it = 0, bkey = 0;

@@ -53,6 +53,19 @@ struct Dims
 template <class D>
 __host__ __device__ inline int per_warp_bytes(int item_cap) { return D::PER_WARP_DOUBLES * 8 + ((item_cap * 2 + 15) & ~15); }
 
+// -DFQ_PHASE_CLOCKS (measurement builds only, tools/phase_clocks.py): clock64() stamps at the ends of the phases of one
+// candidate's solve, accumulated per (mode, outcome) into fq_phase_clk[replica][whole][settled] = 7 phase totals and a
+// count.  Stamp 0 is taken before the claim, stamp k (1..6) ends phase k-1, the return from solve_candidate ends phase 6:
+// claim and input loads, setup_rows and the guards, the segment-0 check, build_items, the first scan (with w = 0 and
+// update_Y), the iterations, the outputs.  Stamp 8 holds the outcome: settled at w = 0 means optimal with no iteration or
+// infeasible at the first entering row.  32 replicas (by CTA) keep the atomics from queueing on one address.
+#ifdef FQ_PHASE_CLOCKS
+#define FQ_STAMP(clk, k) do { if (clk) (clk)[k] = clock64(); } while (0)
+static __device__ unsigned long long fq_phase_clk[32][2][2][8];
+#else
+#define FQ_STAMP(clk, k) do { } while (0)
+#endif
+
 __device__ __forceinline__ double fast_rcp(double x)
 {
   double r;
@@ -303,10 +316,11 @@ __device__ __forceinline__ void setup_rows(const FqKernelArgs& a, int prob, doub
 }
 
 // Corridor item list of the first n_seg segments: item = t << 12 | need_cp0 << 11 | face (row of the staged Ab).
-// `p` = polytope of segment `lane` (meaningful for lane < n_seg).  Returns the number of items.
+// `p` = polytope of segment `lane` (meaningful for lane < n_seg).  Returns the number of items; the caller's next
+// __syncwarp publishes them to the warp.
 template <class D>
-__device__ __forceinline__ int build_items(const WarpState<D>& m, const int* __restrict__ sfo, int* __restrict__ seg_ofs,
-                                           int lane, int n_seg, int p, int item_cap)
+__device__ __forceinline__ int build_items(const WarpState<D>& m, const int* __restrict__ sfo, int lane, int n_seg, int p,
+                                           int item_cap)
 {
   int F = 0;
   if (lane < n_seg) F = sfo[p + 1] - sfo[p];
@@ -321,19 +335,14 @@ __device__ __forceinline__ int build_items(const WarpState<D>& m, const int* __r
   }
   const int total_rows = __shfl_sync(FULL, incl, n_seg - 1);
   if (total_rows > item_cap) return -1;     // a wrong max_faces_per_polytope hint (device-pointer entry): refuse, never overrun
-  // seg_ofs[t] = first item of segment t; seg_ofs[16 + t] = (need_cp0 << 11) | first staged face of sigma[t]
-  if (lane < n_seg) { seg_ofs[lane] = incl - F; seg_ofs[16 + lane] = (need0 << 11) | sfo[p]; }
-  else if (lane < 16) seg_ofs[lane] = 0x7fffffff;
-  __syncwarp();
-  // item_cap >= N * (faces of the largest polytope) >= total_rows by construction (host side)
-  for (int i = lane; i < total_rows; i += 32)
+  // lane t writes segment t's items, in face order from its first item: independent stores, where a search of every item's
+  // segment would chain dependent shared-memory loads.  item_cap >= N * (faces of the largest polytope) >= total_rows by
+  // construction (host side)
+  if (lane < n_seg)
   {
-    int t = 0;                                   // largest t with seg_ofs[t] <= i  (N <= 16: 4 halving steps)
-#pragma unroll
-    for (int step = 8; step; step >>= 1)
-      if (seg_ofs[t + step] <= i) t += step;
-    const int meta = seg_ofs[16 + t];
-    m.items[i] = (unsigned short)((t << 12) | (meta + (i - seg_ofs[t])));
+    unsigned short* dst = m.items + (incl - F);
+    const int meta = (lane << 12) | (need0 << 11) | sfo[p];
+    for (int k = 0; k < F; k++) dst[k] = (unsigned short)(meta + k);
   }
   return total_rows;
 }
@@ -354,7 +363,7 @@ __device__ __forceinline__ int gi_loop(const WarpState<D>& m, const double* __re
                                        double inv3, double lim0, double lim1, double lim2, double row_tol,
                                        double (&lam)[D::SLOTS], double (&rdinv)[D::SLOTS], int& q, int& it, int bkey,
                                        unsigned bcode, const double* __restrict__ dtp = nullptr,
-                                       const double* __restrict__ lim = nullptr)
+                                       const double* __restrict__ lim = nullptr, long long* clk = nullptr)
 {
   constexpr int N = D::N, NZ = D::NZ, NW = D::NW, NYP = D::NYP, LD = D::LD, SLOTS = D::SLOTS;
   double r[SLOTS], z[SLOTS], dreg[SLOTS];
@@ -382,6 +391,9 @@ __device__ __forceinline__ int gi_loop(const WarpState<D>& m, const double* __re
       if (km > bkey) { bkey = km; bcode = (unsigned)i; }
     }
     const int mk = __reduce_max_sync(FULL, bkey);
+#ifdef FQ_PHASE_CLOCKS
+    if (clk && clk[5] == 0) clk[5] = clock64();
+#endif
     if (mk <= 0) { status = 1; break; }
     const int key = bkey;
     const int src = __ffs(__ballot_sync(FULL, key == mk)) - 1;
@@ -638,8 +650,8 @@ __device__ __forceinline__ int gi_loop(const WarpState<D>& m, const double* __re
 template <class D>
 __device__ void solve_candidate(const FqKernelArgs& a, const double* __restrict__ TZ,
                                 const double* __restrict__ SY, const double* __restrict__ sAb,
-                                const int* __restrict__ sfo, const WarpState<D>& m, int* __restrict__ seg_ofs,
-                                int prob, int cand, int lane, int rows_bad)
+                                const int* __restrict__ sfo, const WarpState<D>& m,
+                                int prob, int cand, int lane, int rows_bad, long long* clk = nullptr)
 {
   constexpr int N = D::N, NW = D::NW, NYP = D::NYP, SLOTS = D::SLOTS;
   // N <= 10: 4 CTAs per SM at 128 registers, the whole register file.  These instances keep nothing through the
@@ -649,6 +661,7 @@ __device__ void solve_candidate(const FqKernelArgs& a, const double* __restrict_
   const double inv1 = 1.0 / dt, inv2 = inv1 * inv1, inv3 = inv2 * inv1;
   const double lim0 = a.lim[prob * 3 + 0], lim1 = a.lim[prob * 3 + 1], lim2 = a.lim[prob * 3 + 2];
   const int P = a.poly_ofs[prob + 1] - a.poly_ofs[prob];
+  FQ_STAMP(clk, 1);
 
   // ---- per-lane constants of the owned rows: Yeq, box scale and limit
   double Yeq[D::RPL][3], bthr[D::RPL];
@@ -662,6 +675,7 @@ __device__ void solve_candidate(const FqKernelArgs& a, const double* __restrict_
     for (int r = 0; r < D::RPL; r++)
 #pragma unroll
       for (int ax = 0; ax < 3; ax++) okc = okc && fabs(Yeq[r][ax]) < 1e300;
+    FQ_STAMP(clk, 2);
     if (!__all_sync(FULL, okc))
     {
       if (lane == 0)
@@ -706,8 +720,12 @@ __device__ void solve_candidate(const FqKernelArgs& a, const double* __restrict_
           for (int k = 0; k < 3; k++)
             out = out || rank_key(fma(a01.x, c[k][0], fma(a01.y, c[k][1], fma(a23.x, c[k][2], -a23.y))) * 1e15) > 0;
         }
+        FQ_STAMP(clk, 3);
         if (__any_sync(FULL, out))
         {
+#ifdef FQ_PHASE_CLOCKS
+          if (clk) clk[8] = 1;
+#endif
           if (lane == 0)
           {
             a.feasible[cand] = 0;
@@ -720,7 +738,9 @@ __device__ void solve_candidate(const FqKernelArgs& a, const double* __restrict_
         }
       }
     }
-    total_rows = build_items<D>(m, sfo, seg_ofs, lane, N, p, a.item_cap);
+    FQ_STAMP(clk, 3);
+    total_rows = build_items<D>(m, sfo, lane, N, p, a.item_cap);
+    FQ_STAMP(clk, 4);
     if (total_rows < 0)
     { // the row list does not fit: report "not solved" (iters = -2 marks the cause)
       if (lane == 0)
@@ -751,7 +771,11 @@ __device__ void solve_candidate(const FqKernelArgs& a, const double* __restrict_
   unsigned bcode = 0;
   update_Y<D, true>(m, TZ, Yeq, bthr, SY, lane, bkey, bcode);
   const int status = gi_loop<D, LEAN>(m, TZ, SY, sAb, Yeq, bthr, lane, total_rows, inv1, inv2, inv3, lim0, lim1, lim2,
-                                      a.row_tol, lam, rdinv, q, it, bkey, bcode, a.dt + cand, a.lim + prob * 3);
+                                      a.row_tol, lam, rdinv, q, it, bkey, bcode, a.dt + cand, a.lim + prob * 3, clk);
+  FQ_STAMP(clk, 6);
+#ifdef FQ_PHASE_CLOCKS
+  if (clk) clk[8] = (status == 1 && it == 0) || (status == 0 && it == 1);
+#endif
 
   // ================= outputs =================
 #ifndef FQ_EMULATE_ON_HOST
@@ -869,7 +893,6 @@ __global__ void __launch_bounds__(W * 32, (N_ <= 10 ? (WHOLE_ ? FQ_MIN_CTAS_WHOL
   }
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   WarpState<D> m;
-  int* seg_ofs;
   {
     double* p = reinterpret_cast<double*>(wraw + (size_t)warp * pwb);
     m.J = p;   p += D::NW * D::LD;
@@ -879,8 +902,9 @@ __global__ void __launch_bounds__(W * 32, (N_ <= 10 ? (WHOLE_ ? FQ_MIN_CTAS_WHOL
     m.d = p;   p += D::NW + 2;
     m.zb = p;  p += D::NW;
     m.items = reinterpret_cast<unsigned short*>(p);
-    seg_ofs = sfo0 + 40 * W + warp * 32;
   }
+  // smem_bytes_t (and the branch-and-bound's level_smem) still count 32 ints per warp after the sfo tables, which nothing
+  // uses any more: left in, so that the shared-memory size limits of both kernels stay where they are
   __syncthreads();
   const int n_prob = a.n_prob;
   double* sAb = sAb0 + (size_t)warp * 4 * a.max_faces;
@@ -935,6 +959,12 @@ __global__ void __launch_bounds__(W * 32, (N_ <= 10 ? (WHOLE_ ? FQ_MIN_CTAS_WHOL
     const bool ee = a.first_feasible != nullptr;   // early exit: genNewTraj's "first feasible factor wins" (solverGurobi.cpp:445-446)
     while (c < count)
     {
+#ifdef FQ_PHASE_CLOCKS
+      long long clk[9] = {};
+      clk[0] = clock64();
+#else
+      long long* clk = nullptr;
+#endif
       int cn = 0;
       if (lane == 0) cn = atomicAdd(counters + prob, 1);
       // claims run from the end of the list (long solves first); with the early exit from its start (smallest dt first)
@@ -946,7 +976,22 @@ __global__ void __launch_bounds__(W * 32, (N_ <= 10 ? (WHOLE_ ? FQ_MIN_CTAS_WHOL
         const unsigned long long best = *reinterpret_cast<volatile unsigned long long*>(a.first_feasible + prob);
         skip = (unsigned long long)__double_as_longlong(a.dt[cand]) > best;   // a smaller dt already has a feasible candidate
       }
-      if (!skip) solve_candidate<D>(a, TZ, SY, sAb, sfo, m, seg_ofs, prob, cand, lane, rows_bad);
+      if (!skip)
+      {
+        solve_candidate<D>(a, TZ, SY, sAb, sfo, m, prob, cand, lane, rows_bad, clk);
+#ifdef FQ_PHASE_CLOCKS
+        const long long end = clock64();
+        if (lane == 0)
+        { // a phase an early exit skipped ends where the previous one did
+          unsigned long long* acc = fq_phase_clk[blockIdx.x & 31][WHOLE_ ? 1 : 0][clk[8] ? 1 : 0];
+          for (int k = 1; k <= 6; k++)
+            if (clk[k] == 0) clk[k] = clk[k - 1];
+          for (int k = 0; k < 6; k++) atomicAdd(acc + k, (unsigned long long)(clk[k + 1] - clk[k]));
+          atomicAdd(acc + 6, (unsigned long long)(end - clk[6]));
+          atomicAdd(acc + 7, 1ull);
+        }
+#endif
+      }
       else
       { // not evaluated: it cannot win.  Reported like an unsolved candidate, iters = -3 marks the reason.
         if (a.sorted_dt)
