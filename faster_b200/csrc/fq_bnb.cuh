@@ -70,7 +70,8 @@ struct BnbArgs
   int leaf_cap;
   int* flags;                      // n_prob x 2: [0] overflow of children/leaves or rows, [1] numeric failures
   long long* nodes;                // n_prob: nodes evaluated, summed over the levels, or nullptr
-  int keep_ties;                   // 0: prune at cost >= incumbent and keep strictly improving leaves only;
+  int keep_ties;                   // 0: prune at cost >= incumbent (> at the last level) and keep the leaves that
+                                   //    lower or equal it;
                                    // 1: prune at cost > incumbent (1 + 1e-9) and keep every leaf within that bound
   // keep_ties only (nullptr otherwise), n_prob x n_dt each.  lbound: the smallest relaxation cost of depth 0 (segment 0
   // fixed), a lower bound on every assignment of that time allocation.  closed: set after level 0 (fq_bnb_certify_kernel)
@@ -85,6 +86,9 @@ __global__ void __launch_bounds__(W * 32, (N_ <= 10 ? 4 : (N_ <= 15 ? 3 : 2))) f
 {
   using D = Dims<N_, WHOLE_>;
   constexpr int NW = D::NW, LD = D::LD, SLOTS = D::SLOTS, N = D::N, NYP = D::NYP;
+  // N <= 10: 4 CTAs per SM at 128 registers.  As in the solve kernel (fqt::solve_candidate), the box scales and limits are
+  // read or recomputed where they are needed, bit for bit, instead of held through the node solve
+  constexpr bool LEAN = N <= 10;
   const FqKernelArgs& a = b.k;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   double* sm = reinterpret_cast<double*>(smem_raw);
@@ -142,7 +146,6 @@ __global__ void __launch_bounds__(W * 32, (N_ <= 10 ? 4 : (N_ <= 15 ? 3 : 2))) f
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const size_t slice = (size_t)c * b.cap;
   const int k = b.depth;
-  const double lim0 = a.lim[3 * c], lim1 = a.lim[3 * c + 1], lim2 = a.lim[3 * c + 2];
   unsigned long long* inc_row = b.incumbent + (size_t)c * b.n_dt;
   unsigned long long* lb_row = b.keep_ties && b.lbound ? b.lbound + (size_t)c * b.n_dt : nullptr;
   const unsigned char* closed_row = b.keep_ties && b.closed ? b.closed + (size_t)c * b.n_dt : nullptr;
@@ -176,8 +179,10 @@ __global__ void __launch_bounds__(W * 32, (N_ <= 10 ? 4 : (N_ <= 15 ? 3 : 2))) f
     }
     sig[k] = (unsigned char)pnew;
     if (closed_row && closed_row[dt_idx]) continue;     // the list winner stands at this time allocation (fixed since level 0)
-    const double dt = b.dts[(size_t)c * b.n_dt + dt_idx];
+    const double* dtp = b.dts + (size_t)c * b.n_dt + dt_idx;
+    const double dt = *dtp;
     const double inv1 = 1.0 / dt, inv2 = inv1 * inv1, inv3 = inv2 * inv1;
+    const double lim0 = a.lim[3 * c], lim1 = a.lim[3 * c + 1], lim2 = a.lim[3 * c + 2];
     double Yeq[D::RPL][3], bthr[D::RPL];
     setup_rows<D>(a, c, dt, lim0, lim1, lim2, lane, Yeq, bthr);
     {
@@ -215,22 +220,22 @@ __global__ void __launch_bounds__(W * 32, (N_ <= 10 ? 4 : (N_ <= 15 ? 3 : 2))) f
     }
     __syncwarp();
     // ---- rows of segments 0..k
-    int total_rows = 0;
+    int run = 0;
     {
       int p = 0;
       if (lane <= k) p = sig[0];
 #pragma unroll
       for (int t = 1; t < 16; t++)
         if (lane == t && t <= k) p = sig[t];
-      total_rows = build_items<D>(m, sfo, lane, k + 1, p, a.item_cap);
-      if (total_rows < 0) { if (lane == 0) flg[0] = 1; continue; }
+      run = build_items<D>(m, sfo, lane, k + 1, p, a.item_cap);
+      if (run < 0) { if (lane == 0) flg[0] = 1; continue; }
     }
     int it = 0, bkey = 0;
     unsigned bcode = 0;
     if (k == 0) update_Y<D, true>(m, TZ, Yeq, bthr, SY, lane, bkey, bcode);
     else update_Y<D, false>(m, TZ, Yeq, bthr, SY, lane, bkey, bcode);
-    const int status = gi_loop<D>(m, TZ, SY, sAb, Yeq, bthr, lane, total_rows, inv1, inv2, inv3, lim0, lim1, lim2, a.row_tol,
-                                  lam, rdinv, q, it, bkey, bcode);
+    const int status = gi_loop<D, LEAN>(m, TZ, SY, sAb, Yeq, bthr, lane, run, inv1, inv2, inv3, lim0, lim1, lim2, a.row_tol,
+                                        lam, rdinv, q, it, bkey, bcode, dtp, a.lim + 3 * c);
     if (status != 1)
     {
       if (status == -1 && lane == 0) atomicAdd(flg + 1, 1);
@@ -243,18 +248,22 @@ __global__ void __launch_bounds__(W * 32, (N_ <= 10 ? 4 : (N_ <= 15 ? 3 : 2))) f
       const double u = m.Y[ax * NYP + 3 * N + 1 + t];
       cp = fma(u, u, cp);
     }
-    const double cost = fqt::warp_sum(cp) * (inv3 * inv3);
+    const double oinv1 = LEAN ? 1.0 / dt : inv1, oinv3 = LEAN ? oinv1 * oinv1 * oinv1 : inv3;
+    const double cost = fqt::warp_sum(cp) * (oinv3 * oinv3);
     const unsigned long long cbits = (unsigned long long)__double_as_longlong(cost);
     if (k == 0 && lb_row && lane == 0) atomicMin(lb_row + dt_idx, cbits);
     const unsigned long long inc = *reinterpret_cast<volatile unsigned long long*>(inc_row + dt_idx);
-    // bound: children only add rows, the cost cannot decrease
-    if (b.keep_ties ? !(cost <= __longlong_as_double((long long)inc) * (1.0 + 1e-9)) : cbits >= inc) continue;
+    // bound: children only add rows, the cost cannot decrease.  Without keep_ties a full assignment whose cost equals the
+    // incumbent's is kept as well: the sweep then chooses among equal-cost leaves by assignment, not by which warp finished
+    // first
+    if (b.keep_ties ? !(cost <= __longlong_as_double((long long)inc) * (1.0 + 1e-9)) : (k + 1 == N ? cbits > inc : cbits >= inc))
+      continue;
     if (k + 1 == N)
-    { // a full assignment that beats (or, keeping ties, comes within 1e-9 of) the incumbent
+    { // a full assignment that beats or equals (or, keeping ties, comes within 1e-9 of) the incumbent
       if (lane == 0)
       {
         const unsigned long long old = atomicMin(inc_row + dt_idx, cbits);
-        if (b.keep_ties || cbits < old)
+        if (b.keep_ties || cbits <= old)
         {
           const int slot = atomicAdd(b.n_leaves + c, 1);
           if (slot < b.leaf_cap)

@@ -891,8 +891,15 @@ extern "C" int fq_gen_new_traj_exact(fq_ctx* ctx, int N, int force_final, const 
         if (!(c < INFINITY)) continue;
         win_dt = d;
         bool from_leaf = false;
-        for (int i = 0; i < n_leaves; i++)                         // the last improving leaf of this dt holds the incumbent
-          if (leaves[i].dt_idx == d && leaves[i].cost == c) { std::memcpy(win_sigma.data(), leaves[i].sigma, N); from_leaf = true; }
+        // the list winner stands where the tree found nothing cheaper; otherwise the lowest assignment among the leaves that
+        // hold the incumbent (several can, with costs equal to the bit)
+        const bool list_stands = best_k[d] >= 0 && c == best[d];
+        for (int i = 0; i < n_leaves && !list_stands; i++)
+          if (leaves[i].dt_idx == d && leaves[i].cost == c && (!from_leaf || std::memcmp(leaves[i].sigma, win_sigma.data(), N) < 0))
+          {
+            std::memcpy(win_sigma.data(), leaves[i].sigma, N);
+            from_leaf = true;
+          }
         if (!from_leaf) std::memcpy(win_sigma.data(), &mono[(size_t)best_k[d] * N], N);
       }
     }

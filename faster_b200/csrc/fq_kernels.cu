@@ -816,17 +816,18 @@ cudaError_t fq_launch_map_table(const FqMapTableChunk& c, cudaStream_t stream)
 
 #ifdef FQ_PHASE_CLOCKS
 // measurement builds (tools/phase_clocks.py): fqt::fq_phase_clk of the current device summed over its replicas into
-// out[whole][settled][8] (seven phase totals in clock cycles, then the candidate count); reset != 0 zeroes it afterwards
+// out[whole][settled][9] (seven phase totals in clock cycles, the candidate count, then the corridor-scan total); reset != 0
+// zeroes it afterwards
 extern "C" int fq_phase_clocks(unsigned long long* out, int reset)
 {
-  static unsigned long long h[32][2][2][8];
+  static unsigned long long h[32][2][2][9];
   if (cudaDeviceSynchronize() != cudaSuccess || cudaMemcpyFromSymbol(h, fqt::fq_phase_clk, sizeof(h)) != cudaSuccess) return -1;
-  for (int k = 0; k < 32; k++) out[k] = 0;
+  for (int k = 0; k < 36; k++) out[k] = 0;
   for (int i = 0; i < 32; i++)
-    for (int k = 0; k < 32; k++) out[k] += (&h[i][0][0][0])[k];
+    for (int k = 0; k < 36; k++) out[k] += (&h[i][0][0][0])[k];
   if (reset)
   {
-    static const unsigned long long z[32][2][2][8] = {};
+    static const unsigned long long z[32][2][2][9] = {};
     if (cudaMemcpyToSymbol(fqt::fq_phase_clk, z, sizeof(z)) != cudaSuccess) return -1;
   }
   return 0;

@@ -5,11 +5,13 @@
 //   * every lane OWNS fixed rows of Y (row y = lane + 32 r, all three axes): the plan's constant part Yeq stays in
 //     registers, Y = Yeq + TZ w costs one broadcast read of w per column, and the |v|,|a|,|j| box rows
 //     (solverGurobi.cpp:390-407) are ranked by the owning lane while the value is still in a register;
-//   * corridor rows (solverGurobi.cpp:249-287) are scanned through a per-candidate item list (segment, face), 32 rows
-//     per pass; the control point shared with the previous segment is skipped when both segments use the same polytope;
+//   * corridor rows (solverGurobi.cpp:249-287) are scanned through a per-candidate item list (segment, face), each lane
+//     taking a run of faces of one segment whose control points it reads once; the control point shared with the
+//     previous segment is skipped when both segments use the same polytope;
 //   * the entering row is the one farthest beyond its hyperplane in w-space: rank = (violation - tol) / |TZ[y]|, compared
-//     through the hi word of that double as a signed int (positive <=> violated), so the warp arg-max is one redux.sync
-//     plus a ballot.  This "normalised pivoting" halves the iteration count relative to "largest violation";
+//     through the hi word of that double as a signed int (positive <=> violated), so the warp arg-max is one redux.sync,
+//     and a second one on a tie code picks among equal keys.  This "normalised pivoting" halves the iteration count
+//     relative to "largest violation";
 //   * THIN factorisation: only J1 (NW x q, an orthonormal basis of the active normals, N = J1 R) is kept instead of the
 //     full orthogonal J of the generic kernel.  The projection of a row normal g is z = -(g - J1 J1' g) (q columns, not
 //     NW - q), a new active row appends one column -z/|z| (Gram-Schmidt, with one re-orthogonalisation pass when
@@ -54,14 +56,16 @@ template <class D>
 __host__ __device__ inline int per_warp_bytes(int item_cap) { return D::PER_WARP_DOUBLES * 8 + ((item_cap * 2 + 15) & ~15); }
 
 // -DFQ_PHASE_CLOCKS (measurement builds only, tools/phase_clocks.py): clock64() stamps at the ends of the phases of one
-// candidate's solve, accumulated per (mode, outcome) into fq_phase_clk[replica][whole][settled] = 7 phase totals and a
-// count.  Stamp 0 is taken before the claim, stamp k (1..6) ends phase k-1, the return from solve_candidate ends phase 6:
-// claim and input loads, setup_rows and the guards, the segment-0 check, build_items, the first scan (with w = 0 and
-// update_Y), the iterations, the outputs.  Stamp 8 holds the outcome: settled at w = 0 means optimal with no iteration or
-// infeasible at the first entering row.  32 replicas (by CTA) keep the atomics from queueing on one address.
+// candidate's solve, accumulated per (mode, outcome) into fq_phase_clk[replica][whole][settled] = 7 phase totals, a
+// count and the corridor-scan total.  Stamp 0 is taken before the claim, stamp k (1..6) ends phase k-1, the return from
+// solve_candidate ends phase 6: claim and input loads, setup_rows and the guards, the segment-0 check, build_items, the
+// first scan (with w = 0 and update_Y), the iterations, the outputs.  Stamp 8 holds the outcome: settled at w = 0 means
+// optimal with no iteration or infeasible at the first entering row.  Slot 9 sums the cycles of every corridor-row scan of
+// gi_loop (the first one and those of the iterations, up to the warp's choice of the entering row): a part of phases 4
+// and 5, not a phase of its own.  32 replicas (by CTA) keep the atomics from queueing on one address.
 #ifdef FQ_PHASE_CLOCKS
 #define FQ_STAMP(clk, k) do { if (clk) (clk)[k] = clock64(); } while (0)
-static __device__ unsigned long long fq_phase_clk[32][2][2][8];
+static __device__ unsigned long long fq_phase_clk[32][2][2][9];
 #else
 #define FQ_STAMP(clk, k) do { } while (0)
 #endif
@@ -315,9 +319,12 @@ __device__ __forceinline__ void setup_rows(const FqKernelArgs& a, int prob, doub
   }
 }
 
-// Corridor item list of the first n_seg segments: item = t << 12 | need_cp0 << 11 | face (row of the staged Ab).
-// `p` = polytope of segment `lane` (meaningful for lane < n_seg).  Returns the number of items; the caller's next
-// __syncwarp publishes them to the warp.
+// Corridor item list of the first n_seg segments: item = t << 12 | need_cp0 << 11 | face (row of the staged Ab), segment
+// by segment, in face order within a segment.  `p` = polytope of segment `lane` (meaningful for lane < n_seg).
+// The scan of gi_loop gives every lane one RUN of consecutive items of ONE segment, so that the lane reads the segment's
+// control points once per scan and then only the face rows: each segment is shared by 32 / n_seg lanes in equal runs.
+// Returns this lane's run, count << 20 | first item (count 0: no run), or -1 when the list does not fit item_cap (the
+// same for every lane); the caller's next __syncwarp publishes the items to the warp.
 template <class D>
 __device__ __forceinline__ int build_items(const WarpState<D>& m, const int* __restrict__ sfo, int lane, int n_seg, int p,
                                            int item_cap)
@@ -344,14 +351,21 @@ __device__ __forceinline__ int build_items(const WarpState<D>& m, const int* __r
     const int meta = (lane << 12) | (need0 << 11) | sfo[p];
     for (int k = 0; k < F; k++) dst[k] = (unsigned short)(meta + k);
   }
-  return total_rows;
+  // ---- runs: G = 32 / n_seg lanes per segment (a constant in the solve kernels); lane l takes run l % G of segment l / G,
+  //      ceil(F / G) items long.  Lanes past G * n_seg fall on a segment beyond n_seg (F = 0) and get no items
+  const int G = 32 / n_seg;
+  const int s = lane / G, k = lane - s * G;
+  const int fs = __shfl_sync(FULL, F, s), f0 = __shfl_sync(FULL, incl - F, s);
+  const int len = (fs + G - 1) / G;
+  const int cnt = max(0, min(len, fs - k * len));
+  return (cnt << 20) | (cnt > 0 ? f0 + k * len : 0);
 }
 
 // The dual active-set iteration: from the current state (w, J, R in shared; lam, rdinv, q in registers; Y and the lane's
 // rank key/code already evaluated for the current w) run until no enabled row is violated (returns 1), a violated row
-// cannot be reached (0) or the iteration cap / a NaN is hit (-1).  Enabled rows = box rows + the `total_rows` items of
-// m.items.  Used by the fixed-assignment solve below and by the branch-and-bound node solve (fq_bnb.cuh), which enters
-// with a parent's factorisation instead of the identity.
+// cannot be reached (0) or the iteration cap / a NaN is hit (-1).  Enabled rows = box rows + the items of m.items, which
+// the lanes scan in the runs build_items gave them (`run`: this lane's).  Used by the fixed-assignment solve below and by
+// the branch-and-bound node solve (fq_bnb.cuh), which enters with a parent's factorisation instead of the identity.
 // A box row's scale 1/dt^k (inv1..3) and limit (lim0..2) are held in registers through the iteration, except with
 // BOX_AT_ENTRY: then they are read through `dtp` (the time allocation dt) and `lim` (the problem's three limits) and
 // recomputed, bit for bit, where such a row enters.  That frees twelve registers in the N <= 10 solve kernels, which fill
@@ -359,7 +373,7 @@ __device__ __forceinline__ int build_items(const WarpState<D>& m, const int* __r
 template <class D, bool BOX_AT_ENTRY = false>
 __device__ __forceinline__ int gi_loop(const WarpState<D>& m, const double* __restrict__ TZ, const double* __restrict__ SY,
                                        const double* __restrict__ sAb, const double (&Yeq)[D::RPL][3],
-                                       const double (&bthr)[D::RPL], int lane, int total_rows, double inv1, double inv2,
+                                       const double (&bthr)[D::RPL], int lane, int run, double inv1, double inv2,
                                        double inv3, double lim0, double lim1, double lim2, double row_tol,
                                        double (&lam)[D::SLOTS], double (&rdinv)[D::SLOTS], int& q, int& it, int bkey,
                                        unsigned bcode, const double* __restrict__ dtp = nullptr,
@@ -373,31 +387,60 @@ __device__ __forceinline__ int gi_loop(const WarpState<D>& m, const double* __re
   while (status == -2)
   {
     // ================= most violated corridor row (box rows were checked by update_Y) =================
-#pragma unroll 1
-    for (int i = lane; i < total_rows; i += 32)
+#ifdef FQ_PHASE_CLOCKS
+    const long long scan0 = clock64();
+#endif
+    // The lane scans its run (build_items): items i0 .. i0 + cnt - 1, faces gf0 .. of ONE segment t, whose control points
+    // are read once.  Ties of the rank key are broken as a lane-strided scan (item i on lane i & 31 in pass i >> 5) breaks
+    // them, by a tie code per candidate row: box rows of lane L (bkey/bcode, set by update_Y) L << 16, item i
+    // (i & 31) << 16 | (i >> 5) + 1.  The entering row is the one of largest key, and of smallest tie code among those: the
+    // lowest lane's, its box rows before its items, its earliest item -- the same row, so the same path, bit for bit.
+    int btie = lane << 16;
     {
-      const unsigned item = m.items[i];
-      const int t = item >> 12, gf = item & 0x7ff;
-      const double2 a01 = row_a01(sAb, gf);
-      const double2 a23 = row_a23(sAb, gf);                                         // a23.y = b + tol
-      const double* Y0 = m.Y; const double* Y1 = m.Y + NYP; const double* Y2 = m.Y + 2 * NYP;
-      const int y1 = 4 * N + 1 + t, y2 = 5 * N + 1 + t;
-      const double u1 = fma(a01.x, Y0[y1], fma(a01.y, Y1[y1], fma(a23.x, Y2[y1], -a23.y))) * SY[y1];
-      const double u2 = fma(a01.x, Y0[y2], fma(a01.y, Y1[y2], fma(a23.x, Y2[y2], -a23.y))) * SY[y2];
-      const double u3 = fma(a01.x, Y0[t + 1], fma(a01.y, Y1[t + 1], fma(a23.x, Y2[t + 1], -a23.y))) * SY[t + 1];
-      int km = max(max(rank_key(u1), rank_key(u2)), rank_key(u3));
-      if (item & 0x800u)
-        km = max(km, rank_key(fma(a01.x, Y0[t], fma(a01.y, Y1[t], fma(a23.x, Y2[t], -a23.y))) * SY[t]));
-      if (km > bkey) { bkey = km; bcode = (unsigned)i; }
+      const int cnt = run >> 20;
+      if (cnt > 0)
+      {
+        const int i0 = run & 0xfffff;
+        const unsigned item = m.items[i0];
+        const int t = item >> 12, gf0 = item & 0x7ff;
+        const bool need0 = (item & 0x800u) != 0;
+        const double* Y0 = m.Y; const double* Y1 = m.Y + NYP; const double* Y2 = m.Y + 2 * NYP;
+        const int y1 = 4 * N + 1 + t, y2 = 5 * N + 1 + t;
+        const double c10 = Y0[y1], c11 = Y1[y1], c12 = Y2[y1], s1 = SY[y1];
+        const double c20 = Y0[y2], c21 = Y1[y2], c22 = Y2[y2], s2 = SY[y2];
+        const double c30 = Y0[t + 1], c31 = Y1[t + 1], c32 = Y2[t + 1], s3 = SY[t + 1];
+        double c00 = 0, c01 = 0, c02 = 0, s0 = 0;
+        if (need0) { c00 = Y0[t]; c01 = Y1[t]; c02 = Y2[t]; s0 = SY[t]; }
+#pragma unroll 1
+        for (int k = 0; k < cnt; k++)
+        {
+          const int gf = gf0 + k;
+          const double2 a01 = row_a01(sAb, gf);
+          const double2 a23 = row_a23(sAb, gf);                                       // a23.y = b + tol
+          const double u1 = fma(a01.x, c10, fma(a01.y, c11, fma(a23.x, c12, -a23.y))) * s1;
+          const double u2 = fma(a01.x, c20, fma(a01.y, c21, fma(a23.x, c22, -a23.y))) * s2;
+          const double u3 = fma(a01.x, c30, fma(a01.y, c31, fma(a23.x, c32, -a23.y))) * s3;
+          int km = max(max(rank_key(u1), rank_key(u2)), rank_key(u3));
+          if (need0) km = max(km, rank_key(fma(a01.x, c00, fma(a01.y, c01, fma(a23.x, c02, -a23.y))) * s0));
+          const int i = i0 + k, tie = ((i & 31) << 16) | ((i >> 5) + 1);
+          if (km > bkey || (km == bkey && tie < btie)) { bkey = km; btie = tie; }
+        }
+      }
     }
     const int mk = __reduce_max_sync(FULL, bkey);
 #ifdef FQ_PHASE_CLOCKS
-    if (clk && clk[5] == 0) clk[5] = clock64();
+    if (clk)
+    {
+      const long long scan1 = clock64();
+      if (clk[5] == 0) clk[5] = scan1;
+      clk[9] += scan1 - scan0;
+    }
 #endif
     if (mk <= 0) { status = 1; break; }
-    const int key = bkey;
-    const int src = __ffs(__ballot_sync(FULL, key == mk)) - 1;
-    const unsigned code = __shfl_sync(FULL, bcode, src);
+    const int mt = __reduce_min_sync(FULL, bkey == mk ? btie : 0x7fffffff);
+    // a box row: lane mt >> 16 holds it in bcode (items never overwrite bcode); an item: its index, from the tie code
+    const unsigned boxc = __shfl_sync(FULL, bcode, (mt >> 16) & 31);
+    const unsigned code = (mt & 0xffff) == 0 ? boxc : (unsigned)((((mt & 0xffff) - 1) << 5) | (mt >> 16));
     // ---- decode the chosen row: Y row y, weights (w0,w1,w2), right-hand side h
     int y;
     double w0 = 0, w1 = 0, w2 = 0, h;
@@ -690,7 +733,7 @@ __device__ void solve_candidate(const FqKernelArgs& a, const double* __restrict_
     }
   }
   // ---- corridor item list
-  int total_rows = 0;
+  int run = 0;                                   // this lane's run of corridor items (none without polytopes)
   if (P > 0)
   {
     int p = 0;
@@ -739,9 +782,9 @@ __device__ void solve_candidate(const FqKernelArgs& a, const double* __restrict_
       }
     }
     FQ_STAMP(clk, 3);
-    total_rows = build_items<D>(m, sfo, lane, N, p, a.item_cap);
+    run = build_items<D>(m, sfo, lane, N, p, a.item_cap);
     FQ_STAMP(clk, 4);
-    if (total_rows < 0)
+    if (run < 0)
     { // the row list does not fit: report "not solved" (iters = -2 marks the cause)
       if (lane == 0)
       {
@@ -770,7 +813,7 @@ __device__ void solve_candidate(const FqKernelArgs& a, const double* __restrict_
   int bkey = 0;
   unsigned bcode = 0;
   update_Y<D, true>(m, TZ, Yeq, bthr, SY, lane, bkey, bcode);
-  const int status = gi_loop<D, LEAN>(m, TZ, SY, sAb, Yeq, bthr, lane, total_rows, inv1, inv2, inv3, lim0, lim1, lim2,
+  const int status = gi_loop<D, LEAN>(m, TZ, SY, sAb, Yeq, bthr, lane, run, inv1, inv2, inv3, lim0, lim1, lim2,
                                       a.row_tol, lam, rdinv, q, it, bkey, bcode, a.dt + cand, a.lim + prob * 3, clk);
   FQ_STAMP(clk, 6);
 #ifdef FQ_PHASE_CLOCKS
@@ -960,7 +1003,7 @@ __global__ void __launch_bounds__(W * 32, (N_ <= 10 ? (WHOLE_ ? FQ_MIN_CTAS_WHOL
     while (c < count)
     {
 #ifdef FQ_PHASE_CLOCKS
-      long long clk[9] = {};
+      long long clk[10] = {};
       clk[0] = clock64();
 #else
       long long* clk = nullptr;
@@ -989,6 +1032,7 @@ __global__ void __launch_bounds__(W * 32, (N_ <= 10 ? (WHOLE_ ? FQ_MIN_CTAS_WHOL
           for (int k = 0; k < 6; k++) atomicAdd(acc + k, (unsigned long long)(clk[k + 1] - clk[k]));
           atomicAdd(acc + 6, (unsigned long long)(end - clk[6]));
           atomicAdd(acc + 7, 1ull);
+          atomicAdd(acc + 8, (unsigned long long)clk[9]);
         }
 #endif
       }

@@ -3,7 +3,9 @@
 library built with -DFQ_PHASE_CLOCKS and prints, for the whole and the safe sweep, each phase's share of the solver warps'
 clock cycles, split by outcome: "settled" candidates are decided by the iterate w = 0 (optimal with no iteration, or
 infeasible at the first entering row), the others need the active-set iteration.  Candidates the early exit skips never
-reach solve_candidate and are not counted; the winners' re-solve (one candidate per corridor) is.
+reach solve_candidate and are not counted; the winners' re-solve (one candidate per corridor) is.  The last line of each
+table, "corridor scans", is the part of the first-scan and iteration phases spent scanning the corridor rows for the
+entering row (every scan of gi_loop, up to the warp's choice): a share of the same cycles, not an eighth phase.
 
 usage: phase_clocks.py [--build] [--reps K] [--lib NAME]   (--build compiles faster_b200/lib/NAME first, on any machine)
 """
@@ -39,13 +41,13 @@ L = capi.lib()
 if not hasattr(L, "fq_phase_clocks"):
     sys.exit("%s was not built with -DFQ_PHASE_CLOCKS (run with --build first)" % lib_path)
 L.fq_phase_clocks.argtypes = [C.POINTER(C.c_ulonglong), C.c_int]
-buf = (C.c_ulonglong * 32)()
+buf = (C.c_ulonglong * 36)()
 
 
 def read(reset):
     if L.fq_phase_clocks(buf, 1 if reset else 0) != 0:
         sys.exit("fq_phase_clocks failed")
-    return np.array(buf[:], dtype=np.float64).reshape(2, 2, 8)
+    return np.array(buf[:], dtype=np.float64).reshape(2, 2, 9)
 
 
 dev = torch.device("cuda:0")
@@ -76,8 +78,14 @@ for mi, mode in ((1, "whole"), (0, "safe")):
         rows.append(r)
         print("  %-22s %9.1f %9.1f %9.1f   %12.0f %12.0f" % (name, 100 * r["share"], 100 * r["settled"], 100 * r["other"],
                                                            r["settled_cycles_per_cand"], r["other_cycles_per_cand"]))
+    scan = acc[mi, :, 8]
+    sc = dict(share=scan.sum() / tot, settled=scan[1] / tot, other=scan[0] / tot,
+              settled_cycles_per_cand=scan[1] / max(n[1], 1), other_cycles_per_cand=scan[0] / max(n[0], 1))
+    print("  %-22s %9.1f %9.1f %9.1f   %12.0f %12.0f" % ("(corridor scans)", 100 * sc["share"], 100 * sc["settled"], 100 * sc["other"],
+                                                       sc["settled_cycles_per_cand"], sc["other_cycles_per_cand"]))
     out[mode] = dict(candidates=float(n.sum() / args.reps), settled_fraction=float(n[1] / max(n.sum(), 1)),
-                     settled_cycle_share=float(cyc[1].sum() / max(tot, 1)), phases=rows)
+                     settled_cycle_share=float(cyc[1].sum() / max(tot, 1)), phases=rows,
+                     corridor_scans={k: float(v) for k, v in sc.items()})
 props = torch.cuda.get_device_properties(0)
 print("device:", props.name)
 if args.json:
