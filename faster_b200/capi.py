@@ -21,7 +21,8 @@ EXPORTS = ["fq_abi_version", "fq_create", "fq_destroy", "fq_last_error", "fq_set
            "fq_replan_pairs_decomp_async", "fq_replan_pairs_decomp_dev", "fq_replan_pairs_hr", "fq_replan_pairs_hr_async",
            "fq_replan_pairs_hr_dev", "fq_map_create", "fq_map_destroy", "fq_map_update", "fq_map_update_dev", "fq_map_size",
            "fq_replan_pairs_map", "fq_replan_pairs_map_async", "fq_replan_pairs_map_dev", "fq_replan_pairs_plan",
-           "fq_replan_pairs_plan_async", "fq_replan_pairs_plan_dev"]
+           "fq_replan_pairs_plan_async", "fq_replan_pairs_plan_dev", "fq_map_paths", "fq_map_paths_dev", "fq_paths_cloud",
+           "fq_jps_in"]
 
 
 class FqError(RuntimeError):
@@ -103,6 +104,18 @@ class PairMap(C.Structure):
 class PairPlan(C.Structure):
     """fq_pair_plan of include/faster_b200.h: every corridor's committed plan piece, sampled on the device."""
     _fields_ = [("cap_states", C.c_longlong), ("states", C.c_void_p), ("plan_ofs", C.c_void_p), ("status", C.c_void_p)]
+
+
+class MapPathsArgs(C.Structure):
+    """fq_map_paths_args of include/faster_b200.h; pointers as integers (host or device addresses)."""
+    _fields_ = [("n_prob", C.c_int), ("in_ofs", C.c_void_p), ("in", C.c_void_p), ("maps", C.c_void_p), ("n_maps", C.c_int),
+                ("map_index", C.c_void_p), ("drone_radius", C.c_double), ("max_poly_whole", C.c_int), ("max_poly_safe", C.c_int),
+                ("max_in", C.c_int), ("poly_ofs_whole", C.c_void_p), ("poly_ofs_safe", C.c_void_p), ("path_whole", C.c_void_p),
+                ("path_safe", C.c_void_p), ("status", C.c_void_p), ("crossed", C.c_void_p)]
+
+
+PATHS_OK, PATHS_SHORT, PATHS_STALL, PATHS_MAP, PATHS_INPUT = 0, 1, 2, 3, 4   # FQ_PATHS_*
+PATHS_OUT_KEYS = ["poly_ofs_whole", "poly_ofs_safe", "path_whole", "path_safe", "status", "crossed"]
 
 
 PLAN_OK, PLAN_NONE, PLAN_CAPACITY = 0, 1, 2                             # FQ_PLAN_*
@@ -197,6 +210,10 @@ def lib():
         L.fq_map_update.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
         L.fq_map_update_dev.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p]
         L.fq_map_size.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        L.fq_map_paths.argtypes = [C.POINTER(MapPathsArgs)]
+        L.fq_map_paths_dev.argtypes = [C.POINTER(MapPathsArgs), C.c_void_p]
+        L.fq_paths_cloud.argtypes = [C.POINTER(MapPathsArgs), C.c_void_p, C.c_void_p]
+        L.fq_jps_in.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_void_p, C.c_int]
         L.fq_create_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_void_p]
         L.fq_comm_unique_id.argtypes = [C.c_void_p]
         L.fq_comm_init.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
@@ -397,6 +414,78 @@ class Map:
             self.handle = None
 
     __del__ = close
+
+
+def jps_in(jps, start, goal, ra, dist_max=1.5):
+    """fq_jps_in: JPS_in (float64[n, 3]) of a fq_jps3d_plan_world path from start to goal, clipped at ra around its first
+    vertex and with vertices at most dist_max apart (faster.cpp:361-384)."""
+    p, s, g = np.ascontiguousarray(np.reshape(jps, (-1, 3)), np.float64), _f64(start, 3), _f64(goal, 3)
+    L = lib()
+    n = L.fq_jps_in(p.ctypes.data, len(p), s.ctypes.data, g.ctypes.data, float(ra), float(dist_max), None, 0)
+    if n < 0:
+        raise FqError("fq_jps_in failed (%d): %s" % (n, L.fq_last_error(None).decode()))
+    out = np.zeros((n, 3))
+    L.fq_jps_in(p.ctypes.data, len(p), s.ctypes.data, g.ctypes.data, float(ra), float(dist_max), out.ctypes.data, n)
+    return out
+
+
+def map_paths_args(n_prob, in_ofs, in_, out_ptrs, drone_radius=HR_DEFAULTS["drone_radius"], max_poly_whole=3, max_poly_safe=4,
+                   maps=(), map_index=None, max_in=0):
+    """MapPathsArgs; in_ofs / in_ / map_index: addresses (map_index None: NULL), out_ptrs: addresses of PATHS_OUT_KEYS
+    (status and crossed may be 0/None/missing = NULL), maps: Map objects.  The struct keeps the maps' table alive."""
+    s = MapPathsArgs()
+    s.table = (C.c_void_p * max(len(maps), 1))(*[m.handle for m in maps])
+    s.n_prob, s.in_ofs = int(n_prob), in_ofs
+    setattr(s, "in", in_)
+    s.maps, s.n_maps, s.map_index = (C.addressof(s.table) if len(maps) else None), len(maps), map_index or None
+    s.drone_radius, s.max_poly_whole, s.max_poly_safe, s.max_in = float(drone_radius), int(max_poly_whole), int(max_poly_safe), int(max_in)
+    for k in PATHS_OUT_KEYS:
+        setattr(s, k, out_ptrs.get(k) or None)
+    return s
+
+
+def _paths_call(paths, call, max_poly_whole, max_poly_safe, **kw):
+    """Packs the JPS_in list `paths`, calls call(args) and returns the outputs: poly_ofs_* (int32, n_prob + 1), path_*
+    (float64, the rows written), status (int32) and crossed (uint8)."""
+    n = len(paths)
+    pts = [np.asarray(p, np.float64).reshape(-1, 3) for p in paths]
+    in_ofs = np.concatenate([[0], np.cumsum([len(p) for p in pts])]).astype(np.int32)
+    in_ = np.ascontiguousarray(np.vstack(pts)) if in_ofs[-1] else np.zeros((1, 3))
+    out = dict(poly_ofs_whole=np.zeros(n + 1, np.int32), poly_ofs_safe=np.zeros(n + 1, np.int32),
+               path_whole=np.zeros((n * (max_poly_whole + 1), 3)), path_safe=np.zeros((n * (max_poly_safe + 1), 3)),
+               status=np.full(n, -1, np.int32), crossed=np.full(n, 255, np.uint8))
+    s = map_paths_args(n, in_ofs.ctypes.data, in_.ctypes.data, {k: v.ctypes.data for k, v in out.items()},
+                       max_poly_whole=max_poly_whole, max_poly_safe=max_poly_safe, **kw)
+    rc = call(s)
+    if rc != 0:
+        raise FqError("map_paths failed (%d): %s" % (rc, lib().fq_last_error(None).decode()))
+    for k in ("whole", "safe"):
+        out["path_" + k] = out["path_" + k][:int(out["poly_ofs_" + k][-1]) + n].copy()
+    return out
+
+
+def map_paths(paths, maps, map_index=None, drone_radius=HR_DEFAULTS["drone_radius"], max_poly_whole=3, max_poly_safe=4):
+    """fq_map_paths: each corridor's whole and safe paths from its JPS_in (paths: list of [n_j, 3]) against the U of
+    maps[map_index[j]] (Map objects; map_index None: maps[0])."""
+    idx = None if map_index is None else np.ascontiguousarray(map_index, np.int32)
+    return _paths_call(paths, lambda s: lib().fq_map_paths(C.byref(s)), max_poly_whole, max_poly_safe, maps=maps,
+                       map_index=None if idx is None else idx.ctypes.data, drone_radius=drone_radius)
+
+
+def paths_cloud(paths, unks, drone_radius=HR_DEFAULTS["drone_radius"], max_poly_whole=3, max_poly_safe=4):
+    """fq_paths_cloud: map_paths on the host over per-corridor unknown clouds (unks: list of [m_j, 3])."""
+    u = [np.asarray(x, np.float64).reshape(-1, 3) for x in unks]
+    ofs = np.concatenate([[0], np.cumsum([len(x) for x in u])]).astype(np.int32)
+    cloud = np.ascontiguousarray(np.vstack(u)) if ofs[-1] else np.zeros((1, 3))
+    return _paths_call(paths, lambda s: lib().fq_paths_cloud(C.byref(s), ofs.ctypes.data, cloud.ctypes.data), max_poly_whole,
+                       max_poly_safe, drone_radius=drone_radius)
+
+
+def map_paths_dev(args, stream=0):
+    """fq_map_paths_dev: `args` (MapPathsArgs, map_paths_args) holds device addresses and max_in."""
+    rc = lib().fq_map_paths_dev(C.byref(args), stream or None)
+    if rc != 0:
+        raise FqError("fq_map_paths_dev failed (%d): %s" % (rc, lib().fq_last_error(None).decode()))
 
 
 def make_decomp_workload(pairs, max_faces=400, max_poly_faces=64):

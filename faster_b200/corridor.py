@@ -359,24 +359,9 @@ def forest_pair_paths(seed, N=10, max_poly_whole=3, max_poly_safe=4, Ra=4.0, r_f
     Vertex 0 of path_safe is the estimate of R that make_forest_pair_mixed cuts the safe corridor around (R_estimate, 9
     doubles); the device replaces it with its own R.  xf_whole / xf_safe put E and M at the paths' last vertices, as
     make_forest_pair_mixed does.  -> dict."""
-    from . import capi
     prof = UAV
     rng = np.random.default_rng(seed)
-    _, centres, radii = make_forest(seed, n_trees=n_trees)
-    grid_jps, origin, res = voxelise_forest(centres, radii, inflation=0.47)
-    grid, _, _ = voxelise_forest(centres, radii)
-    for _ in range(400):
-        s = np.array([rng.uniform(-6, 6), rng.uniform(-6, 6), rng.uniform(0.8, 1.4)])
-        ang = rng.uniform(-np.pi, np.pi)
-        t = s + rng.uniform(*query) * np.array([np.cos(ang), np.sin(ang), 0.0])
-        t[2] = rng.uniform(0.8, 1.4)
-        if np.abs(t[:2]).max() > 7.5:
-            continue
-        path, _ = capi.jps3d_plan_world(grid_jps, origin, res, s, t, True)
-        if len(path) >= 2 and np.linalg.norm(path[-1] - path[0]) > 0.3:
-            break
-    else:
-        raise RuntimeError("no path found")
+    path, _, t, grid, origin, res = _forest_query(rng, seed, n_trees, query)
     path_all = split_long_segments(path, 1.5)
     verts = split_long_segments(clip_path_to_sphere(path, path[0], Ra), 1.5)[:max_poly_whole + 1]
     obs = (np.argwhere(grid > 0)[:, ::-1] + 0.5) * res + origin
@@ -405,6 +390,34 @@ def forest_pair_paths(seed, N=10, max_poly_whole=3, max_poly_safe=4, Ra=4.0, r_f
     xfs[:3] = spath[-1]
     return dict(N=N, DC=DC, path_whole=np.asarray(verts, float), path_safe=np.asarray(spath, float), path_all=path_all, obs=obs,
                 goal=np.asarray(t, float), x0=x0, xf_whole=xf, xf_safe=xfs, lim=lim, R_estimate=R9, seed=seed, profile="uav")
+
+
+def _forest_query(rng, seed, n_trees, query):
+    """The JPS query of forest_pair_paths: a start and a goal `query` metres apart drawn from rng, and the product's JPS path
+    between them on the inflated forest.  -> (path, goal, grid, origin, res) with the uninflated grid."""
+    from . import capi
+    _, centres, radii = make_forest(seed, n_trees=n_trees)
+    grid_jps, origin, res = voxelise_forest(centres, radii, inflation=0.47)
+    grid, _, _ = voxelise_forest(centres, radii)
+    for _ in range(400):
+        s = np.array([rng.uniform(-6, 6), rng.uniform(-6, 6), rng.uniform(0.8, 1.4)])
+        ang = rng.uniform(-np.pi, np.pi)
+        t = s + rng.uniform(*query) * np.array([np.cos(ang), np.sin(ang), 0.0])
+        t[2] = rng.uniform(0.8, 1.4)
+        if np.abs(t[:2]).max() > 7.5:
+            continue
+        path, _ = capi.jps3d_plan_world(grid_jps, origin, res, s, t, True)
+        if len(path) >= 2 and np.linalg.norm(path[-1] - path[0]) > 0.3:
+            return path, s, t, grid, origin, res
+    raise RuntimeError("no path found")
+
+
+def forest_jps(seed, n_trees=60, query=(0.6, 7.0)):
+    """The JPS query of forest_pair_paths(seed) before anything is cut from it: the planner's path (cell centres, as
+    fq_jps3d_plan_world returns it), its start and its goal.  -> dict(jps, start, goal, seed, x0) with x0 = the start."""
+    rng = np.random.default_rng(seed)
+    path, s, t, _, _, _ = _forest_query(rng, seed, n_trees, query)
+    return dict(jps=path, start=s, goal=np.asarray(t, float), seed=seed, x0=np.concatenate([s, np.zeros(6)]))
 
 
 def forest_unknown_cloud(p, seed=None, half=3.0, dz=0.6, sensing=(1.6, 4.5), n_trees=60):

@@ -6,6 +6,7 @@
 #pragma once
 #include "fq_assign.h"
 #include "fq_dtinit.h"
+#include "fq_paths.h"
 #include "fq_window.h"
 
 namespace fqp
@@ -281,26 +282,7 @@ __global__ void fq_pair_mid_kernel(const FqPairMidArgs a)
 //      close, at any coordinate magnitude.
 //   R: the first i in 0 .. indexH whose braking distance sign(v (H - p)) v^2 / (2 delta_a a_max) exceeds |H - p| in x or y,
 //      else indexH.  Threads take strided samples, each walking its own sample clock; the first index is a block minimum.
-#if defined(__CUDA_ARCH__)
-#define FQ_F2(x) __double2float_rn(x)
-#define FQ_FMUL(a, b) __fmul_rn((a), (b))
-#define FQ_FADD(a, b) __fadd_rn((a), (b))
-#define FQ_FSUB(a, b) __fsub_rn((a), (b))
-#define FQ_FSQRT(a) __fsqrt_rn(a)
-#else
-#define FQ_F2(x) ((float)(x))
-#define FQ_FMUL(a, b) ((a) * (b))
-#define FQ_FADD(a, b) ((a) + (b))
-#define FQ_FSUB(a, b) ((a) - (b))
-#define FQ_FSQRT(a) std::sqrt((float)(a))
-#endif
-
-// squared float distance in FLANN's L2 order (flann/algorithms/dist.h, L2::operator() for 3 values)
-FQ_HD float flann_l2(const float* q, const double* p)
-{
-  const float dx = FQ_FSUB(FQ_F2(p[0]), q[0]), dy = FQ_FSUB(FQ_F2(p[1]), q[1]), dz = FQ_FSUB(FQ_F2(p[2]), q[2]);
-  return FQ_FADD(FQ_FADD(FQ_FADD(0.0f, FQ_FMUL(dx, dx)), FQ_FMUL(dy, dy)), FQ_FMUL(dz, dz));
-}
+// (flann_l2 and the float FQ_F* operations: fq_paths.h)
 
 // findIndexR's test of one sample (faster.cpp:186-196): any of x, y with a braking distance above |H - p|
 FQ_HD bool brakes_past(const double* H, const double* o, double delta_a, double a_max)

@@ -48,7 +48,7 @@ typedef struct fq_ctx fq_ctx;     /* opaque: device, stream, plan tables, scratc
 int fq_abi_version(void);
 /* 1 if this build has the named feature: "sweep_early_exit", "replan_pairs", "multi_gpu", "row_tol", "certificates",
  * "replan_pairs_assign", "replan_pairs_window", "replan_pairs_exact", "replan_pairs_decomp", "replan_pairs_hr",
- * "replan_pairs_map", "replan_pairs_plan". */
+ * "replan_pairs_map", "replan_pairs_plan", "map_paths". */
 int fq_has_feature(const char* name);
 
 /* Threading: a context is used from one thread at a time, like a SolverGurobi instance in the reference (one replan
@@ -579,6 +579,87 @@ int fq_replan_pairs_map_async(fq_ctx* ctx, const fq_pair_args* args, const fq_pa
 int fq_replan_pairs_map_dev(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
                             const fq_pair_exact* exact, const fq_pair_decomp* decomp, const fq_pair_hr* hr, const fq_pair_map* map,
                             fq_pair_result* results_all, void* stream);
+
+/* ---- whole and safe paths from JPS_in against an indexed map ----------------------------------------------------------
+ *
+ * Faster::replan decomposes two paths (faster.cpp:373-393, :449-496): JPS_whole = deleteVertexes(JPS_in, max_poly_whole)
+ * and JPS_safe, which is JPS_in cropped where it first nears unknown space -- getFirstCollisionJPS(JPS_in, UNKNOWN_MAP,
+ * RETURN_INTERSECTION) (:767-921) -- then trimmed by deleteVertexes(., max_poly_safe).  (The reference then replaces vertex
+ * 0 of JPS_safe by R, :485; the decomposing chains do that on the device.)  fq_map_paths computes both from each corridor's
+ * JPS_in and the U of its map, and writes them in the layout fq_pair_args.poly_ofs_* / fq_pair_decomp.path_* take, so its
+ * outputs feed fq_replan_pairs_map* as they are.  Feature "map_paths".
+ *
+ * The crop, per corridor, in the reference's own mix of float and double (faster_b200/csrc/fq_paths.h):
+ *   the head starts at vertex 0; each step takes q = the head rounded to float (eigenPoint2pclPoint), d^2 = the exact float
+ *   minimum of FLANN's L2 ((0 + dx^2) + dy^2) + dz^2 over U (as fq_pair_hr's findIndexH; DESIGN.md 3.2) and r = sqrtf(d^2);
+ *   r < drone_radius: a collision -- at the first step the path becomes [v0, v0 + (0.01, 0, 0)] (:833-841), later the vertices
+ *     passed so far plus the head, shortened by drone_radius (reduceJPSbyDistance, utils.cpp:690-710); crossed = 1;
+ *   otherwise the head moves to where the path leaves the sphere (head, r) (getFirstIntersectionWithSphere and
+ *     getIntersectionWithSphere, utils.cpp:713-866, with their float temporaries and the fallback of a discriminant <= 0);
+ *   no vertex outside the sphere, or an empty U: the path is JPS_in unchanged, crossed = 0.
+ * A step reads only the map cells within max(drone_radius, the farthest vertex left) of the head, widened for the float
+ * rounding as fq_replan_pairs_map's H/R does: a nearest point beyond that range changes nothing.  A crop that takes
+ * FQ_PATHS_MAX_STEPS steps stops with FQ_PATHS_STALL.
+ *
+ * Outputs: corridor j's whole path has P_w + 1 vertices (P_w = min(n_in - 1, max_poly_whole)) at rows poly_ofs_whole[j] + j
+ * .. poly_ofs_whole[j+1] + j of path_whole, the safe path likewise with P_s = min(|cropped| - 1, max_poly_safe).  So
+ * neither array ever needs more than n_prob x (max_poly_* + 1) rows.  A corridor whose status is not FQ_PATHS_OK gets one
+ * vertex of NaN (P = 0) in both, which the chained replan gives no winner.
+ *
+ * A map must not be updated or destroyed while a call that reads it is in flight.  The call reads each map through the
+ * descriptor of fq_replan_pairs_map*, so a CUDA graph of fq_map_paths_dev replayed after later updates reads the last one. */
+#define FQ_PATHS_OK 0
+#define FQ_PATHS_SHORT 1      /* JPS_in has fewer than 2 vertices (_dev)                                                */
+#define FQ_PATHS_STALL 2      /* the crop took FQ_PATHS_MAX_STEPS steps                                                 */
+#define FQ_PATHS_MAP 3        /* map_index out of range (_dev)                                                          */
+#define FQ_PATHS_INPUT 4      /* JPS_in has more than max_in vertices, a negative offset or a non-finite vertex (_dev)  */
+#define FQ_PATHS_MAX_STEPS 4096
+#define FQ_PATHS_MAX_IN 4096  /* vertices of one JPS_in                                                                 */
+typedef struct fq_map_paths_args
+{
+  int n_prob;
+  const int* in_ofs;                     /* n_prob + 1: JPS_in of corridor j (faster.cpp:373-384) is rows in_ofs[j] ..     */
+  const double* in;                      /*   in_ofs[j+1]-1 of in (x, y, z), >= 2 vertices; fq_jps_in makes it             */
+  const fq_map* const* maps;             /* n_maps maps, all on one device: corridor j reads the U of maps[map_index[j]]   */
+  int n_maps;
+  const int* map_index;                  /* n_prob, or NULL: every corridor reads maps[0]                                  */
+  double drone_radius;                   /* par_.drone_radius, > 0                                                          */
+  int max_poly_whole, max_poly_safe;     /* par_.max_poly_whole / _safe, 1 .. FQ_MAX_POLY                                   */
+  int max_in;                            /* _dev only: the longest JPS_in, 2 .. FQ_PATHS_MAX_IN (longer: FQ_PATHS_INPUT)   */
+  int *poly_ofs_whole, *poly_ofs_safe;   /* out n_prob + 1: fq_pair_args.poly_ofs_*                                         */
+  double *path_whole, *path_safe;        /* out, room for n_prob x (max_poly_* + 1) rows: fq_pair_decomp.path_*            */
+  int* status;                           /* out n_prob, or NULL: FQ_PATHS_*                                                 */
+  uint8_t* crossed;                      /* out n_prob, or NULL: getFirstCollisionJPS's thereIsIntersection                 */
+} fq_map_paths_args;
+
+/* HOST pointers everywhere (maps and map_index included); blocks until every output is in the caller's arrays.  Runs on
+ * the maps' device.  FQ_E_ARG (text in fq_last_error(NULL)): p NULL, n_prob <= 0, a NULL input or output array, in_ofs not
+ * starting at 0 or decreasing, a corridor with fewer than 2 or more than FQ_PATHS_MAX_IN vertices, a non-finite vertex,
+ * drone_radius not finite or <= 0 (the reference can then loop forever on a point of the path), max_poly_* outside
+ * 1 .. FQ_MAX_POLY, no maps, a NULL map, maps on different devices, a map whose last update failed, and a map_index entry
+ * outside 0 .. n_maps-1.  max_in is not read. */
+int fq_map_paths(const fq_map_paths_args* p);
+/* DEVICE pointers (the struct and the maps array live on the host; map_index is a device array); stream-ordered on
+ * `stream`, which must belong to the maps' device (NULL: the legacy default stream), and never synchronises, so a CUDA
+ * graph can capture it.  Its scratch (n_prob x 40 bytes and the map table) is stream-ordered memory (cudaMallocAsync).
+ * Refused as fq_map_paths, except that what only the arrays tell -- offsets, vertex counts and values, map_index -- is
+ * reported per corridor in status instead: FQ_PATHS_SHORT, FQ_PATHS_INPUT, FQ_PATHS_MAP. */
+int fq_map_paths_dev(const fq_map_paths_args* p, void* stream);
+/* The same crop on the host over per-corridor clouds instead of maps: corridor j's U is rows unk_ofs[j] .. unk_ofs[j+1]-1
+ * of unk (n_prob + 1 offsets from 0, non-decreasing; unk may be NULL when every cloud is empty), and the nearest point is
+ * found by brute force.  For the same JPS_in and clouds it writes what fq_map_paths writes, byte for byte.  maps,
+ * n_maps, map_index and max_in are not read; the other refusals are fq_map_paths's, plus a non-finite unknown point.  Pure
+ * host code. */
+int fq_paths_cloud(const fq_map_paths_args* p, const int* unk_ofs, const double* unk);
+/* JPS_in from a path of fq_jps3d_plan_world (faster.cpp:361-384): vertex 0 := start and the last vertex := goal, both with
+ * z raised to 0 if below, as solveJPS3D forces them (jps_manager.cpp:143-144, :172-186: a one-vertex path becomes [start,
+ * goal]); the path up to where it first leaves the sphere of radius ra around vertex 0 (getFirstIntersectionWithSphere,
+ * :373-382; the caller passes ra = min(dist_to_goal - 0.001, Ra)); then createMoreVertexes(dist_max) (:80-97).  Writes
+ * the first min(count, cap) vertices to out and returns the count (out may be NULL with cap 0).  FQ_E_ARG: jps, start or
+ * goal NULL, n < 1, cap < 0, out NULL with cap > 0, a non-finite vertex, start, goal or ra, dist_max not finite or <= 0,
+ * and a count above 2^30.  Pure host code. */
+int fq_jps_in(const double* jps, int n, const double* start, const double* goal, double ra, double dist_max, double* out,
+              int cap);
 
 /* ---- chained replan that returns each corridor's committed plan --------------------------------------------------------
  *
