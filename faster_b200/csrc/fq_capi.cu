@@ -226,16 +226,9 @@ int fq_settle(fq_ctx* ctx)
 
 namespace
 {
-struct HostLayout
-{ // byte offsets of each array inside the input / output arenas
-  size_t x0, xf, lim, dt, Ab, poly_ofs, face_ofs, cand_ofs, sigma, in_bytes;
-  size_t cost, coeffs, iters, feasible, win_cost, win_dt, win_idx, win_ofs, out_bytes;
-};
-
 // validates the host description and computes sizes
 int describe(fq_ctx* ctx, int N, int force_final, int n_prob, const int* poly_ofs, const int* face_ofs,
-             const int* cand_ofs, const uint8_t* sigma, bool want_coeffs, bool want_iters, HostLayout* L,
-             FqCorridorSizes* cs, int* n_cand, int* max_cand)
+             const int* cand_ofs, const uint8_t* sigma, FqCorridorSizes* cs, int* n_cand, int* max_cand)
 {
   const int ne = force_final ? 3 : 2;
   if (N < ne || N > FQ_MAX_N) return fq_fail(ctx, FQ_E_ARG, "N out of range");
@@ -255,27 +248,6 @@ int describe(fq_ctx* ctx, int N, int force_final, int n_prob, const int* poly_of
     if (nc > *max_cand) *max_cand = nc;
   }
   *n_cand = cand_ofs[n_prob];
-  size_t o = 0;
-  L->Ab = o;        o = fq_align16(o + sizeof(double) * 4 * (size_t)(cs->n_face > 0 ? cs->n_face : 1));
-  L->x0 = o;        o += sizeof(double) * 9 * (size_t)n_prob;
-  L->xf = o;        o += sizeof(double) * 9 * (size_t)n_prob;
-  L->lim = o;       o += sizeof(double) * 3 * (size_t)n_prob;
-  L->poly_ofs = o;  o += sizeof(int) * (size_t)(n_prob + 1);
-  L->face_ofs = o;  o += sizeof(int) * (size_t)(cs->n_poly + 1);
-  L->cand_ofs = o;  o = fq_align16(o + sizeof(int) * (size_t)(n_prob + 1));
-  L->dt = o;        o += sizeof(double) * (size_t)*n_cand;      // per-candidate arrays last: [0, dt) is the
-  L->sigma = o;     o += (size_t)*n_cand * N;                   // per-problem description
-  L->in_bytes = fq_align16(o);
-  o = 0;
-  L->cost = o;      o += sizeof(double) * (size_t)*n_cand;
-  L->win_cost = o;  o += sizeof(double) * (size_t)n_prob;       // per-problem winners (fq_solve_multi_sharded)
-  L->win_dt = o;    o += sizeof(double) * (size_t)n_prob;
-  L->coeffs = o;    o += want_coeffs ? sizeof(double) * 12 * (size_t)N * (size_t)*n_cand : 0;
-  L->iters = o;     o += want_iters ? sizeof(int32_t) * (size_t)*n_cand : 0;
-  L->win_idx = o;   o += sizeof(int) * (size_t)n_prob;
-  L->win_ofs = o;   o += sizeof(int) * (size_t)(n_prob + 1);
-  L->feasible = o;  o += (size_t)*n_cand;
-  L->out_bytes = fq_align16(o);
   return 0;
 }
 
@@ -300,7 +272,7 @@ struct Trace
 int solve_multi_impl(fq_ctx* ctx, int N, int force_final, int n_prob, const double* x0, const double* xf,
                      const double* lim, const int* poly_ofs, const int* face_ofs, const double* Ab,
                      const int* cand_ofs, const double* dt, const uint8_t* sigma, uint8_t* feasible,
-                     double* cost, double* coeffs, int32_t* iters, bool deferred, HostLayout* L_out = nullptr,
+                     double* cost, double* coeffs, int32_t* iters, bool deferred, FqSelectMultiArgs* sel = nullptr,
                      double* cert = nullptr, int cert_stride = 0)
 {
   if (!ctx) return FQ_E_ARG;
@@ -308,13 +280,10 @@ int solve_multi_impl(fq_ctx* ctx, int N, int force_final, int n_prob, const doub
   Trace tr;
   if (!x0 || !xf || !lim || !poly_ofs || !face_ofs || !cand_ofs || !dt || !feasible || !cost)
     return fq_fail(ctx, FQ_E_ARG, "NULL argument");
-  HostLayout L;
   FqCorridorSizes cs;
   int n_cand, max_cand;
-  int rc = describe(ctx, N, force_final, n_prob, poly_ofs, face_ofs, cand_ofs, sigma, coeffs != nullptr,
-                    iters != nullptr, &L, &cs, &n_cand, &max_cand);
+  int rc = describe(ctx, N, force_final, n_prob, poly_ofs, face_ofs, cand_ofs, sigma, &cs, &n_cand, &max_cand);
   if (rc) return rc;
-  if (L_out) *L_out = L;
   tr.mark("describe");
   if (n_cand == 0) return 0;
   const int n_poly = cs.n_poly;
@@ -329,53 +298,66 @@ int solve_multi_impl(fq_ctx* ctx, int N, int force_final, int n_prob, const doub
     if (!fq_scan_all_positive_finite(lim, 3 * (size_t)n_prob)) return "limits must be finite and > 0";
     return nullptr;
   };
-  const bool big = L.in_bytes > kPackThreshold;
+  FqKernelArgs a{};      // the whole batch; a slice of it offsets the per-problem pointers
+  a.N = N; a.force_final = force_final; a.n_prob = n_prob; a.max_faces = cs.max_faces;
+  a.cert = cert; a.cert_stride = cert_stride;
+  const size_t sig_bytes = (size_t)n_cand * N;
+  bool big = false;
+  size_t head = 0;
+  double* d_dt = nullptr;
+  uint8_t* d_sig = nullptr;
+  // the per-problem description comes first, the per-candidate arrays last: the throughput path uploads [0, head) as one
+  // head copy, then slices of dt and sigma straight from the caller's buffers
+  auto layout_in = [&](FqPack& p) {
+    a.Ab = cs.n_face > 0 ? p.in(Ab, 4 * (size_t)cs.n_face) : p.scratch<double>(0);
+    a.x0 = p.in(x0, 9 * (size_t)n_prob);  a.xf = p.in(xf, 9 * (size_t)n_prob);  a.lim = p.in(lim, 3 * (size_t)n_prob);
+    a.poly_ofs = p.in(poly_ofs, n_prob + 1);  a.face_ofs = p.in(face_ofs, n_poly + 1);  a.cand_ofs = p.in(cand_ofs, n_prob + 1);
+    head = p.at;
+    a.dt = d_dt = big ? p.scratch<double>(n_cand) : p.in(dt, n_cand);
+    a.sigma = d_sig = big || n_poly == 0 ? p.scratch<uint8_t>(sig_bytes) : p.in(sigma, sig_bytes);
+  };
+  auto layout_out = [&](FqPack& p) {
+    a.cost = p.scratch<double>(n_cand);  a.coeffs = p.out(coeffs, 12 * (size_t)N * n_cand);  a.iters = p.out(iters, n_cand);
+    a.feasible = p.scratch<uint8_t>(n_cand);
+    if (sel)
+    { // the per-problem winners of fq_solve_multi_host_ex
+      sel->win_cost = p.scratch<double>(n_prob);  sel->win_dt = p.scratch<double>(n_prob);
+      sel->win_idx = p.scratch<int>(n_prob);  sel->win_ofs = p.scratch<int>(n_prob + 1);
+    }
+  };
+  FqPack in, out;
+  layout_in(in);
+  layout_out(out);
+  big = in.at > kPackThreshold;
   if (!big)
     if (const char* why = values_ok()) return fq_fail(ctx, FQ_E_ARG, why);
   FQ_CUDA(cudaSetDevice(ctx->device));
-  FQ_CUDA(ctx->d_in.reserve(L.in_bytes));
-  FQ_CUDA(ctx->d_out.reserve(L.out_bytes));
-  char* din = (char*)ctx->d_in.p;
-  char* dout = (char*)ctx->d_out.p;
-  FqKernelArgs a{};      // the whole batch; a slice of it offsets the per-problem pointers
-  a.N = N; a.force_final = force_final; a.n_prob = n_prob;
-  a.x0 = (const double*)(din + L.x0); a.xf = (const double*)(din + L.xf); a.lim = (const double*)(din + L.lim);
-  a.poly_ofs = (const int*)(din + L.poly_ofs); a.face_ofs = (const int*)(din + L.face_ofs); a.Ab = (const double*)(din + L.Ab);
-  a.max_faces = cs.max_faces; a.cand_ofs = (const int*)(din + L.cand_ofs); a.dt = (const double*)(din + L.dt);
-  a.sigma = (const uint8_t*)(din + L.sigma); a.feasible = (uint8_t*)(dout + L.feasible); a.cost = (double*)(dout + L.cost);
-  a.coeffs = coeffs ? (double*)(dout + L.coeffs) : nullptr; a.iters = iters ? (int32_t*)(dout + L.iters) : nullptr;
-  a.cert = cert; a.cert_stride = cert_stride;
+  FQ_CUDA(ctx->d_in.reserve(in.at));
+  FQ_CUDA(ctx->d_out.reserve(out.at));
   cudaStream_t st = ctx->stream;
-  const size_t sig_bytes = (size_t)n_cand * N;
-  struct Piece { size_t off; const void* src; size_t bytes; };
-  const Piece pieces[] = {
-    { L.Ab, Ab, sizeof(double) * 4 * (size_t)cs.n_face }, { L.x0, x0, sizeof(double) * 9 * (size_t)n_prob },
-    { L.xf, xf, sizeof(double) * 9 * (size_t)n_prob }, { L.lim, lim, sizeof(double) * 3 * (size_t)n_prob },
-    { L.dt, dt, sizeof(double) * (size_t)n_cand },     { L.poly_ofs, poly_ofs, sizeof(int) * (size_t)(n_prob + 1) },
-    { L.face_ofs, face_ofs, sizeof(int) * (size_t)(n_poly + 1) },
-    { L.cand_ofs, cand_ofs, sizeof(int) * (size_t)(n_prob + 1) }, { L.sigma, sigma, n_poly > 0 ? sig_bytes : 0 },
-  };
-  if (L.in_bytes <= kPackThreshold)
+  // staged: everything (latency path) or the head; a head too large to stage goes up array by array
+  const bool staged = !big || head <= kPackThreshold;
+  if (staged) FQ_CUDA(ctx->h_in.reserve(big ? head : in.at));
+  in = in.place(ctx->d_in.p, staged ? ctx->h_in.p : nullptr, st);
+  layout_in(in);
+  out = out.place(ctx->d_out.p);
+  layout_out(out);
+  if (int prc = in.done(ctx)) return prc;
+  if (int prc = out.done(ctx)) return prc;
+  if (sel)
+  {
+    sel->cand_ofs = a.cand_ofs; sel->dt = a.dt; sel->feasible = a.feasible; sel->cost = a.cost;
+  }
+  if (!big)
   { // latency path: one pinned staging buffer, one H2D copy
-    FQ_CUDA(ctx->h_in.reserve(L.in_bytes));
-    for (const Piece& p : pieces)
-      if (p.bytes) std::memcpy((char*)ctx->h_in.p + p.off, p.src, p.bytes);
-    FQ_CUDA(cudaMemcpyAsync(din, ctx->h_in.p, L.in_bytes, cudaMemcpyHostToDevice, st));
+    FQ_CUDA(cudaMemcpyAsync(in.base, ctx->h_in.p, in.at, cudaMemcpyHostToDevice, st));
   }
   else
   { // throughput path: the per-problem description is small and goes through one staged copy; the per-candidate arrays
     // (dt, sigma) are DMA'd straight from the caller's buffers (true async when they are pinned) in up to four slices
     // of whole problems, alternating between two streams: slice k+1 uploads while slice k computes and slice k-1
     // downloads, and the next slice's CTAs fill the SMs that the previous launch's tail leaves idle.
-    const bool pack_head = L.dt <= kPackThreshold;
-    if (pack_head) FQ_CUDA(ctx->h_in.reserve(L.dt));
-    for (const Piece& p : pieces)
-    {
-      if (!p.bytes || p.off >= L.dt) continue;
-      if (pack_head) std::memcpy((char*)ctx->h_in.p + p.off, p.src, p.bytes);
-      else FQ_CUDA(cudaMemcpyAsync(din + p.off, p.src, p.bytes, cudaMemcpyHostToDevice, st));
-    }
-    if (pack_head) FQ_CUDA(cudaMemcpyAsync(din, ctx->h_in.p, L.dt, cudaMemcpyHostToDevice, st));
+    if (staged) FQ_CUDA(cudaMemcpyAsync(in.base, ctx->h_in.p, head, cudaMemcpyHostToDevice, st));
     FQ_CUDA(cudaEventRecord(ctx->ev_head, st));
     FQ_CUDA(cudaStreamWaitEvent(ctx->stream2, ctx->ev_head, 0));
     // chosen with bench.py (64 corridors x 1024 candidates) on the GPU the kernel was first tuned on: 4 slices are best for a blocking call (copies hide behind the
@@ -397,23 +379,23 @@ int solve_multi_impl(fq_ctx* ctx, int N, int force_final, int n_prob, const doub
       for (int j = p_lo; j < p_hi; j++) mc = std::max(mc, cand_ofs[j + 1] - cand_ofs[j]);
       if (c_n > 0)
       {
-        FQ_CUDA(cudaMemcpyAsync(din + L.dt + sizeof(double) * c_lo, dt + c_lo, sizeof(double) * c_n, cudaMemcpyHostToDevice, s2));
+        FQ_CUDA(cudaMemcpyAsync(d_dt + c_lo, dt + c_lo, sizeof(double) * c_n, cudaMemcpyHostToDevice, s2));
         if (n_poly > 0)
-          FQ_CUDA(cudaMemcpyAsync(din + L.sigma + c_lo * N, sigma + c_lo * N, c_n * N, cudaMemcpyHostToDevice, s2));
+          FQ_CUDA(cudaMemcpyAsync(d_sig + c_lo * N, sigma + c_lo * N, c_n * N, cudaMemcpyHostToDevice, s2));
         else
-          FQ_CUDA(cudaMemsetAsync(din + L.sigma + c_lo * N, 0, c_n * N, s2));
+          FQ_CUDA(cudaMemsetAsync(d_sig + c_lo * N, 0, c_n * N, s2));
         FqKernelArgs slice = a;
         slice.n_prob = p_hi - p_lo; slice.x0 += 9 * (size_t)p_lo; slice.xf += 9 * (size_t)p_lo; slice.lim += 3 * (size_t)p_lo;
         slice.poly_ofs += p_lo; slice.cand_ofs += p_lo;
         rc = fq_launch_solve_ctx(ctx, slice, mc, cs.max_poly_faces, s2);
         if (rc) { cudaStreamSynchronize(st); cudaStreamSynchronize(ctx->stream2); return rc; }
-        FQ_CUDA(cudaMemcpyAsync(cost + c_lo, dout + L.cost + sizeof(double) * c_lo, sizeof(double) * c_n, cudaMemcpyDeviceToHost, s2));
-        FQ_CUDA(cudaMemcpyAsync(feasible + c_lo, dout + L.feasible + c_lo, c_n, cudaMemcpyDeviceToHost, s2));
+        FQ_CUDA(cudaMemcpyAsync(cost + c_lo, a.cost + c_lo, sizeof(double) * c_n, cudaMemcpyDeviceToHost, s2));
+        FQ_CUDA(cudaMemcpyAsync(feasible + c_lo, a.feasible + c_lo, c_n, cudaMemcpyDeviceToHost, s2));
         if (coeffs)
-          FQ_CUDA(cudaMemcpyAsync(coeffs + 12 * (size_t)N * c_lo, dout + L.coeffs + sizeof(double) * 12 * (size_t)N * c_lo,
+          FQ_CUDA(cudaMemcpyAsync(coeffs + 12 * (size_t)N * c_lo, a.coeffs + 12 * (size_t)N * c_lo,
                                   sizeof(double) * 12 * (size_t)N * c_n, cudaMemcpyDeviceToHost, s2));
         if (iters)
-          FQ_CUDA(cudaMemcpyAsync(iters + c_lo, dout + L.iters + sizeof(int32_t) * c_lo, sizeof(int32_t) * c_n, cudaMemcpyDeviceToHost, s2));
+          FQ_CUDA(cudaMemcpyAsync(iters + c_lo, a.iters + c_lo, sizeof(int32_t) * c_n, cudaMemcpyDeviceToHost, s2));
       }
       p_lo = p_hi;
     }
@@ -427,28 +409,28 @@ int solve_multi_impl(fq_ctx* ctx, int N, int force_final, int n_prob, const doub
     if (why) return fq_fail(ctx, FQ_E_ARG, why);      // outputs were written but are not to be trusted
     return 0;
   }
-  if (n_poly == 0) FQ_CUDA(cudaMemsetAsync(din + L.sigma, 0, sig_bytes, st));
+  if (n_poly == 0) FQ_CUDA(cudaMemsetAsync(d_sig, 0, sig_bytes, st));
   rc = fq_launch_solve_ctx(ctx, a, max_cand, cs.max_poly_faces, st);
   if (rc) return rc;
-  if (L.out_bytes <= kPackThreshold)
+  if (out.at <= kPackThreshold)
   {
-    FQ_CUDA(ctx->h_out.reserve(L.out_bytes));
-    FQ_CUDA(cudaMemcpyAsync(ctx->h_out.p, dout, L.out_bytes, cudaMemcpyDeviceToHost, st));
+    FQ_CUDA(ctx->h_out.reserve(out.at));
+    FQ_CUDA(cudaMemcpyAsync(ctx->h_out.p, out.base, out.at, cudaMemcpyDeviceToHost, st));
     FQ_CUDA(cudaStreamSynchronize(st));
-    const char* ho = (const char*)ctx->h_out.p;
-    std::memcpy(cost, ho + L.cost, sizeof(double) * (size_t)n_cand);
-    std::memcpy(feasible, ho + L.feasible, (size_t)n_cand);
-    if (coeffs) std::memcpy(coeffs, ho + L.coeffs, sizeof(double) * 12 * (size_t)N * n_cand);
-    if (iters) std::memcpy(iters, ho + L.iters, sizeof(int32_t) * (size_t)n_cand);
+    out.host = (char*)ctx->h_out.p;
+    std::memcpy(cost, out.mirror(a.cost), sizeof(double) * (size_t)n_cand);
+    std::memcpy(feasible, out.mirror(a.feasible), (size_t)n_cand);
+    if (coeffs) std::memcpy(coeffs, out.mirror(a.coeffs), sizeof(double) * 12 * (size_t)N * n_cand);
+    if (iters) std::memcpy(iters, out.mirror(a.iters), sizeof(int32_t) * (size_t)n_cand);
   }
   else
   {
-    FQ_CUDA(cudaMemcpyAsync(cost, dout + L.cost, sizeof(double) * (size_t)n_cand, cudaMemcpyDeviceToHost, st));
-    FQ_CUDA(cudaMemcpyAsync(feasible, dout + L.feasible, (size_t)n_cand, cudaMemcpyDeviceToHost, st));
+    FQ_CUDA(cudaMemcpyAsync(cost, a.cost, sizeof(double) * (size_t)n_cand, cudaMemcpyDeviceToHost, st));
+    FQ_CUDA(cudaMemcpyAsync(feasible, a.feasible, (size_t)n_cand, cudaMemcpyDeviceToHost, st));
     if (coeffs)
-      FQ_CUDA(cudaMemcpyAsync(coeffs, dout + L.coeffs, sizeof(double) * 12 * (size_t)N * n_cand, cudaMemcpyDeviceToHost, st));
+      FQ_CUDA(cudaMemcpyAsync(coeffs, a.coeffs, sizeof(double) * 12 * (size_t)N * n_cand, cudaMemcpyDeviceToHost, st));
     if (iters)
-      FQ_CUDA(cudaMemcpyAsync(iters, dout + L.iters, sizeof(int32_t) * (size_t)n_cand, cudaMemcpyDeviceToHost, st));
+      FQ_CUDA(cudaMemcpyAsync(iters, a.iters, sizeof(int32_t) * (size_t)n_cand, cudaMemcpyDeviceToHost, st));
     FQ_CUDA(cudaStreamSynchronize(st));
   }
   return 0;
@@ -489,22 +471,16 @@ int fq_solve_multi_host_ex(fq_ctx* ctx, int N, int force_final, int n_prob, cons
                            const uint8_t* sigma, uint8_t* feasible, double* cost, double* coeffs, int32_t* iters, bool deferred,
                            int** d_win_idx, double** d_win_cost)
 {
-  HostLayout L;
+  FqSelectMultiArgs sa{};              // the solve's candidates and room for the winners, in the context's arenas
   int rc = solve_multi_impl(ctx, N, force_final, n_prob, x0, xf, lim, poly_ofs, face_ofs, Ab, cand_ofs, dt, sigma, feasible, cost,
-                            coeffs, iters, true, &L);
+                            coeffs, iters, true, &sa);
   if (rc) return rc;
   if (cand_ofs[n_prob] == 0) return fq_fail(ctx, FQ_E_ARG, "no candidates");
   FQ_CUDA(cudaSetDevice(ctx->device));
   // slices of a large batch alternate between the two streams: join before selecting
   FQ_CUDA(cudaEventRecord(ctx->ev_head, ctx->stream2));
   FQ_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_head, 0));
-  char* din = (char*)ctx->d_in.p;
-  char* dout = (char*)ctx->d_out.p;
-  FqSelectMultiArgs sa;
-  sa.n_prob = n_prob; sa.N = N; sa.n_sig = 0; sa.cand_ofs = (const int*)(din + L.cand_ofs); sa.dt = (const double*)(din + L.dt);
-  sa.sigma = nullptr; sa.feasible = (const uint8_t*)(dout + L.feasible); sa.cost = (const double*)(dout + L.cost);
-  sa.win_idx = (int*)(dout + L.win_idx); sa.win_cost = (double*)(dout + L.win_cost); sa.win_dt = (double*)(dout + L.win_dt);
-  sa.win_sigma = nullptr; sa.win_ofs = (int*)(dout + L.win_ofs);
+  sa.n_prob = n_prob; sa.N = N; sa.n_sig = 0; sa.sigma = nullptr; sa.win_sigma = nullptr;
   FQ_CUDA(fq_launch_select_multi(sa, ctx->stream));
   if (d_win_idx) *d_win_idx = sa.win_idx;
   if (d_win_cost) *d_win_cost = sa.win_cost;
@@ -583,40 +559,48 @@ int gen_new_traj_impl(fq_ctx* ctx, int N, int force_final, const double* x0, con
   if (P > 0 && fq_scan_max_u8(sigmas, (size_t)n_sigma * N) >= P) return fq_fail(ctx, FQ_E_ARG, "sigma entry >= number of polytopes");
   FQ_CUDA(cudaSetDevice(ctx->device));
   // ---- pack the (small) problem description; the dt x sigma grid is expanded on the host side of the copy
-  size_t o = 0;
-  const size_t oAb = o;   o = fq_align16(o + sizeof(double) * 4 * (size_t)(n_face > 0 ? n_face : 1));
-  const size_t ox0 = o;   o += sizeof(double) * 9;
-  const size_t oxf = o;   o += sizeof(double) * 9;
-  const size_t olim = o;  o += sizeof(double) * 3;
-  const size_t odt = o;   o += sizeof(double) * (size_t)n_cand;
-  const size_t opo = o;   o += sizeof(int) * 2;
-  const size_t ofo = o;   o += sizeof(int) * (size_t)(P + 1);
-  const size_t oco = o;   o += sizeof(int) * 2;
-  const size_t osig = o;  o = fq_align16(o + (size_t)n_cand * N);
-  const size_t odts = o;  o += sizeof(double) * (size_t)n_dt;      // the n_dt distinct time allocations (for fillX)
-  const size_t in_bytes = fq_align16(o);
-  o = 0;
-  const size_t ocost = o;   o += sizeof(double) * (size_t)n_cand;
-  const size_t ocoef = o;   o += sizeof(double) * 12 * (size_t)N * n_cand;
-  const size_t owin = o;    o += sizeof(double) * (1 + 12 * (size_t)N);     // winner: cost + coeffs
-  const size_t oidx = o;    o += sizeof(int) * 2;
-  const size_t onsamp = o;  o += sizeof(int) * 2;
-  const size_t osamp = o;   o += samples ? sizeof(double) * 12 * (size_t)max_samples : 0;
-  const size_t ofeas = o;   o += (size_t)n_cand;
-  const size_t out_bytes = fq_align16(o);
-  FQ_CUDA(ctx->d_in.reserve(in_bytes));
-  FQ_CUDA(ctx->d_out.reserve(out_bytes));
-  FQ_CUDA(ctx->h_in.reserve(in_bytes));
-  FQ_CUDA(ctx->h_out.reserve(sizeof(double) * (1 + 12 * (size_t)N) + 4 * sizeof(int) +
-                             (samples ? sizeof(double) * 12 * (size_t)max_samples : 0)));
-  char* hi = (char*)ctx->h_in.p;
-  if (n_face) std::memcpy(hi + oAb, Ab, sizeof(double) * 4 * (size_t)n_face);
-  std::memcpy(hi + ox0, x0, sizeof(double) * 9);
-  std::memcpy(hi + oxf, xf, sizeof(double) * 9);
-  std::memcpy(hi + olim, lim, sizeof(double) * 3);
+  const int cand_ofs[2] = { 0, n_cand };
+  FqKernelArgs a{};
+  a.N = N; a.force_final = force_final; a.n_prob = 1; a.max_faces = n_face;
+  int* d_fo = nullptr;
+  double *d_dt = nullptr, *d_dts = nullptr;
+  uint8_t* d_sig = nullptr;
+  auto layout_in = [&](FqPack& p) {
+    a.Ab = n_face > 0 ? p.in(Ab, 4 * (size_t)n_face) : p.scratch<double>(0);
+    a.x0 = p.in(x0, 9);  a.xf = p.in(xf, 9);  a.lim = p.in(lim, 3);
+    a.poly_ofs = p.in(poly_ofs, 2);  a.cand_ofs = p.in(cand_ofs, 2);
+    a.face_ofs = d_fo = p.scratch<int>(P + 1);
+    a.dt = d_dt = p.scratch<double>(n_cand);  a.sigma = d_sig = p.scratch<uint8_t>((size_t)n_cand * N);
+    d_dts = p.in(dts, n_dt);                                 // the n_dt distinct time allocations (for fillX)
+  };
+  // the winner record is one block at fixed spacing: cost, 12 N coefficients, two indices, two sample counts, then the
+  // samples.  The kernel's tail writes it through h_out's device address, one copy brings it back otherwise, and the host
+  // reads it at the same spacing, so it is packed whole: 8 (1 + 12 N) is not a multiple of 16, and aligning the indices
+  // apart would move them.
+  const size_t win_bytes = sizeof(double) * (1 + 12 * (size_t)N);
+  const size_t rec_bytes = win_bytes + 4 * sizeof(int) + (samples ? sizeof(double) * 12 * (size_t)max_samples : 0);
+  char* rec = nullptr;
+  auto layout_out = [&](FqPack& p) {
+    a.cost = p.scratch<double>(n_cand);  a.coeffs = p.scratch<double>(12 * (size_t)N * n_cand);
+    rec = p.scratch<char>(rec_bytes);
+    a.feasible = p.scratch<uint8_t>(n_cand);
+  };
+  FqPack in, out;
+  layout_in(in);
+  layout_out(out);
+  FQ_CUDA(ctx->d_in.reserve(in.at));
+  FQ_CUDA(ctx->d_out.reserve(out.at));
+  FQ_CUDA(ctx->h_in.reserve(in.at));
+  FQ_CUDA(ctx->h_out.reserve(rec_bytes));
+  in = in.place(ctx->d_in.p, ctx->h_in.p);
+  layout_in(in);
+  out = out.place(ctx->d_out.p);
+  layout_out(out);
+  if (int prc = in.done(ctx)) return prc;
+  if (int prc = out.done(ctx)) return prc;
   {
-    double* hd = (double*)(hi + odt);
-    uint8_t* hs = (uint8_t*)(hi + osig);
+    double* hd = in.mirror(d_dt);
+    uint8_t* hs = in.mirror(d_sig);
     for (int d = 0; d < n_dt; d++)
       for (int s = 0; s < n_sigma; s++)
       {
@@ -624,33 +608,21 @@ int gen_new_traj_impl(fq_ctx* ctx, int N, int force_final, const double* x0, con
         if (P > 0) std::memcpy(hs + ((size_t)d * n_sigma + s) * N, sigmas + (size_t)s * N, N);
         else std::memset(hs + ((size_t)d * n_sigma + s) * N, 0, N);
       }
-    std::memcpy(hi + odts, dts, sizeof(double) * (size_t)n_dt);
-    int* po = (int*)(hi + opo); po[0] = 0; po[1] = P;
-    int* fo = (int*)(hi + ofo); fo[0] = 0; for (int p = 0; p < P; p++) fo[p + 1] = face_ofs[p + 1];
-    int* co = (int*)(hi + oco); co[0] = 0; co[1] = n_cand;
+    int* fo = in.mirror(d_fo); fo[0] = 0; for (int p = 0; p < P; p++) fo[p + 1] = face_ofs[p + 1];
   }
   tr.mark("pack");
   cudaStream_t st = ctx->stream;
-  char* din = (char*)ctx->d_in.p;
-  char* dout = (char*)ctx->d_out.p;
   cudaEvent_t tev[5] = { nullptr, nullptr, nullptr, nullptr, nullptr };      // FQ_TRACE: device-side phase times
   if (tr.on)
     for (auto& e : tev) cudaEventCreate(&e);
   if (tr.on) cudaEventRecord(tev[0], st);
-  FQ_CUDA(cudaMemcpyAsync(din, hi, in_bytes, cudaMemcpyHostToDevice, st));
+  FQ_CUDA(cudaMemcpyAsync(in.base, in.host, in.at, cudaMemcpyHostToDevice, st));
   if (tr.on) cudaEventRecord(tev[1], st);
-  FqKernelArgs a{};
-  a.N = N; a.force_final = force_final; a.n_prob = 1;
-  a.x0 = (const double*)(din + ox0); a.xf = (const double*)(din + oxf); a.lim = (const double*)(din + olim);
-  a.poly_ofs = (const int*)(din + opo); a.face_ofs = (const int*)(din + ofo); a.Ab = (const double*)(din + oAb);
-  a.max_faces = n_face; a.cand_ofs = (const int*)(din + oco); a.dt = (const double*)(din + odt);
-  a.sigma = (const uint8_t*)(din + osig); a.feasible = (uint8_t*)(dout + ofeas); a.cost = (double*)(dout + ocost);
-  a.coeffs = (double*)(dout + ocoef);
   a.sorted_dt = 1;
   for (int d = 1; d < n_dt; d++) a.sorted_dt = a.sorted_dt && dts[d] >= dts[d - 1];
   a.ee_width = a.sorted_dt ? n_sigma : 0;
   char* ho = (char*)ctx->h_out.p;
-  const size_t win_bytes = sizeof(double) * (1 + 12 * (size_t)N);
+  int* rec_idx = (int*)(rec + win_bytes);
   if (!samples)
   { // the last warp to finish selects the winner and writes the record (cost, coefficients, indices) into this pinned,
     // device-visible host buffer: no selection launch and no device-to-host copy on the latency path
@@ -670,23 +642,20 @@ int gen_new_traj_impl(fq_ctx* ctx, int N, int force_final, const double* x0, con
   if (rc) return rc;
   if (tr.on) cudaEventRecord(tev[2], st);
   FqSelectArgs sa;
-  sa.n_dt = n_dt; sa.n_sigma = n_sigma; sa.N = N;
-  sa.feasible = (const uint8_t*)(dout + ofeas); sa.cost = (const double*)(dout + ocost);
-  sa.coeffs = (const double*)(dout + ocoef);
-  sa.out_idx = (int*)(dout + oidx); sa.out_cost = (double*)(dout + owin); sa.out_coeffs = (double*)(dout + owin) + 1;
+  sa.n_dt = n_dt; sa.n_sigma = n_sigma; sa.N = N; sa.feasible = a.feasible; sa.cost = a.cost; sa.coeffs = a.coeffs;
+  sa.out_idx = rec_idx; sa.out_cost = (double*)rec; sa.out_coeffs = (double*)rec + 1;
   if (!tail) FQ_CUDA(fq_launch_select(sa, st));
   size_t tail_bytes = 2 * sizeof(int);
   if (samples)
   { // fillX on the device, chained on the same stream; samples travel back with the winner record
     FqFillArgs fa;
-    fa.N = N; fa.n_dt = n_dt; fa.max_samples = max_samples; fa.DC = DC;
-    fa.dts = (const double*)(din + odts); fa.win_idx = (const int*)(dout + oidx);
-    fa.coeffs = (const double*)(dout + owin) + 1; fa.out = (double*)(dout + osamp); fa.n_samples = (int*)(dout + onsamp);
+    fa.N = N; fa.n_dt = n_dt; fa.max_samples = max_samples; fa.DC = DC; fa.dts = d_dts; fa.win_idx = rec_idx;
+    fa.coeffs = (const double*)rec + 1; fa.out = (double*)(rec + win_bytes + 4 * sizeof(int)); fa.n_samples = rec_idx + 2;
     FQ_CUDA(fq_launch_fill(fa, st));
     tail_bytes = 4 * sizeof(int) + sizeof(double) * 12 * (size_t)max_samples;
   }
   if (tr.on) cudaEventRecord(tev[3], st);
-  if (!tail) FQ_CUDA(cudaMemcpyAsync(ho, dout + owin, win_bytes + tail_bytes, cudaMemcpyDeviceToHost, st));
+  if (!tail) FQ_CUDA(cudaMemcpyAsync(ho, rec, win_bytes + tail_bytes, cudaMemcpyDeviceToHost, st));
   if (tr.on) cudaEventRecord(tev[4], st);
   tr.mark("enqueue");
   FQ_CUDA(cudaStreamSynchronize(st));
@@ -795,34 +764,30 @@ extern "C" int fq_gen_new_traj_exact(fq_ctx* ctx, int N, int force_final, const 
   int win_dt = -1;
   if (exact)
   {
-    // ---- 2. device buffers
+    // ---- 2. device buffers: only the head is staged and uploaded; the leaves and both node pools stay on the device
     const int cap = 65536, leaf_cap = 4096;
-    size_t o = 0;
-    const size_t oAb = o;    o = fq_align16(o + sizeof(double) * 4 * (size_t)n_face);
-    const size_t ox0 = o;    o += sizeof(double) * 9;
-    const size_t oxf = o;    o += sizeof(double) * 9;
-    const size_t olim = o;   o += sizeof(double) * 3;
-    const size_t odts = o;   o += sizeof(double) * (size_t)n_dt;
-    const size_t oinc = o;   o += sizeof(unsigned long long) * (size_t)n_dt;
-    const size_t opo = o;    o += sizeof(int) * 2;
-    const size_t ofo = o;    o += sizeof(int) * (size_t)(P + 1);
-    const size_t oroot = o;  o += sizeof(int) * (size_t)n_dt;
-    const size_t ocnt = o;   o = fq_align16(o + sizeof(int) * 8);   // [0..1] parents of even / odd levels [2] n_leaves [3..4] flags
-    const size_t head = o;
-    const size_t oleaf = o;  o = fq_align16(o + 32 * (size_t)leaf_cap);
-    const size_t opoolA = o; o = fq_align16(o + nb * (size_t)cap);
-    const size_t opoolB = o; o = fq_align16(o + nb * (size_t)cap);
+    FqBnbLevel L{};
+    int *d_roots = nullptr, *d_cnt = nullptr;       // d_cnt: [0..1] parents of even / odd levels [2] n_leaves [3..4] flags
+    unsigned char* pools[2] = { nullptr, nullptr };
+    size_t head = 0;
+    auto layout = [&](FqPack& p) {
+      L.k.Ab = p.in(Ab, 4 * (size_t)n_face);  L.k.x0 = p.in(x0, 9);  L.k.xf = p.in(xf, 9);  L.k.lim = p.in(lim, 3);
+      L.dts = p.in(dts, n_dt);  L.incumbent = p.scratch<unsigned long long>(n_dt);
+      L.k.poly_ofs = p.in(poly_ofs, 2);  L.k.face_ofs = p.in(face_ofs, P + 1);
+      L.roots = d_roots = p.scratch<int>(n_dt);  d_cnt = p.scratch<int>(8);
+      head = p.at;
+      L.leaves = p.scratch<char>(32 * (size_t)leaf_cap);
+      pools[0] = p.scratch<unsigned char>(nb * (size_t)cap);  pools[1] = p.scratch<unsigned char>(nb * (size_t)cap);
+    };
+    FqPack pk;
+    layout(pk);
     FQ_CUDA(cudaSetDevice(ctx->device));
-    FQ_CUDA(ctx->d_bnb.reserve(o));
+    FQ_CUDA(ctx->d_bnb.reserve(pk.at));
     FQ_CUDA(ctx->h_in.reserve(head));
-    char* hi = (char*)ctx->h_in.p;
-    char* db = (char*)ctx->d_bnb.p;
-    std::memset(hi, 0, head);
-    std::memcpy(hi + oAb, Ab, sizeof(double) * 4 * (size_t)n_face);
-    std::memcpy(hi + ox0, x0, sizeof(double) * 9);
-    std::memcpy(hi + oxf, xf, sizeof(double) * 9);
-    std::memcpy(hi + olim, lim, sizeof(double) * 3);
-    std::memcpy(hi + odts, dts, sizeof(double) * (size_t)n_dt);
+    std::memset(ctx->h_in.p, 0, head);             // the counters go up zeroed, apart from n_roots
+    pk = pk.place(ctx->d_bnb.p, ctx->h_in.p);
+    layout(pk);
+    if (int prc = pk.done(ctx)) return prc;
     // presolve (fq_presolve.h): time allocations at which no assignment can be feasible get no root
     int n_roots = 0;
     for (int d = 0; d < n_dt; d++)
@@ -830,43 +795,36 @@ extern "C" int fq_gen_new_traj_exact(fq_ctx* ctx, int N, int force_final, const 
       unsigned long long bits;
       const double c = best[d];
       std::memcpy(&bits, &c, 8);
-      ((unsigned long long*)(hi + oinc))[d] = bits;              // +inf orders above every finite cost
+      pk.mirror(L.incumbent)[d] = bits;          // the incumbent holds best[]'s bit patterns: +inf orders above every finite cost
       if (d >= n_search) continue;
       const bool possible = fqs::root_possible(P, face_ofs, Ab, x0, xf, force_final, dts[d], ctx->row_tol);
-      if (possible) ((int*)(hi + oroot))[n_roots++] = d;
+      if (possible) pk.mirror(d_roots)[n_roots++] = d;
     }
-    ((int*)(hi + ocnt))[0] = n_roots;
-    ((int*)(hi + opo))[0] = 0; ((int*)(hi + opo))[1] = P;
-    for (int p = 0; p <= P; p++) ((int*)(hi + ofo))[p] = face_ofs[p];
+    pk.mirror(d_cnt)[0] = n_roots;
     cudaStream_t st = ctx->stream;
-    FQ_CUDA(cudaMemcpyAsync(db, hi, head, cudaMemcpyHostToDevice, st));
+    FQ_CUDA(cudaMemcpyAsync(pk.base, pk.host, head, cudaMemcpyHostToDevice, st));
     FqPlanDev* pd = nullptr;
     rc = fq_get_plan(ctx, N, force_final, &pd);
     if (rc) return rc;
-    FqBnbLevel L{};
     fq_fill_plan_args(*pd, &L.k);
-    L.k.n_prob = 1; L.k.x0 = (const double*)(db + ox0); L.k.xf = (const double*)(db + oxf); L.k.lim = (const double*)(db + olim);
-    L.k.poly_ofs = (const int*)(db + opo); L.k.face_ofs = (const int*)(db + ofo); L.k.Ab = (const double*)(db + oAb);
-    L.k.max_faces = n_face; L.k.item_cap = N * cs.max_poly_faces; L.k.row_tol = ctx->row_tol;
-    L.n_dt = n_dt; L.dts = (const double*)(db + odts); L.roots = (const int*)(db + oroot);
-    L.incumbent = (unsigned long long*)(db + oinc); L.leaves = db + oleaf; L.n_leaves = (int*)(db + ocnt) + 2;
-    L.leaf_cap = leaf_cap; L.flags = (int*)(db + ocnt) + 3; L.cap = cap; L.nodes = nullptr; L.keep_ties = 0;
+    L.k.n_prob = 1; L.k.max_faces = n_face; L.k.item_cap = N * cs.max_poly_faces; L.k.row_tol = ctx->row_tol;
+    L.n_dt = n_dt; L.n_leaves = d_cnt + 2; L.leaf_cap = leaf_cap; L.flags = d_cnt + 3; L.cap = cap; L.nodes = nullptr;
+    L.keep_ties = 0;
     int n_par = n_roots;
     long nodes = 0;
-    unsigned char* pools[2] = { (unsigned char*)(db + opoolA), (unsigned char*)(db + opoolB) };
     int cnt[5] = { 0, 0, 0, 0, 0 };
     // one corridor, one warp per child.  The levels are driven from the host: it sizes each launch to the level's
     // children and stops at the first cut, which keeps this sweep's node counts and costs as they were
     for (int depth = 0; depth < N && n_par > 0; depth++)
     {
       L.depth = depth; L.cpc = (int)(((long long)n_par * P + FQ_WARPS_PER_CTA - 1) / FQ_WARPS_PER_CTA);
-      L.n_parents = (int*)(db + ocnt) + (depth & 1); L.n_children = (int*)(db + ocnt) + ((depth + 1) & 1);
+      L.n_parents = d_cnt + (depth & 1); L.n_children = d_cnt + ((depth + 1) & 1);
       L.parents = pools[depth & 1]; L.children = pools[(depth + 1) & 1];
       FQ_CUDA(cudaMemsetAsync(L.n_children, 0, sizeof(int), st));
       cudaError_t e = fq_launch_bnb_level(L, st);
       if (e == cudaErrorInvalidConfiguration) { exact = false; break; }
       FQ_CUDA(e);
-      FQ_CUDA(cudaMemcpyAsync(cnt, db + ocnt, sizeof(cnt), cudaMemcpyDeviceToHost, st));
+      FQ_CUDA(cudaMemcpyAsync(cnt, d_cnt, sizeof(cnt), cudaMemcpyDeviceToHost, st));
       FQ_CUDA(cudaStreamSynchronize(st));
       nodes += (long)n_par * P;
       if (cnt[3]) { exact = false; break; }                      // pool overflow: the tree was cut
@@ -881,8 +839,8 @@ extern "C" int fq_gen_new_traj_exact(fq_ctx* ctx, int N, int force_final, const 
       struct Leaf { int dt_idx, pad; double cost; unsigned char sigma[16]; };
       std::vector<Leaf> leaves((size_t)std::max(n_leaves, 1));
       std::vector<unsigned long long> inc(n_dt);
-      if (n_leaves) FQ_CUDA(cudaMemcpyAsync(leaves.data(), db + oleaf, sizeof(Leaf) * (size_t)n_leaves, cudaMemcpyDeviceToHost, st));
-      FQ_CUDA(cudaMemcpyAsync(inc.data(), db + oinc, sizeof(unsigned long long) * (size_t)n_dt, cudaMemcpyDeviceToHost, st));
+      if (n_leaves) FQ_CUDA(cudaMemcpyAsync(leaves.data(), L.leaves, sizeof(Leaf) * (size_t)n_leaves, cudaMemcpyDeviceToHost, st));
+      FQ_CUDA(cudaMemcpyAsync(inc.data(), L.incumbent, sizeof(unsigned long long) * (size_t)n_dt, cudaMemcpyDeviceToHost, st));
       FQ_CUDA(cudaStreamSynchronize(st));
       for (int d = 0; d < n_search && win_dt < 0; d++)
       {

@@ -5,6 +5,7 @@
 #include "fq_kernels.cuh"
 #include "fq_plan.h"
 
+#include <cstring>
 #include <map>
 #include <string>
 #include <vector>
@@ -15,39 +16,25 @@ struct FqPlanDev
   double *TZ = nullptr, *T0 = nullptr, *FT = nullptr;
 };
 
-struct FqArena
-{ // grow-only device buffer
+template <cudaError_t (*Alloc)(void**, size_t), cudaError_t (*Free)(void*)>
+struct FqGrowArena
+{ // grow-only buffer: device memory (FqArena) or pinned host memory (FqHostArena)
   void* p = nullptr;
   size_t cap = 0;
   cudaError_t reserve(size_t n)
   {
     if (n <= cap) return cudaSuccess;
-    if (p) cudaFree(p);
+    if (p) Free(p);
     p = nullptr; cap = 0;
     size_t want = n + n / 4 + 4096;
-    cudaError_t e = cudaMalloc(&p, want);
+    cudaError_t e = Alloc(&p, want);
     if (e == cudaSuccess) cap = want;
     return e;
   }
-  void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+  void release() { if (p) Free(p); p = nullptr; cap = 0; }
 };
-
-struct FqPinnedArena
-{
-  void* p = nullptr;
-  size_t cap = 0;
-  cudaError_t reserve(size_t n)
-  {
-    if (n <= cap) return cudaSuccess;
-    if (p) cudaFreeHost(p);
-    p = nullptr; cap = 0;
-    size_t want = n + n / 4 + 4096;
-    cudaError_t e = cudaMallocHost(&p, want);
-    if (e == cudaSuccess) cap = want;
-    return e;
-  }
-  void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
-};
+using FqArena = FqGrowArena<cudaMalloc, cudaFree>;
+using FqHostArena = FqGrowArena<cudaMallocHost, cudaFreeHost>;
 
 struct FqComm;                    // fq_multi.cu: NCCL communicator(s) of a context (loaded lazily with dlopen)
 
@@ -58,7 +45,7 @@ struct fq_ctx
   cudaEvent_t ev_head = nullptr;
   std::map<int, FqPlanDev> plans; // key N*2+force_final
   FqArena d_in, d_out, d_bnb, d_pair, d_pair_io;
-  FqPinnedArena h_in, h_out;
+  FqHostArena h_in, h_out;
   std::string err;
   bool force_generic = false;
   int sm_count = 0;
@@ -98,6 +85,55 @@ int fq_settle(fq_ctx* ctx);
 int fq_launch_solve_ctx(fq_ctx* ctx, FqKernelArgs a, int max_cand, int max_poly_faces, cudaStream_t stream, bool* tail = nullptr,
                         bool early_exit_ok = true);
 inline size_t fq_align16(size_t x) { return (x + 15) & ~(size_t)15; }
+// Places arrays in an arena, each on a 16-byte boundary (so that any of them can be read as double2).  A layout is one
+// piece of code run twice: over a default FqPack, the sizing pass, which only counts the bytes (`at`; its pointers are
+// NULL), and, once the arena holds that many, over place(), which returns typed pointers into the arena and copies every
+// input's host data into the arena's pinned host mirror or, without one, straight into the arena on `stream`.  done()
+// refuses a placement that did not end where the sizing pass did (nothing is copied past that end).
+struct FqPack
+{
+  char* base = nullptr;                 // the arena (nullptr: the sizing pass)
+  char* host = nullptr;                 // its pinned host mirror, or nullptr
+  cudaStream_t stream = nullptr;
+  size_t at = 0, sized = 0;             // bytes placed so far; bytes the sizing pass counted
+  cudaError_t err = cudaSuccess;        // the first direct upload that failed
+  FqPack place(void* arena, void* mirror = nullptr, cudaStream_t st = nullptr) const
+  {
+    FqPack p;
+    p.base = (char*)arena; p.host = (char*)mirror; p.stream = st; p.sized = at;
+    return p;
+  }
+  // room for count T (count 0 takes none: the pointer is not NULL, and is the next array's)
+  template <class T> T* scratch(size_t count)
+  {
+    T* r = base ? reinterpret_cast<T*>(base + at) : nullptr;
+    at = fq_align16(at + sizeof(T) * count);
+    return r;
+  }
+  // room for an output the caller wants (want == NULL: not wanted, NULL)
+  template <class T> T* out(T* want, size_t count) { return want ? scratch<T>(count) : nullptr; }
+  // the arena's copy of the input src (NULL: NULL)
+  template <class T> T* in(const T* src, size_t count)
+  {
+    if (!src) return nullptr;
+    const size_t o = at, bytes = sizeof(T) * count;
+    T* r = scratch<T>(count);
+    if (base && bytes && at <= sized)
+    {
+      if (host) std::memcpy(host + o, src, bytes);
+      else if (err == cudaSuccess) err = cudaMemcpyAsync(r, src, bytes, cudaMemcpyHostToDevice, stream);
+    }
+    return r;
+  }
+  // the host mirror's copy of the array at arena address p
+  template <class T> T* mirror(T* p) const { return reinterpret_cast<T*>(host + ((const char*)p - base)); }
+  int done(fq_ctx* ctx) const
+  {
+    if (at != sized) return fq_fail(ctx, FQ_E_CUDA, "internal: an arena layout placed another size than it reserved");
+    if (err != cudaSuccess) return fq_cuda_fail(ctx, err, "cudaMemcpyAsync (upload)");
+    return 0;
+  }
+};
 // corridors of n_prob problems (problem j: polytopes poly_ofs[j] .. poly_ofs[j+1]-1; polytope p: rows face_ofs[p] ..
 // face_ofs[p+1]-1 of Ab).  fq_scan_corridors checks that every polytope count is in 0..FQ_MAX_POLY and that face_ofs is
 // monotone, and returns why it refuses the description, or nullptr.  Entries that stage the arrays as given also

@@ -8,7 +8,6 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
-#include <type_traits>
 
 namespace
 {
@@ -200,7 +199,7 @@ int check_map(fq_ctx* ctx, const fq_pair_decomp* dc, const fq_pair_hr* hr, const
   return 0;
 }
 
-// the chain's intermediate arrays, carved from ctx->d_pair: those of both sweeps, and a SweepScratch per sweep
+// the chain's intermediate arrays, placed in ctx->d_pair: those of both sweeps, and a SweepScratch per sweep
 struct Shared
 {
   double *x0_safe, *re_cost;            // R, the safe sweep's start states; the winners' re-solves (costs and flags)
@@ -227,15 +226,7 @@ struct SweepScratch
   int* dc_face;
 };
 
-template <class T>
-T* carve(char*& p, size_t count)
-{
-  T* r = reinterpret_cast<T*>(p);
-  p += fq_align16(sizeof(T) * count);
-  return r;
-}
-
-// Exact stage (fq_replan_pairs_exact*): node pools, leaves and per-corridor tree state, carved from ctx->d_bnb.  Corridor c
+// Exact stage (fq_replan_pairs_exact*): node pools, leaves and per-corridor tree state, placed in ctx->d_bnb.  Corridor c
 // owns a slice of kTreeCap(n_prob) nodes in each of the two level pools (parents / children) and of kLeafCap leaves, so a
 // cut tree never takes room from another corridor.
 const int kLeafCap = 4096;
@@ -254,21 +245,19 @@ struct Tree
   unsigned char *pool0, *pool1;
 };
 
-size_t tree_layout(char* base, int n_prob, int stride, int max_N, size_t nb, Tree* t)
+void tree_layout(FqPack& p, int n_prob, int stride, int max_N, size_t nb, Tree* t)
 {
-  char* p = base;
   const size_t np = (size_t)n_prob, cells = np * (size_t)std::max(stride, 1);
-  t->dts = carve<double>(p, cells);  t->incumbent = carve<unsigned long long>(p, cells);  t->roots = carve<int>(p, cells);
-  t->lbound = carve<unsigned long long>(p, cells);  t->closed = carve<uint8_t>(p, cells);
-  t->keep_idx = carve<int>(p, np);  t->keep_cost = carve<double>(p, np);  t->keep_dt = carve<double>(p, np);
-  t->keep_sig = carve<uint8_t>(p, np * max_N);  t->redo_dt = carve<double>(p, np);  t->redo_coeffs = carve<double>(p, np * 12 * max_N);
-  t->n_par = carve<int>(p, 2 * np);  t->n_leaves = carve<int>(p, np);  t->flags = carve<int>(p, 2 * np);
-  t->nodes = carve<long long>(p, np);
-  t->status = carve<uint8_t>(p, np); t->changed_w = carve<uint8_t>(p, np);  t->changed_s = carve<uint8_t>(p, np);
-  t->leaves = carve<char>(p, np * kLeafCap * 32);
-  t->pool0 = carve<unsigned char>(p, np * tree_cap(n_prob) * nb);
-  t->pool1 = carve<unsigned char>(p, np * tree_cap(n_prob) * nb);
-  return (size_t)(p - base);
+  t->dts = p.scratch<double>(cells);  t->incumbent = p.scratch<unsigned long long>(cells);  t->roots = p.scratch<int>(cells);
+  t->lbound = p.scratch<unsigned long long>(cells);  t->closed = p.scratch<uint8_t>(cells);
+  t->keep_idx = p.scratch<int>(np);  t->keep_cost = p.scratch<double>(np);  t->keep_dt = p.scratch<double>(np);
+  t->keep_sig = p.scratch<uint8_t>(np * max_N);  t->redo_dt = p.scratch<double>(np);  t->redo_coeffs = p.scratch<double>(np * 12 * max_N);
+  t->n_par = p.scratch<int>(2 * np);  t->n_leaves = p.scratch<int>(np);  t->flags = p.scratch<int>(2 * np);
+  t->nodes = p.scratch<long long>(np);
+  t->status = p.scratch<uint8_t>(np); t->changed_w = p.scratch<uint8_t>(np);  t->changed_s = p.scratch<uint8_t>(np);
+  t->leaves = p.scratch<char>(np * kLeafCap * 32);
+  t->pool0 = p.scratch<unsigned char>(np * tree_cap(n_prob) * nb);
+  t->pool1 = p.scratch<unsigned char>(np * tree_cap(n_prob) * nb);
 }
 
 // One sweep's exact stage, enqueued on `st` after its selection: roots, N level launches (parent counts stay on the
@@ -341,32 +330,34 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
   }
   Shared sh;
   SweepScratch ss[2];
-  auto layout = [&](char* base) {
-    char* p = base;
-    sh.x0_safe = carve<double>(p, (size_t)9 * P);  sh.re_cost = carve<double>(p, P);  sh.re_feas = carve<uint8_t>(p, P);
-    sh.win_ofs = carve<int>(p, P + 1);  sh.n_samples = carve<int>(p, P);  sh.k_safe = carve<int>(p, P);
-    sh.hr_r = carve<int>(p, hr ? P : 0);  sh.hr_need = carve<uint8_t>(p, hr ? P : 0);
-    sh.dc_stage = carve<double>(p, dslots * dcap * 4);    sh.dc_stage_n = carve<int>(p, dslots);
-    sh.dc_spill = carve<double>(p, dslots * dspill * 4);  sh.dc_spill_flag = carve<uint8_t>(p, dslots * dspill);
-    sh.dc_spill_idx = carve<int>(p, mp ? dslots * dspill : 0);  sh.map_table = carve<const FqMapDev*>(p, mp ? mp->n_maps : 0);
+  auto layout = [&](FqPack& p) {
+    sh.x0_safe = p.scratch<double>((size_t)9 * P);  sh.re_cost = p.scratch<double>(P);  sh.re_feas = p.scratch<uint8_t>(P);
+    sh.win_ofs = p.scratch<int>(P + 1);  sh.n_samples = p.scratch<int>(P);  sh.k_safe = p.scratch<int>(P);
+    sh.hr_r = p.scratch<int>(hr ? P : 0);  sh.hr_need = p.scratch<uint8_t>(hr ? P : 0);
+    sh.dc_stage = p.scratch<double>(dslots * dcap * 4);    sh.dc_stage_n = p.scratch<int>(dslots);
+    sh.dc_spill = p.scratch<double>(dslots * dspill * 4);  sh.dc_spill_flag = p.scratch<uint8_t>(dslots * dspill);
+    sh.dc_spill_idx = p.scratch<int>(mp ? dslots * dspill : 0);  sh.map_table = p.scratch<const FqMapDev*>(mp ? mp->n_maps : 0);
     for (int i = 0; i < 2; i++)
     {
       const Sweep& w = sw[i];
       SweepScratch& s = ss[i];
       const size_t nc = (size_t)w.n_cand;
-      s.dt = carve<double>(p, nc);  s.cost = carve<double>(p, nc);  s.feas = carve<uint8_t>(p, nc);  s.sig = carve<uint8_t>(p, nc * w.N);
-      s.dt_base = carve<double>(p, P);  s.win_cost = carve<double>(p, P);  s.win_dt = carve<double>(p, P);
-      s.coeffs = carve<double>(p, (size_t)12 * w.N * P);
-      s.cand_ofs = carve<int>(p, P + 1);  s.win_idx = carve<int>(p, P);  s.win_sig = carve<uint8_t>(p, (size_t)P * w.N);
-      s.fac = carve<double>(p, win ? (size_t)P * w.max_fac : 0);  s.nf = carve<int>(p, win ? P : 0);
-      s.dc_Ab = carve<double>(p, dc && !w.Ab_out ? (size_t)P * w.max_faces * 4 : 0);
-      s.dc_face = carve<int>(p, dc && !w.face_ofs_out ? (size_t)P * w.max_poly + 1 : 0);
-      s.dc_xf = carve<double>(p, dc ? (size_t)9 * P : 0);
+      s.dt = p.scratch<double>(nc);  s.cost = p.scratch<double>(nc);  s.feas = p.scratch<uint8_t>(nc);  s.sig = p.scratch<uint8_t>(nc * w.N);
+      s.dt_base = p.scratch<double>(P);  s.win_cost = p.scratch<double>(P);  s.win_dt = p.scratch<double>(P);
+      s.coeffs = p.scratch<double>((size_t)12 * w.N * P);
+      s.cand_ofs = p.scratch<int>(P + 1);  s.win_idx = p.scratch<int>(P);  s.win_sig = p.scratch<uint8_t>((size_t)P * w.N);
+      s.fac = p.scratch<double>(win ? (size_t)P * w.max_fac : 0);  s.nf = p.scratch<int>(win ? P : 0);
+      s.dc_Ab = p.scratch<double>(dc && !w.Ab_out ? (size_t)P * w.max_faces * 4 : 0);
+      s.dc_face = p.scratch<int>(dc && !w.face_ofs_out ? (size_t)P * w.max_poly + 1 : 0);
+      s.dc_xf = p.scratch<double>(dc ? (size_t)9 * P : 0);
     }
-    return (size_t)(p - base);
   };
-  FQ_CUDA(ctx->d_pair.reserve(layout(nullptr)));   // grows only on the first call / a larger batch (synchronous cudaMalloc)
-  layout((char*)ctx->d_pair.p);
+  FqPack pk;
+  layout(pk);
+  FQ_CUDA(ctx->d_pair.reserve(pk.at));   // grows only on the first call / a larger batch (synchronous cudaMalloc)
+  pk = pk.place(ctx->d_pair.p);
+  layout(pk);
+  if (int rc = pk.done(ctx)) return rc;
   if (mp)
     for (int at = 0; at < mp->n_maps; at += FqMapTableChunk::kCap)
     {
@@ -381,8 +372,12 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
   { // the whole tree is done before the safe one starts: one pool serves both
     const int max_N = std::max(sw[0].N, sw[1].N);
     const size_t nb = std::max(fq_bnb_node_bytes(sw[0].N, sw[0].force_final), fq_bnb_node_bytes(sw[1].N, sw[1].force_final));
-    FQ_CUDA(ctx->d_bnb.reserve(tree_layout(nullptr, P, stride, max_N, nb, &tree)));
-    tree_layout((char*)ctx->d_bnb.p, P, stride, max_N, nb, &tree);
+    FqPack tp;
+    tree_layout(tp, P, stride, max_N, nb, &tree);
+    FQ_CUDA(ctx->d_bnb.reserve(tp.at));
+    tp = tp.place(ctx->d_bnb.p);
+    tree_layout(tp, P, stride, max_N, nb, &tree);
+    if (int rc = tp.done(ctx)) return rc;
   }
 
   // One sweep from the start states x0: a decomposing chain's corridors (`first`: their vertex 0, NULL: the path's own),
@@ -832,8 +827,9 @@ int submit_host(fq_ctx* ctx, const Checked& k, const fq_pair_args* a, bool defer
   const FqCorridorSizes* cs = k.cs;
   const int* n_obs = k.n_obs;
   FQ_CUDA(cudaSetDevice(ctx->device));
-  // ---- one packed upload of the inputs and one block for the outputs.  stage() runs twice: to size them, then to copy
-  //      the inputs into the pinned staging buffer and point the device copies of the structs at both
+  // ---- one packed upload of the inputs (pi) and, after it in d_pair_io, one block for the outputs (po).  stage() runs
+  //      twice: to size them, then to copy the inputs into the pinned staging buffer and point the device copies of the
+  //      structs at both
   fq_pair_args d = *a;
   fq_pair_assign da{};
   fq_pair_window dw{};
@@ -844,21 +840,7 @@ int submit_host(fq_ctx* ctx, const Checked& k, const fq_pair_args* a, bool defer
   fq_pair_plan dp = pl ? *pl : fq_pair_plan{};
   if (as) da.all_limit = as->all_limit;
   Sweep dv[2];
-  char *hi = nullptr, *din = nullptr, *dout = nullptr;
-  size_t n_in = 0, n_out = 0;
-  auto in = [&](auto* src, size_t count) {        // the device copy of an input (NULL: none)
-    using T = std::remove_const_t<std::remove_pointer_t<decltype(src)>>;
-    const size_t at = n_in, bytes = sizeof(T) * count;
-    if (!src) return (T*)nullptr;
-    n_in = fq_align16(n_in + bytes);
-    if (hi && bytes) std::memcpy(hi + at, src, bytes);
-    return (T*)(din + at);
-  };
-  auto out = [&](auto* want, size_t count) {      // room for an output the caller wants (NULL: not wanted)
-    const size_t at = n_out;
-    if (want) n_out = fq_align16(n_out + sizeof(*want) * count);
-    return want ? (decltype(want))(dout + at) : nullptr;
-  };
+  FqPack pi, po;
   // f(the caller's array, its device copy, elements) for every output of sweep i
   auto each_output = [&](int i, auto&& f) {
     const Sweep& w = sw[i];
@@ -872,45 +854,44 @@ int submit_host(fq_ctx* ctx, const Checked& k, const fq_pair_args* a, bool defer
     f(w.pos_out, v.pos_out, 3 * P);  f(w.status, v.status, P);
   };
   auto stage = [&] {
-    n_in = n_out = 0;
-    d.x0 = in(a->x0, 9 * (size_t)P);
-    d.lim = in(a->lim, 3 * (size_t)P);
-    d.results = out(a->results, P);
-    if (dc) dd.goal = in(dc->goal, 3 * (size_t)P);
-    if (mp) dm.map_index = in(mp->map_index, P);
+    d.x0 = pi.in(a->x0, 9 * (size_t)P);
+    d.lim = pi.in(a->lim, 3 * (size_t)P);
+    d.results = po.out(a->results, P);
+    if (dc) dd.goal = pi.in(dc->goal, 3 * (size_t)P);
+    if (mp) dm.map_index = pi.in(mp->map_index, P);
     if (hr)
     { // last_factor_safe is updated in its uploaded copy, which goes back to the caller's array
-      dh.unk_ofs = in(hr->unk_ofs, P + 1);  dh.unk = in(hr->unk, 3 * (size_t)n_unk);
-      dh.last_factor_safe = in(hr->last_factor_safe, P);
-      dh.index_H = out(hr->index_H, P);  dh.need_safe = out(hr->need_safe, P);
+      dh.unk_ofs = pi.in(hr->unk_ofs, P + 1);  dh.unk = pi.in(hr->unk, 3 * (size_t)n_unk);
+      dh.last_factor_safe = pi.in(hr->last_factor_safe, P);
+      dh.index_H = po.out(hr->index_H, P);  dh.need_safe = po.out(hr->need_safe, P);
     }
     if (pl)
     {
-      dp.states = out(pl->states, 12 * (size_t)pl->cap_states);
-      dp.plan_ofs = out(pl->plan_ofs, P + 1);  dp.status = out(pl->status, P);
+      dp.states = po.out(pl->states, 12 * (size_t)pl->cap_states);
+      dp.plan_ofs = po.out(pl->plan_ofs, P + 1);  dp.status = po.out(pl->status, P);
     }
     for (int i = 0; i < 2; i++)
     {
       const Sweep& w = sw[i];
       Sweep& v = dv[i];
       v = w;
-      v.xf = in(w.xf, 9 * (size_t)P);  v.poly_ofs = in(w.poly_ofs, P + 1);  v.face_ofs = in(w.face_ofs, cs[i].n_poly + 1);
-      v.Ab = in(w.Ab, 4 * (size_t)cs[i].n_face);  v.factors = in(w.factors, w.n_fac);  v.sigmas = in(w.sigmas, (size_t)w.n_sig * w.N);
-      v.init = in(w.init, P);  v.final_ = in(w.final_, P);
-      v.path = in(w.path, 3 * (size_t)(cs[i].n_poly + P));  v.obs_ofs = in(w.obs_ofs, P + 1);  v.obs = in(w.obs, 3 * (size_t)n_obs[i]);
-      each_output(i, [&](auto* host, auto*& dev, size_t n) { dev = out(host, n); });
+      v.xf = pi.in(w.xf, 9 * (size_t)P);  v.poly_ofs = pi.in(w.poly_ofs, P + 1);  v.face_ofs = pi.in(w.face_ofs, cs[i].n_poly + 1);
+      v.Ab = pi.in(w.Ab, 4 * (size_t)cs[i].n_face);  v.factors = pi.in(w.factors, w.n_fac);  v.sigmas = pi.in(w.sigmas, (size_t)w.n_sig * w.N);
+      v.init = pi.in(w.init, P);  v.final_ = pi.in(w.final_, P);
+      v.path = pi.in(w.path, 3 * (size_t)(cs[i].n_poly + P));  v.obs_ofs = pi.in(w.obs_ofs, P + 1);  v.obs = pi.in(w.obs, 3 * (size_t)n_obs[i]);
+      each_output(i, [&](auto* host, auto*& dev, size_t n) { dev = po.out(host, n); });
     }
   };
   stage();
-  const size_t in_bytes = n_in;
-  FQ_CUDA(ctx->h_in.reserve(in_bytes));
-  FQ_CUDA(ctx->d_pair_io.reserve(in_bytes + n_out));
-  hi = (char*)ctx->h_in.p;
-  din = (char*)ctx->d_pair_io.p;
-  dout = din + in_bytes;
+  FQ_CUDA(ctx->h_in.reserve(pi.at));
+  FQ_CUDA(ctx->d_pair_io.reserve(pi.at + po.at));
+  pi = pi.place(ctx->d_pair_io.p, ctx->h_in.p);
+  po = po.place((char*)ctx->d_pair_io.p + pi.sized);
   stage();
+  if (int rc = pi.done(ctx)) return rc;
+  if (int rc = po.done(ctx)) return rc;
   cudaStream_t st = ctx->stream;
-  FQ_CUDA(cudaMemcpyAsync(din, hi, in_bytes, cudaMemcpyHostToDevice, st));
+  FQ_CUDA(cudaMemcpyAsync(pi.base, pi.host, pi.at, cudaMemcpyHostToDevice, st));
   for (int i = 0; i < 2; i++) put_sweep(dv[i], i, &d, &da, &dw, &dx, &dd);
   int rc = family_dev(ctx, &d, as ? &da : nullptr, win ? &dw : nullptr, ex ? &dx : nullptr, dc ? &dd : nullptr, hr ? &dh : nullptr,
                       mp ? &dm : nullptr, pl ? &dp : nullptr, nullptr, st);
