@@ -22,7 +22,8 @@ EXPORTS = ["fq_abi_version", "fq_create", "fq_destroy", "fq_last_error", "fq_set
            "fq_replan_pairs_hr_dev", "fq_map_create", "fq_map_destroy", "fq_map_update", "fq_map_update_dev", "fq_map_size",
            "fq_replan_pairs_map", "fq_replan_pairs_map_async", "fq_replan_pairs_map_dev", "fq_replan_pairs_plan",
            "fq_replan_pairs_plan_async", "fq_replan_pairs_plan_dev", "fq_map_paths", "fq_map_paths_dev", "fq_paths_cloud",
-           "fq_jps_in"]
+           "fq_jps_in", "fq_queue_reset", "fq_queue_reset_dev", "fq_queue_select", "fq_queue_select_dev", "fq_queue_pop",
+           "fq_queue_pop_dev", "fq_replan_pairs_queue", "fq_replan_pairs_queue_async", "fq_replan_pairs_queue_dev"]
 
 
 class FqError(RuntimeError):
@@ -122,6 +123,23 @@ PLAN_OK, PLAN_NONE, PLAN_CAPACITY = 0, 1, 2                             # FQ_PLA
 PLAN_KEYS = ["states", "plan_ofs", "status"]
 
 
+class Queue(C.Structure):
+    """fq_queue of include/faster_b200.h: n_rows planners' committed plans as rings of cap states; pointers as integers."""
+    _fields_ = [("states", C.c_void_p), ("head", C.c_void_p), ("size", C.c_void_p), ("n_rows", C.c_int), ("cap", C.c_int),
+                ("delta_t", C.c_int)]
+
+
+class PairQueue(C.Structure):
+    """fq_pair_queue of include/faster_b200.h: the rings a chained replan appends its pieces to."""
+    _fields_ = [("ring", Queue), ("rows", C.c_void_p), ("k_end", C.c_void_p), ("G_term", C.c_void_p), ("goal_radius", C.c_double),
+                ("status", C.c_void_p), ("goal_seen", C.c_void_p)]
+
+
+QUEUE_OK, QUEUE_NONE, QUEUE_PUBLISHED, QUEUE_CAPACITY, QUEUE_ROWS = 0, 1, 2, 3, 4   # FQ_QUEUE_*
+QUEUE_DELTA_T = 10                                                      # deltaT_, faster.hpp:131
+GOAL_RADIUS = 0.3                                                       # faster.yaml:6
+
+
 HR_OUT_KEYS = ["last_factor_safe", "index_H", "need_safe"]
 HR_DEFAULTS = dict(drone_radius=0.42, delta_a=0.5, delta_H=1.0)         # faster.yaml:7,35,36
 
@@ -204,6 +222,16 @@ def lib():
         L.fq_replan_pairs_plan.argtypes = L.fq_replan_pairs_map.argtypes + [C.POINTER(PairPlan)]
         L.fq_replan_pairs_plan_async.argtypes = L.fq_replan_pairs_plan.argtypes
         L.fq_replan_pairs_plan_dev.argtypes = L.fq_replan_pairs_plan.argtypes + [C.c_void_p, C.c_void_p]
+        L.fq_replan_pairs_queue.argtypes = L.fq_replan_pairs_map.argtypes + [C.POINTER(PairQueue)]
+        L.fq_replan_pairs_queue_async.argtypes = L.fq_replan_pairs_queue.argtypes
+        L.fq_replan_pairs_queue_dev.argtypes = L.fq_replan_pairs_queue.argtypes + [C.c_void_p, C.c_void_p]
+        Q = C.POINTER(Queue)
+        L.fq_queue_reset.argtypes = [Q, C.c_int, C.c_void_p, C.c_void_p]
+        L.fq_queue_reset_dev.argtypes = L.fq_queue_reset.argtypes + [C.c_void_p]
+        L.fq_queue_select.argtypes = [Q, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.fq_queue_select_dev.argtypes = L.fq_queue_select.argtypes + [C.c_void_p]
+        L.fq_queue_pop.argtypes = [Q, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+        L.fq_queue_pop_dev.argtypes = L.fq_queue_pop.argtypes + [C.c_void_p]
         L.fq_map_create.argtypes = [C.POINTER(C.c_void_p), C.c_int]
         L.fq_map_destroy.argtypes = [C.c_void_p]
         L.fq_map_destroy.restype = None
@@ -359,6 +387,104 @@ def plan_args(cap_states, out_ptrs):
     for k in PLAN_KEYS:
         setattr(s, k, out_ptrs.get(k) or None)
     return s
+
+
+def _addr(x, dtype=None, shape=None, what="array"):
+    """The address of a numpy array or torch tensor, an integer address as it is, None as None (NULL).  With dtype (a numpy
+    dtype name) the array must have that element type and be C-contiguous, and with shape that shape (None entries: any
+    extent): the queue arrays are read and written in place by address, so they cannot be converted."""
+    if x is None or isinstance(x, int):
+        return x or None
+    torch_like = hasattr(x, "data_ptr")
+    if dtype is not None:
+        got = str(x.dtype).replace("torch.", "")
+        contiguous = x.is_contiguous() if torch_like else x.flags.c_contiguous
+        if got != np.dtype(dtype).name or not contiguous:
+            raise ValueError("%s must be a C-contiguous %s array (got %s%s)" % (what, np.dtype(dtype).name, got,
+                                                                                "" if contiguous else ", not contiguous"))
+    if shape is not None:
+        sh = tuple(x.shape)
+        if len(sh) != len(shape) or any(w is not None and g != w for g, w in zip(sh, shape)):
+            raise ValueError("%s must have shape %s (got %s)" % (what, tuple("*" if w is None else w for w in shape), sh))
+    return x.data_ptr() if torch_like else x.ctypes.data
+
+
+def queue_new(n_rows, cap):
+    """Host ring arrays for n_rows planners of cap states each, every row empty: dict(states (n_rows x cap x 12), head, size
+    (int32)).  A device ring is the same arrays as torch tensors (float64 / int32)."""
+    return dict(states=np.zeros((n_rows, cap, 12)), head=np.zeros(n_rows, np.int32), size=np.zeros(n_rows, np.int32))
+
+
+def queue_args(ring, delta_t=QUEUE_DELTA_T):
+    """Queue over a ring dict (queue_new, or torch tensors of the same shapes and types: device addresses)."""
+    n_rows, cap = ring["states"].shape[:2]
+    return Queue(_addr(ring["states"], "float64", (None, None, 12), "ring states"), _addr(ring["head"], "int32", (n_rows,), "ring head"),
+                 _addr(ring["size"], "int32", (n_rows,), "ring size"), int(n_rows), int(cap), int(delta_t))
+
+
+def queue_deque(ring, r):
+    """Row r of a host ring as the states front to back (size x 12)."""
+    cap = ring["states"].shape[1]
+    return ring["states"][r][(ring["head"][r] + np.arange(ring["size"][r])) % cap]
+
+
+def _queue_call(name, *args):
+    rc = getattr(lib(), name)(*args)
+    if rc != 0:
+        raise FqError("%s failed (%d): %s" % (name, rc, lib().fq_last_error(None).decode()))
+
+
+def queue_reset(ring, pos, rows=None, delta_t=QUEUE_DELTA_T):
+    """fq_queue_reset on a host ring: row rows[j] (None: j) := [the state at pos[j] (n x 3)]."""
+    pos = np.ascontiguousarray(pos, np.float64).reshape(-1, 3)
+    rows = None if rows is None else np.ascontiguousarray(rows, np.int32)
+    _queue_call("fq_queue_reset", C.byref(queue_args(ring, delta_t)), len(pos), _addr(rows), pos.ctypes.data)
+
+
+def queue_select(ring, n, rows=None, delta_t=QUEUE_DELTA_T):
+    """fq_queue_select on a host ring for n corridors.  -> (x0 (n x 9), k_end (int32))."""
+    rows = None if rows is None else np.ascontiguousarray(rows, np.int32)
+    x0, k_end = np.zeros((n, 9)), np.zeros(n, np.int32)
+    _queue_call("fq_queue_select", C.byref(queue_args(ring, delta_t)), n, _addr(rows), x0.ctypes.data, k_end.ctypes.data)
+    return x0, k_end
+
+
+def queue_pop(ring, ticks, rows=None, max_ticks=None, goals=None):
+    """fq_queue_pop on a host ring: ticks[j] publications of corridor j.  -> goals (n x max_ticks x 12; slots past ticks[j]
+    keep what `goals` held, NaN by default)."""
+    ticks = np.ascontiguousarray(ticks, np.int32)
+    rows = None if rows is None else np.ascontiguousarray(rows, np.int32)
+    mt = int(ticks.max(initial=0)) if max_ticks is None else int(max_ticks)
+    if goals is None:
+        goals = np.full((len(ticks), mt, 12), np.nan)
+    _queue_call("fq_queue_pop", C.byref(queue_args(ring)), len(ticks), _addr(rows), ticks.ctypes.data, mt,
+                _addr(goals, "float64", (len(ticks), mt, 12), "goals"))
+    return goals
+
+
+def queue_reset_dev(q, n, rows, pos, stream=0):
+    """fq_queue_reset_dev: q a Queue of device addresses; rows / pos device tensors or addresses (rows may be None)."""
+    _queue_call("fq_queue_reset_dev", C.byref(q), int(n), _addr(rows, "int32", (n,), "rows"), _addr(pos, "float64", (n, 3), "pos"),
+                stream or None)
+
+
+def queue_select_dev(q, n, rows, x0, k_end, stream=0):
+    """fq_queue_select_dev into the device arrays x0 (n x 9) and k_end (n, int32)."""
+    _queue_call("fq_queue_select_dev", C.byref(q), int(n), _addr(rows, "int32", (n,), "rows"), _addr(x0, "float64", (n, 9), "x0"),
+                _addr(k_end, "int32", (n,), "k_end"), stream or None)
+
+
+def queue_pop_dev(q, n, rows, ticks, max_ticks, goals, stream=0):
+    """fq_queue_pop_dev into the device array goals (n x max_ticks x 12)."""
+    _queue_call("fq_queue_pop_dev", C.byref(q), int(n), _addr(rows, "int32", (n,), "rows"), _addr(ticks, "int32", (n,), "ticks"),
+                int(max_ticks), _addr(goals, "float64", (n, max_ticks, 12), "goals"), stream or None)
+
+
+def pair_queue_args(q, rows, k_end, status, goal_seen=None, G_term=None, goal_radius=GOAL_RADIUS):
+    """PairQueue over the Queue q; the arrays are numpy arrays (host entry) or device tensors / addresses (_dev entry)."""
+    n = None if isinstance(k_end, int) else len(k_end)
+    return PairQueue(q, _addr(rows, "int32", (n,), "rows"), _addr(k_end, "int32", (n,), "k_end"), _addr(G_term, "float64", (n, 3), "G_term"),
+                     float(goal_radius), _addr(status, "int32", (n,), "status"), _addr(goal_seen, "uint8", (n,), "goal_seen"))
 
 
 def map_args(maps, map_index=None, max_local=4096):
@@ -735,12 +861,13 @@ class Solver:
 
     def _submit(self, family, deferred, structs, plan):
         """The host entry fq_replan_pairs<family> (sync or async) with `structs` (ctypes references or None, in its argument
-        order), or, given a PairPlan, fq_replan_pairs_plan with the same structs and the plan."""
+        order), or, given a PairPlan (PairQueue), fq_replan_pairs_plan (_queue) with the same structs and the plan."""
         if plan is None:
             fn = getattr(self._L, "fq_replan_pairs" + family + ("_async" if deferred else ""))
             self._check(fn(self._h, *structs))
         else:
-            fn = self._L.fq_replan_pairs_plan_async if deferred else self._L.fq_replan_pairs_plan
+            kind = "_queue" if isinstance(plan, PairQueue) else "_plan"
+            fn = getattr(self._L, "fq_replan_pairs" + kind + ("_async" if deferred else ""))
             self._check(fn(self._h, *(list(structs) + [None] * (7 - len(structs))), C.byref(plan)))
 
     def replan_pairs_plan(self, w, cap_states, chain="assign", *args, **kw):
@@ -763,6 +890,33 @@ class Solver:
         B = lambda x: C.byref(x) if x is not None else None  # noqa: E731
         self._check(self._L.fq_replan_pairs_plan_dev(self._h, C.byref(a), B(s), B(win), B(ex), B(dc), B(hr), B(mp), C.byref(plan),
                                                      results_all or None, stream or None))
+
+    def replan_pairs_queue(self, w, ring, k_end, chain="assign", *args, rows=None, G_term=None, goal_radius=GOAL_RADIUS,
+                           delta_t=QUEUE_DELTA_T, **kw):
+        """fq_replan_pairs_queue: the chained replan `chain` (as replan_pairs_plan takes it, with `args` / `kw`), whose pieces
+        are appended to the host ring `ring` (queue_new) as appendToPlan does.  w["x0"] should be queue_select's x0 and
+        k_end its k_end (updated in place: -1 after the call, as are the ring's arrays).  -> that method's dict plus
+        queue_status (int32, QUEUE_*) and goal_seen (uint8).  With deferred=True they are valid after wait()."""
+        n = w["n_prob"]
+        _addr(k_end, "int32", (n,), "k_end")                 # in/out: not converted, so checked
+        qo = dict(queue_status=np.zeros(n, np.int32), goal_seen=np.zeros(n, np.uint8))
+        rows = None if rows is None else np.ascontiguousarray(rows, np.int32)
+        G = None if G_term is None else np.ascontiguousarray(G_term, np.float64).reshape(n, 3)
+        pq = pair_queue_args(queue_args(ring, delta_t), rows, k_end, qo["queue_status"], qo["goal_seen"], G, goal_radius)
+        pq.keep = (rows, G)                     # what pq points to, alive as long as pq
+        fam = self.replan_pairs if chain == "shared" else getattr(self, "replan_pairs_" + chain)
+        out = fam(w, *args, plan=pq, **kw)
+        out.update(qo)
+        if kw.get("deferred"):
+            out["_keep_queue"] = pq
+        return out
+
+    def replan_pairs_queue_dev(self, a, s, win, ex, dc, hr, mp, q, results_all=0, stream=0):
+        """fq_replan_pairs_queue_dev: the structs of the selected family's _dev entry (as replan_pairs_plan_dev), with `q`
+        (PairQueue, pair_queue_args) holding device addresses."""
+        B = lambda x: C.byref(x) if x is not None else None  # noqa: E731
+        self._check(self._L.fq_replan_pairs_queue_dev(self._h, C.byref(a), B(s), B(win), B(ex), B(dc), B(hr), B(mp), C.byref(q),
+                                                      results_all or None, stream or None))
 
     def _list_outputs(self, w, all_limit, windows, inc, gamma, want_candidates, want_coeffs, extra=()):
         """What the per-corridor-list entries share: each sweep's candidate offsets, from the factors_* of `w` or from

@@ -788,6 +788,34 @@ cudaError_t fq_launch_pair_plan(const FqPairPlanArgs& a, cudaStream_t stream)
   return cudaGetLastError();
 }
 
+cudaError_t fq_launch_queue_reset(const FqQueueArgs& q, cudaStream_t stream)
+{
+  if (q.n <= 0) return cudaSuccess;
+  fqp::fq_queue_reset_kernel<<<(q.n + 127) / 128, 128, 0, stream>>>(q);
+  return cudaGetLastError();
+}
+
+cudaError_t fq_launch_queue_select(const FqQueueArgs& q, cudaStream_t stream)
+{
+  if (q.n <= 0) return cudaSuccess;
+  fqp::fq_queue_select_kernel<<<(q.n + 127) / 128, 128, 0, stream>>>(q);
+  return cudaGetLastError();
+}
+
+cudaError_t fq_launch_queue_pop(const FqQueueArgs& q, cudaStream_t stream)
+{
+  if (q.n <= 0) return cudaSuccess;
+  fqp::fq_queue_pop_kernel<<<(q.n + 127) / 128, 128, 0, stream>>>(q);
+  return cudaGetLastError();
+}
+
+cudaError_t fq_launch_pair_queue(const FqPairPlanArgs& a, const FqQueueArgs& q, cudaStream_t stream)
+{
+  if (a.n_prob <= 0) return cudaSuccess;
+  fqp::fq_pair_queue_kernel<<<a.n_prob, 128, 0, stream>>>(a, q);
+  return cudaGetLastError();
+}
+
 size_t fq_decomp_spill_n(int max_obs) { return max_obs > fqd::kFitPts ? (size_t)(max_obs - fqd::kFitPts) : 0; }
 
 cudaError_t fq_launch_decomp(const FqDecompArgs& a, cudaStream_t stream)

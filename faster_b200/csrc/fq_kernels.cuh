@@ -273,6 +273,9 @@ struct FqPairWindowArgs
   // NULL: every replan runs both sweeps.
   const uint8_t* need_safe = nullptr;
   double* last_factor_safe = nullptr;
+  // fq_replan_pairs_queue*: n_prob FQ_QUEUE_* statuses of the appends; a corridor whose append is not FQ_QUEUE_OK keeps its
+  // input windows (replan() returns before the update, faster.cpp:548-551).  NULL: no append gates the update.
+  const int* gate = nullptr;
 };
 
 // the plan piece of every corridor (fq_replan_pairs_plan*, fq_pair.cuh): whole samples 0 .. k_safe, then every safe sample,
@@ -292,6 +295,31 @@ struct FqPairPlanArgs
   int* status;                          // out n_prob (FQ_PLAN_*), or NULL
 };
 cudaError_t fq_launch_pair_plan(const FqPairPlanArgs& a, cudaStream_t stream);
+
+// the committed plans of fq_queue_* and fq_replan_pairs_queue* (fq_queue.h, fq_pair.cuh): n_rows rings of cap states;
+// corridor j works on row rows[j] (NULL: row j)
+struct FqQueueArgs
+{
+  int n, n_rows, cap, delta_t;
+  const int* rows;
+  double* states;                       // n_rows x cap x 12
+  int *head, *size;                     // n_rows
+  const double* pos;                    // reset: n x 3
+  double* x0;                           // select: out n x 9
+  int* k_end;                           // select: out n; append: in/out
+  const int* ticks;                     // pop: n
+  int max_ticks;
+  double* goals;                        // pop: out n x max_ticks x 12
+  const double* G_term;                 // append: n x 3, or NULL
+  double goal_radius;
+  int* status;                          // append: out n (FQ_QUEUE_*)
+  uint8_t* goal_seen;                   // append: out n, or NULL
+};
+cudaError_t fq_launch_queue_reset(const FqQueueArgs& q, cudaStream_t stream);
+cudaError_t fq_launch_queue_select(const FqQueueArgs& q, cudaStream_t stream);
+cudaError_t fq_launch_queue_pop(const FqQueueArgs& q, cudaStream_t stream);
+// appendToPlan of every corridor's piece (the FqPairPlanArgs of the chain, whose cap, states, plan_ofs and status are not read)
+cudaError_t fq_launch_pair_queue(const FqPairPlanArgs& a, const FqQueueArgs& q, cudaStream_t stream);
 
 // the device decomposition of one sweep's corridors (fq_decomp.cuh): fq_decomp_kernel stages every polytope's rows in a slot
 // of cap_pf rows (slot j * max_poly + s), fq_decomp_csr_kernel packs them into the sweep's CSR and sets the final states

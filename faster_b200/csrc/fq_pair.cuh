@@ -7,6 +7,7 @@
 #include "fq_assign.h"
 #include "fq_dtinit.h"
 #include "fq_paths.h"
+#include "fq_queue.h"
 #include "fq_window.h"
 
 namespace fqp
@@ -419,7 +420,8 @@ __global__ void fq_pair_final_kernel(const FqPairFinalArgs a)
   a.out[j] = r;
 }
 
-// factor_that_worked_, trials_ and the next windows of every corridor (fq_window.h), after fq_pair_final_kernel.  trials:
+// factor_that_worked_, trials_ and the next windows of every corridor (fq_window.h), after fq_pair_final_kernel (and with
+// a gate after fq_pair_queue_kernel, whose failed appends keep the input windows).  trials:
 // the winner's index in F_j + 1; |F_j| without a winner; 0 for a sweep that did not run (a safe sweep after a whole sweep
 // without winner, or a sweep the offsets kernel emptied).  Each thread reads its corridor's windows before it writes the
 // next ones, so those may alias.  With need_safe (fq_replan_pairs_hr*), a replan that needed no safe path ran no safe sweep
@@ -442,7 +444,7 @@ __global__ void fq_pair_window_kernel(const FqPairWindowArgs a)
   if (a.trials_w) a.trials_w[j] = !ran_w ? 0 : (dw >= 0 ? dw + 1 : a.n_fac_w[j]);
   if (a.trials_s) a.trials_s[j] = !ran_s ? 0 : (ds >= 0 ? ds + 1 : a.n_fac_s[j]);
   if (a.last_factor_safe && ds >= 0) a.last_factor_safe[j] = fs;
-  const bool both = dw >= 0 && (ds >= 0 || no_safe);
+  const bool both = dw >= 0 && (ds >= 0 || no_safe) && (!a.gate || a.gate[j] == FQ_QUEUE_OK);
   double ni, nf;
   fqw::next_window(both, fw, a.gamma_w, a.gammap_w, iw, ew, &ni, &nf);
   if (a.next_init_w) a.next_init_w[j] = ni;
@@ -525,5 +527,115 @@ __global__ void __launch_bounds__(128) fq_pair_plan_sample_kernel(const FqPairPl
     double* out = a.states + 12 * (size_t)(base + r);
     for (int q = 0; q < 12; q++) out[q] = o[q];
   }
+}
+
+// ---- each planner's committed plan kept on the device (fq_queue_*, fq_replan_pairs_queue*; the row operations are
+//      fq_queue.h's)
+
+// corridor j's row, or -1 when the device may not touch it: out of range, not a ring (unless `any`: reset makes one), or
+// (`unique`) named by another corridor as well
+FQ_HD int queue_row(const FqQueueArgs& q, int j, bool unique, bool any)
+{
+  const int r = q.rows ? q.rows[j] : j;
+  if (r < 0 || r >= q.n_rows || (!any && !fqq::ring_ok(q.head[r], q.size[r], q.cap))) return -1;
+  for (int i = 0; unique && q.rows && i < q.n; i++)
+    if (i != j && q.rows[i] == r) return -1;
+  return r;
+}
+
+FQ_HD double* queue_states(const FqQueueArgs& q, int r) { return q.states + (size_t)r * q.cap * fqq::kState; }
+
+// one thread per corridor
+__global__ void fq_queue_reset_kernel(const FqQueueArgs q)
+{
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= q.n) return;
+  const int r = queue_row(q, j, true, true);
+  if (r >= 0) fqq::reset(queue_states(q, r), q.head + r, q.size + r, q.pos + 3 * (size_t)j);
+}
+
+__global__ void fq_queue_select_kernel(const FqQueueArgs q)
+{
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= q.n) return;
+  const int r = queue_row(q, j, false, false);
+  q.k_end[j] = r < 0 ? fqq::select(nullptr, 0, 0, q.cap, q.delta_t, q.x0 + 9 * (size_t)j)
+                     : fqq::select(queue_states(q, r), q.head[r], q.size[r], q.cap, q.delta_t, q.x0 + 9 * (size_t)j);
+}
+
+__global__ void fq_queue_pop_kernel(const FqQueueArgs q)
+{
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= q.n) return;
+  const int r = queue_row(q, j, true, false);
+  const int t = q.ticks[j] < 0 ? 0 : q.ticks[j] > q.max_ticks ? q.max_ticks : q.ticks[j];
+  double* g = q.goals + (size_t)j * q.max_ticks * fqq::kState;
+  int head = 0, size = 0;
+  if (r < 0)
+  {
+    fqq::pop(nullptr, &head, &size, q.cap, t, g);
+    return;
+  }
+  head = q.head[r]; size = q.size[r];
+  fqq::pop(queue_states(q, r), &head, &size, q.cap, t, g);
+  q.head[r] = head; q.size[r] = size;
+}
+
+// appendToPlan (faster.cpp:606-648) of corridor j's piece onto its row, after the chain's records.  The piece is sampled
+// straight into the ring (plan_rows / sample_at, as fq_pair_plan_sample_kernel samples it): its length is known before a
+// row is sampled, so each row's decision needs nothing from any other corridor and no staging.  One CTA per corridor (any
+// block size): thread 0 decides, every thread samples a contiguous run of the piece, thread 0 then moves the row's size.
+__global__ void __launch_bounds__(128) fq_pair_queue_kernel(const FqPairPlanArgs a, const FqQueueArgs q)
+{
+  __shared__ int s_status;
+  __shared__ long long s_keep;
+  const int j = blockIdx.x;
+  if (j >= a.n_prob) return;
+  const int r = q.rows ? q.rows[j] : j;
+  int clash = 0;
+  for (int i = threadIdx.x; q.rows && i < a.n_prob; i += blockDim.x) clash |= i != j && q.rows[i] == r;
+  clash = __syncthreads_or(clash);
+  int k, ns;
+  const long long rows = plan_rows(a, j, &k, &ns);
+  if (threadIdx.x == 0)
+  {
+    long long keep = 0;
+    const bool mine = !clash && r >= 0 && r < q.n_rows && fqq::ring_ok(q.head[r], q.size[r], q.cap);
+    s_status = mine ? fqq::append_status(q.size[r], q.cap, q.k_end[j], rows, &keep) : FQ_QUEUE_ROWS;
+    s_keep = keep;
+  }
+  __syncthreads();
+  const int st = s_status;
+  const long long keep = s_keep;
+  if (st == FQ_QUEUE_OK)
+  {
+    double* row = queue_states(q, r);
+    const int head = q.head[r], nw = a.n_samples[j];
+    const long long per = (rows + blockDim.x - 1) / blockDim.x, r0 = per * threadIdx.x;
+    const long long r1 = r0 + per < rows ? r0 + per : rows;
+    const double* cw = a.coeffs_w + (size_t)j * a.N_w * 12;
+    const double* cs = a.coeffs_s + (size_t)j * a.N_s * 12;
+    SampleClock clock_w, clock_s;
+    for (long long i = r0; i < r1; i++)
+    {
+      double o[12];
+      if (i <= k) sample_at(clock_w, (int)i, cw, a.N_w, a.win_dt_w[j], a.DC, nw, o);
+      else sample_at(clock_s, (int)(i - k - 1), cs, a.N_s, a.win_dt_s[j], a.DC, ns, o);
+      double* out = row + fqq::kState * fqq::slot(head, keep + i, q.cap);
+      for (int c = 0; c < 12; c++) out[c] = o[c];
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  bool seen = false;
+  if (st == FQ_QUEUE_OK)
+  {
+    q.size[r] = (int)(keep + rows);
+    const double* last = queue_states(q, r) + fqq::kState * fqq::slot(q.head[r], keep + rows - 1, q.cap);
+    seen = q.G_term && fqq::goal_seen(last, q.G_term + 3 * (size_t)j, q.goal_radius);
+  }
+  q.k_end[j] = -1;
+  q.status[j] = st;
+  if (q.goal_seen) q.goal_seen[j] = seen;
 }
 }  // namespace fqp

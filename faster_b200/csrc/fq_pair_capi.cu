@@ -3,6 +3,7 @@
 // (safe).  Kernels: the batch solve (fq_kernels_t.cuh) and the small kernels of fq_pair.cuh.
 #include "fq_assign.h"
 #include "fq_ctx.h"
+#include "fq_queue.h"
 #include "fq_window.h"
 
 #include <algorithm>
@@ -316,7 +317,7 @@ long long longest_list(int N, int max_poly, long long all_limit)
 // the chain itself, every pointer a device pointer and every argument checked.  as == NULL: the shared lists of `a`;
 // sw: the two sweeps, their candidate counts set by the entry
 int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex,
-              const fq_pair_decomp* dc, const fq_pair_hr* hr, const fq_pair_map* mp, const fq_pair_plan* pl, const Sweep* sw,
+              const fq_pair_decomp* dc, const fq_pair_hr* hr, const fq_pair_map* mp, const fq_pair_plan* pl, const fq_pair_queue* qu, const Sweep* sw,
               fq_pair_result* results_all, cudaStream_t st)
 {
   const int P = a->n_prob;
@@ -483,7 +484,7 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
   }
   FQ_CUDA(fq_launch_pair_mid(m, st));
   // the safe winners' coefficients: wanted, or needed by the exact stage's confirmation or by the plan
-  double* coeffs_s = sw[1].coeffs ? sw[1].coeffs : ex || pl ? ss[1].coeffs : nullptr;
+  double* coeffs_s = sw[1].coeffs ? sw[1].coeffs : ex || pl || qu ? ss[1].coeffs : nullptr;
   if (int rc = run_sweep(sw[1], ss[1], sh.x0_safe, sh.x0_safe, coeffs_s, tree.changed_s, 1)) return rc;
 
   FqPairFinalArgs f;
@@ -507,6 +508,20 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
         FQ_CUDA(cudaMemcpyAsync(sw[i].cand_ofs_out, ss[i].cand_ofs, sizeof(int) * (size_t)(P + 1), cudaMemcpyDeviceToDevice, st));
   }
   FQ_CUDA(fq_launch_pair_final(f, st));
+  // the plan pieces (appendToPlan, faster.cpp:606-648) from the winners and k_safe
+  FqPairPlanArgs q;
+  q.n_prob = P; q.N_w = sw[0].N; q.N_s = sw[1].N; q.DC = a->DC;
+  q.win_idx_w = ss[0].win_idx; q.win_idx_s = ss[1].win_idx; q.win_dt_w = ss[0].win_dt; q.win_dt_s = ss[1].win_dt;
+  q.n_samples = sh.n_samples; q.k_safe = sh.k_safe; q.need = hr ? sh.hr_need : nullptr;
+  q.coeffs_w = coeffs_w; q.coeffs_s = coeffs_s;
+  if (qu)
+  { // ---- the pieces appended to the planners' plans; before the windows, whose update the appends gate
+    FqQueueArgs u{};
+    u.n = P; u.n_rows = qu->ring.n_rows; u.cap = qu->ring.cap; u.delta_t = qu->ring.delta_t; u.rows = qu->rows;
+    u.states = qu->ring.states; u.head = qu->ring.head; u.size = qu->ring.size; u.k_end = qu->k_end;
+    u.G_term = qu->G_term; u.goal_radius = qu->goal_radius; u.status = qu->status; u.goal_seen = qu->goal_seen;
+    FQ_CUDA(fq_launch_pair_queue(q, u, st));
+  }
   if (win)
   {
     FqPairWindowArgs wa;
@@ -519,15 +534,11 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
     wa.next_init_w = sw[0].next_init; wa.next_final_w = sw[0].next_final;
     wa.next_init_s = sw[1].next_init; wa.next_final_s = sw[1].next_final;
     if (hr) { wa.need_safe = sh.hr_need; wa.last_factor_safe = hr->last_factor_safe; }
+    if (qu) wa.gate = qu->status;
     FQ_CUDA(fq_launch_pair_window(wa, st));
   }
   if (pl)
-  { // ---- the plan pieces (appendToPlan, faster.cpp:606-648) from the winners and k_safe
-    FqPairPlanArgs q;
-    q.n_prob = P; q.N_w = sw[0].N; q.N_s = sw[1].N; q.DC = a->DC;
-    q.win_idx_w = ss[0].win_idx; q.win_idx_s = ss[1].win_idx; q.win_dt_w = ss[0].win_dt; q.win_dt_s = ss[1].win_dt;
-    q.n_samples = sh.n_samples; q.k_safe = sh.k_safe; q.need = hr ? sh.hr_need : nullptr;
-    q.coeffs_w = coeffs_w; q.coeffs_s = coeffs_s;
+  { // ---- the plan pieces as rows of the caller's array
     q.cap = pl->cap_states; q.states = pl->states; q.plan_ofs = pl->plan_ofs; q.status = pl->status;
     FQ_CUDA(fq_launch_pair_plan(q, st));
   }
@@ -544,7 +555,7 @@ int run_chain(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
 // of the structs is a device pointer; the sweeps' sizes come from the hints of `as` (capacities) and `win` (factor rows)
 int chain_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex,
               const fq_pair_decomp* dc, fq_pair_result* results_all, void* stream_v, const fq_pair_hr* hr = nullptr,
-              const fq_pair_map* mp = nullptr, const fq_pair_plan* pl = nullptr)
+              const fq_pair_map* mp = nullptr, const fq_pair_plan* pl = nullptr, const fq_pair_queue* qu = nullptr)
 {
   if (!ctx) return FQ_E_ARG;
   if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
@@ -568,11 +579,12 @@ int chain_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, cons
     w.ee_width = (int)longest;
   }
   FQ_CUDA(cudaSetDevice(ctx->device));
-  return run_chain(ctx, a, as, win, ex, dc, hr, mp, pl, sw, results_all, stream_v ? (cudaStream_t)stream_v : ctx->stream);
+  return run_chain(ctx, a, as, win, ex, dc, hr, mp, pl, qu, sw, results_all, stream_v ? (cudaStream_t)stream_v : ctx->stream);
 }
 
 // the chain with the shared lists of `a` (fq_replan_pairs_dev): every pointer of `a` is a device pointer
-int shared_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_result* results_all, void* stream_v, const fq_pair_plan* pl = nullptr)
+int shared_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_result* results_all, void* stream_v, const fq_pair_plan* pl = nullptr,
+               const fq_pair_queue* qu = nullptr)
 {
   if (!ctx) return FQ_E_ARG;
   Sweep sw[2];
@@ -585,7 +597,7 @@ int shared_dev(fq_ctx* ctx, const fq_pair_args* a, fq_pair_result* results_all, 
     w.ee_width = w.n_sig;
   }
   FQ_CUDA(cudaSetDevice(ctx->device));
-  return run_chain(ctx, a, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, pl, sw, results_all,
+  return run_chain(ctx, a, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, pl, qu, sw, results_all,
                    stream_v ? (cudaStream_t)stream_v : ctx->stream);
 }
 
@@ -600,16 +612,53 @@ int check_plan(fq_ctx* ctx, const fq_pair_plan* pl)
   return 0;
 }
 
+// what a ring's struct alone shows wrong (fq_queue_*, fq_replan_pairs_queue*), or nullptr
+const char* queue_struct(const fq_queue* q)
+{
+  if (!q) return "queue is NULL";
+  if (!q->states || !q->head || !q->size) return "queue: states, head and size must not be NULL";
+  if (q->n_rows < 1) return "queue: n_rows < 1";
+  if (q->cap < 1) return "queue: cap < 1";
+  if (q->delta_t < 1) return "queue: delta_t < 1";
+  return nullptr;
+}
+
+// the host entries' row checks: every row named in range, named once (`unique`), and a ring (`ring`)
+const char* queue_rows(const fq_queue* q, int n, const int* rows, bool unique, bool ring)
+{
+  std::vector<char> named((size_t)q->n_rows, 0);
+  for (int j = 0; j < n; j++)
+  {
+    const int r = rows ? rows[j] : j;
+    if (r < 0 || r >= q->n_rows) return "queue: a row outside 0 .. n_rows-1";
+    if (unique && named[(size_t)r]) return "queue: a row named twice";
+    named[(size_t)r] = 1;
+    if (ring && !fqq::ring_ok(q->head[r], q->size[r], q->cap)) return "queue: an invalid row (head outside 0 .. cap-1 or size outside 0 .. cap)";
+  }
+  return nullptr;
+}
+
+// the queue's own refusals (fq_replan_pairs_queue*)
+int check_queue(fq_ctx* ctx, const fq_pair_queue* qu)
+{
+  if (!qu) return fq_fail(ctx, FQ_E_ARG, "queue is NULL");
+  if (const char* why = queue_struct(&qu->ring)) return fq_fail(ctx, FQ_E_ARG, why);
+  if (!qu->k_end || !qu->status) return fq_fail(ctx, FQ_E_ARG, "queue: k_end and status must not be NULL");
+  if (ctx->is_group || ctx->comm)
+    return fq_fail(ctx, FQ_E_ARG, "fq_replan_pairs_queue: multi-GPU contexts are not supported");
+  return 0;
+}
+
 // The device chain the non-NULL structs select (fq_replan_pairs_plan*; the same dispatch as the host entries): the shared
 // lists without assign, else _map, _hr, _decomp, _exact, _window or _assign, each with its own family's checks.
 int family_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex,
                const fq_pair_decomp* dc, const fq_pair_hr* hr, const fq_pair_map* mp, const fq_pair_plan* pl,
-               fq_pair_result* results_all, void* stream_v)
+               fq_pair_result* results_all, void* stream_v, const fq_pair_queue* qu = nullptr)
 {
   if (!as)
   {
     if (win || ex || dc || hr || mp) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
-    return shared_dev(ctx, a, results_all, stream_v, pl);
+    return shared_dev(ctx, a, results_all, stream_v, pl, qu);
   }
   if (mp)
   {
@@ -619,7 +668,7 @@ int family_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, con
   {
     if (int rc = check_hr(ctx, win, dc, hr)) return rc;
   }
-  return chain_dev(ctx, a, as, win, ex, dc, results_all, stream_v, hr, mp, pl);
+  return chain_dev(ctx, a, as, win, ex, dc, results_all, stream_v, hr, mp, pl, qu);
 }
 }  // namespace
 
@@ -635,6 +684,99 @@ extern "C" int fq_replan_pairs_plan_dev(fq_ctx* ctx, const fq_pair_args* a, cons
   if (!ctx) return FQ_E_ARG;
   if (int rc = check_plan(ctx, pl)) return rc;
   return family_dev(ctx, a, as, win, ex, dc, hr, mp, pl, results_all, stream_v);
+}
+
+extern "C" int fq_replan_pairs_queue_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
+                                         const fq_pair_exact* ex, const fq_pair_decomp* dc, const fq_pair_hr* hr, const fq_pair_map* mp,
+                                         const fq_pair_queue* qu, fq_pair_result* results_all, void* stream_v)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (int rc = check_queue(ctx, qu)) return rc;
+  return family_dev(ctx, a, as, win, ex, dc, hr, mp, nullptr, results_all, stream_v, qu);
+}
+
+namespace
+{
+// the FqQueueArgs of a small ring kernel
+FqQueueArgs queue_args(const fq_queue* q, int n, const int* rows)
+{
+  FqQueueArgs u{};
+  u.n = n; u.n_rows = q->n_rows; u.cap = q->cap; u.delta_t = q->delta_t; u.rows = rows;
+  u.states = q->states; u.head = q->head; u.size = q->size;
+  return u;
+}
+
+int queue_launched(cudaError_t e) { return e == cudaSuccess ? 0 : fq_cuda_fail(nullptr, e, "fq_queue_*_dev launch"); }
+}  // namespace
+
+extern "C" int fq_queue_reset(const fq_queue* q, int n, const int* rows, const double* pos)
+{
+  if (const char* why = queue_struct(q)) return fq_fail(nullptr, FQ_E_ARG, why);
+  if (n < 0 || (n > 0 && !pos)) return fq_fail(nullptr, FQ_E_ARG, "queue: n < 0, or pos NULL");
+  if (const char* why = queue_rows(q, n, rows, true, false)) return fq_fail(nullptr, FQ_E_ARG, why);
+  for (int j = 0; j < n; j++)
+  {
+    const int r = rows ? rows[j] : j;
+    fqq::reset(q->states + (size_t)r * q->cap * fqq::kState, q->head + r, q->size + r, pos + 3 * (size_t)j);
+  }
+  return 0;
+}
+
+extern "C" int fq_queue_select(const fq_queue* q, int n, const int* rows, double* x0, int* k_end)
+{
+  if (const char* why = queue_struct(q)) return fq_fail(nullptr, FQ_E_ARG, why);
+  if (n < 0 || (n > 0 && (!x0 || !k_end))) return fq_fail(nullptr, FQ_E_ARG, "queue: n < 0, or x0 or k_end NULL");
+  if (const char* why = queue_rows(q, n, rows, false, true)) return fq_fail(nullptr, FQ_E_ARG, why);
+  for (int j = 0; j < n; j++)
+  {
+    const int r = rows ? rows[j] : j;
+    k_end[j] = fqq::select(q->states + (size_t)r * q->cap * fqq::kState, q->head[r], q->size[r], q->cap, q->delta_t, x0 + 9 * (size_t)j);
+  }
+  return 0;
+}
+
+extern "C" int fq_queue_pop(const fq_queue* q, int n, const int* rows, const int* ticks, int max_ticks, double* goals)
+{
+  if (const char* why = queue_struct(q)) return fq_fail(nullptr, FQ_E_ARG, why);
+  if (n < 0 || max_ticks < 0 || (n > 0 && (!ticks || (max_ticks > 0 && !goals))))
+    return fq_fail(nullptr, FQ_E_ARG, "queue: n < 0, max_ticks < 0, or ticks or goals NULL");
+  if (const char* why = queue_rows(q, n, rows, true, true)) return fq_fail(nullptr, FQ_E_ARG, why);
+  for (int j = 0; j < n; j++)
+  {
+    const int r = rows ? rows[j] : j;
+    const int t = ticks[j] < 0 ? 0 : std::min(ticks[j], max_ticks);
+    fqq::pop(q->states + (size_t)r * q->cap * fqq::kState, q->head + r, q->size + r, q->cap, t,
+             goals + (size_t)j * max_ticks * fqq::kState);
+  }
+  return 0;
+}
+
+extern "C" int fq_queue_reset_dev(const fq_queue* q, int n, const int* rows, const double* pos, void* stream)
+{
+  if (const char* why = queue_struct(q)) return fq_fail(nullptr, FQ_E_ARG, why);
+  if (n < 0 || (n > 0 && !pos)) return fq_fail(nullptr, FQ_E_ARG, "queue: n < 0, or pos NULL");
+  FqQueueArgs u = queue_args(q, n, rows);
+  u.pos = pos;
+  return queue_launched(fq_launch_queue_reset(u, (cudaStream_t)stream));
+}
+
+extern "C" int fq_queue_select_dev(const fq_queue* q, int n, const int* rows, double* x0, int* k_end, void* stream)
+{
+  if (const char* why = queue_struct(q)) return fq_fail(nullptr, FQ_E_ARG, why);
+  if (n < 0 || (n > 0 && (!x0 || !k_end))) return fq_fail(nullptr, FQ_E_ARG, "queue: n < 0, or x0 or k_end NULL");
+  FqQueueArgs u = queue_args(q, n, rows);
+  u.x0 = x0; u.k_end = k_end;
+  return queue_launched(fq_launch_queue_select(u, (cudaStream_t)stream));
+}
+
+extern "C" int fq_queue_pop_dev(const fq_queue* q, int n, const int* rows, const int* ticks, int max_ticks, double* goals, void* stream)
+{
+  if (const char* why = queue_struct(q)) return fq_fail(nullptr, FQ_E_ARG, why);
+  if (n < 0 || max_ticks < 0 || (n > 0 && (!ticks || (max_ticks > 0 && !goals))))
+    return fq_fail(nullptr, FQ_E_ARG, "queue: n < 0, max_ticks < 0, or ticks or goals NULL");
+  FqQueueArgs u = queue_args(q, n, rows);
+  u.ticks = ticks; u.max_ticks = max_ticks; u.goals = goals;
+  return queue_launched(fq_launch_queue_pop(u, (cudaStream_t)stream));
 }
 
 extern "C" int fq_replan_pairs_assign_dev(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, fq_pair_result* results_all,
@@ -820,7 +962,7 @@ int check_host(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, con
 // copy_results = false leaves the caller's `results` untouched (the sharded chain reads the all-gathered table instead).
 int submit_host(fq_ctx* ctx, const Checked& k, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results,
                 const fq_pair_assign* as, const fq_pair_window* win, const fq_pair_exact* ex, const fq_pair_decomp* dc,
-                const fq_pair_hr* hr, const fq_pair_map* mp, const fq_pair_plan* pl = nullptr)
+                const fq_pair_hr* hr, const fq_pair_map* mp, const fq_pair_plan* pl = nullptr, const fq_pair_queue* qu = nullptr)
 {
   const int P = a->n_prob, n_unk = k.n_unk;
   const Sweep* sw = k.sw;
@@ -838,6 +980,8 @@ int submit_host(fq_ctx* ctx, const Checked& k, const fq_pair_args* a, bool defer
   fq_pair_hr dh = hr ? *hr : fq_pair_hr{};
   fq_pair_map dm = mp ? *mp : fq_pair_map{};
   fq_pair_plan dp = pl ? *pl : fq_pair_plan{};
+  fq_pair_queue du = qu ? *qu : fq_pair_queue{};
+  const size_t ring_n = qu ? (size_t)qu->ring.n_rows * qu->ring.cap * fqq::kState : 0;
   if (as) da.all_limit = as->all_limit;
   Sweep dv[2];
   FqPack pi, po;
@@ -870,6 +1014,13 @@ int submit_host(fq_ctx* ctx, const Checked& k, const fq_pair_args* a, bool defer
       dp.states = po.out(pl->states, 12 * (size_t)pl->cap_states);
       dp.plan_ofs = po.out(pl->plan_ofs, P + 1);  dp.status = po.out(pl->status, P);
     }
+    if (qu)
+    { // the rings and k_end are updated in their uploaded copies, which go back to the caller's arrays
+      du.ring.states = pi.in(qu->ring.states, ring_n);
+      du.ring.head = pi.in(qu->ring.head, qu->ring.n_rows);  du.ring.size = pi.in(qu->ring.size, qu->ring.n_rows);
+      du.rows = pi.in(qu->rows, P);  du.k_end = pi.in(qu->k_end, P);  du.G_term = pi.in(qu->G_term, 3 * (size_t)P);
+      du.status = po.out(qu->status, P);  du.goal_seen = po.out(qu->goal_seen, P);
+    }
     for (int i = 0; i < 2; i++)
     {
       const Sweep& w = sw[i];
@@ -894,7 +1045,7 @@ int submit_host(fq_ctx* ctx, const Checked& k, const fq_pair_args* a, bool defer
   FQ_CUDA(cudaMemcpyAsync(pi.base, pi.host, pi.at, cudaMemcpyHostToDevice, st));
   for (int i = 0; i < 2; i++) put_sweep(dv[i], i, &d, &da, &dw, &dx, &dd);
   int rc = family_dev(ctx, &d, as ? &da : nullptr, win ? &dw : nullptr, ex ? &dx : nullptr, dc ? &dd : nullptr, hr ? &dh : nullptr,
-                      mp ? &dm : nullptr, pl ? &dp : nullptr, nullptr, st);
+                      mp ? &dm : nullptr, pl ? &dp : nullptr, nullptr, st, qu ? &du : nullptr);
   if (rc) return rc;
   // ---- results straight into the caller's arrays (asynchronous when they are pinned).  The caller's window arrays were
   //      copied into the upload above, so the next_* outputs may alias them.
@@ -919,6 +1070,14 @@ int submit_host(fq_ctx* ctx, const Checked& k, const fq_pair_args* a, bool defer
     if (deferred && pl->cap_states > 0)      // the rows' total is not known yet: all cap_states rows
       FQ_CUDA(cudaMemcpyAsync(pl->states, dp.states, sizeof(double) * 12 * (size_t)pl->cap_states, cudaMemcpyDeviceToHost, st));
   }
+  if (qu)
+  {
+    FQ_CUDA(cudaMemcpyAsync(qu->ring.states, du.ring.states, sizeof(double) * ring_n, cudaMemcpyDeviceToHost, st));
+    FQ_CUDA(cudaMemcpyAsync(qu->ring.size, du.ring.size, sizeof(int) * (size_t)qu->ring.n_rows, cudaMemcpyDeviceToHost, st));
+    FQ_CUDA(cudaMemcpyAsync(qu->k_end, du.k_end, sizeof(int) * (size_t)P, cudaMemcpyDeviceToHost, st));
+    FQ_CUDA(cudaMemcpyAsync(qu->status, du.status, sizeof(int) * (size_t)P, cudaMemcpyDeviceToHost, st));
+    if (qu->goal_seen) FQ_CUDA(cudaMemcpyAsync(qu->goal_seen, du.goal_seen, (size_t)P, cudaMemcpyDeviceToHost, st));
+  }
   if (deferred) { ctx->pending = true; return 0; }
   FQ_CUDA(cudaStreamSynchronize(st));
   if (pl)
@@ -940,13 +1099,15 @@ int submit_host(fq_ctx* ctx, const Checked& k, const fq_pair_args* a, bool defer
 int host_chain(fq_ctx* ctx, const fq_pair_args* a, bool deferred, fq_pair_result** d_results, bool copy_results,
                const fq_pair_assign* as = nullptr, const fq_pair_window* win = nullptr, const fq_pair_exact* ex = nullptr,
                const fq_pair_decomp* dc = nullptr, const fq_pair_hr* hr = nullptr, const fq_pair_map* mp = nullptr,
-               const fq_pair_plan* pl = nullptr)
+               const fq_pair_plan* pl = nullptr, const fq_pair_queue* qu = nullptr)
 {
   if (!ctx) return FQ_E_ARG;
   if (int rc = fq_settle(ctx)) return rc;
   Checked k;
   if (int rc = check_host(ctx, a, as, win, ex, dc, hr, mp, &k)) return rc;
-  return submit_host(ctx, k, a, deferred, d_results, copy_results, as, win, ex, dc, hr, mp, pl);
+  if (qu)
+    if (const char* why = queue_rows(&qu->ring, a->n_prob, qu->rows, true, true)) return fq_fail(ctx, FQ_E_ARG, why);
+  return submit_host(ctx, k, a, deferred, d_results, copy_results, as, win, ex, dc, hr, mp, pl, qu);
 }
 
 // checked sweep w cut to the corridors [lo, hi) (ofs: its candidate offsets, empty with a shared list): corridor offsets
@@ -1081,30 +1242,32 @@ namespace
 // exchange besides the records'.
 int lists_host(fq_ctx* ctx, const fq_pair_args* a, bool deferred, const fq_pair_assign* as, const fq_pair_window* win,
                const fq_pair_exact* ex = nullptr, const fq_pair_decomp* dc = nullptr, const fq_pair_hr* hr = nullptr,
-               const fq_pair_map* mp = nullptr, const fq_pair_plan* pl = nullptr)
+               const fq_pair_map* mp = nullptr, const fq_pair_plan* pl = nullptr, const fq_pair_queue* qu = nullptr)
 {
   if (!as) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
   if ((ex || dc) && (ctx->is_group || ctx->comm))
     return fq_fail(ctx, FQ_E_ARG, "fq_replan_pairs_exact / _decomp / _hr / _map: multi-GPU contexts are not supported (use the _dev entry)");
   if (ctx->is_group || ctx->comm) return sharded_chain(ctx, a, deferred, as, win);
-  return host_chain(ctx, a, deferred, nullptr, true, as, win, ex, dc, hr, mp, pl);
+  return host_chain(ctx, a, deferred, nullptr, true, as, win, ex, dc, hr, mp, pl, qu);
 }
 
 // fq_replan_pairs_plan / _async: the plan's refusals (multi-GPU contexts among them, so nothing here is sharded), then the
 // host entry of the family the structs select, with its own checks in its own order
+// (fq_replan_pairs_queue / _async: the same with the queue's refusals instead of the plan's)
 int plan_host(fq_ctx* ctx, const fq_pair_args* a, bool deferred, const fq_pair_assign* as, const fq_pair_window* win,
-              const fq_pair_exact* ex, const fq_pair_decomp* dc, const fq_pair_hr* hr, const fq_pair_map* mp, const fq_pair_plan* pl)
+              const fq_pair_exact* ex, const fq_pair_decomp* dc, const fq_pair_hr* hr, const fq_pair_map* mp, const fq_pair_plan* pl,
+              const fq_pair_queue* qu = nullptr)
 {
   if (!ctx) return FQ_E_ARG;
-  if (int rc = check_plan(ctx, pl)) return rc;
+  if (int rc = qu ? check_queue(ctx, qu) : check_plan(ctx, pl)) return rc;
   if (!as)
   {
     if (win || ex || dc || hr || mp) return fq_fail(ctx, FQ_E_ARG, "assign is NULL");
-    return host_chain(ctx, a, deferred, nullptr, true, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, pl);
+    return host_chain(ctx, a, deferred, nullptr, true, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, pl, qu);
   }
   if (hr && !mp)
     if (int rc = check_hr(ctx, win, dc, hr)) return rc;
-  return lists_host(ctx, a, deferred, as, win, ex, dc, hr, mp, pl);
+  return lists_host(ctx, a, deferred, as, win, ex, dc, hr, mp, pl, qu);
 }
 }  // namespace
 
@@ -1119,6 +1282,23 @@ extern "C" int fq_replan_pairs_plan_async(fq_ctx* ctx, const fq_pair_args* a, co
                                           const fq_pair_map* mp, const fq_pair_plan* pl)
 {
   return plan_host(ctx, a, true, as, win, ex, dc, hr, mp, pl);
+}
+
+extern "C" int fq_replan_pairs_queue(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
+                                     const fq_pair_exact* ex, const fq_pair_decomp* dc, const fq_pair_hr* hr, const fq_pair_map* mp,
+                                     const fq_pair_queue* qu)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (int rc = check_queue(ctx, qu)) return rc;
+  return plan_host(ctx, a, false, as, win, ex, dc, hr, mp, nullptr, qu);
+}
+extern "C" int fq_replan_pairs_queue_async(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as, const fq_pair_window* win,
+                                           const fq_pair_exact* ex, const fq_pair_decomp* dc, const fq_pair_hr* hr,
+                                           const fq_pair_map* mp, const fq_pair_queue* qu)
+{
+  if (!ctx) return FQ_E_ARG;
+  if (int rc = check_queue(ctx, qu)) return rc;
+  return plan_host(ctx, a, true, as, win, ex, dc, hr, mp, nullptr, qu);
 }
 
 extern "C" int fq_replan_pairs_assign(fq_ctx* ctx, const fq_pair_args* a, const fq_pair_assign* as)

@@ -12,8 +12,9 @@
 // Next window (faster.cpp:582-588), applied only when BOTH sweeps of the replan have a winner; otherwise Faster::replan
 // returns before the update (:420-424, :529-533) and the window stays as it was:
 //     init  = max(f* - gamma, 1.0)        final = f* + gammap
-// appendToPlan's early return (:548) depends on the planner's state and is not modelled: a caller whose plan could not
-// be appended keeps its previous windows itself.
+// appendToPlan's early return (:548) depends on the planner's plan_ deque: fq_replan_pairs_queue* keeps it on the device and
+// gates the update on it (FqPairWindowArgs::gate); with the other families a caller whose plan could not be appended keeps
+// its previous windows itself.
 #pragma once
 #include "fq_dtinit.h"
 

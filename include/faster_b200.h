@@ -48,7 +48,7 @@ typedef struct fq_ctx fq_ctx;     /* opaque: device, stream, plan tables, scratc
 int fq_abi_version(void);
 /* 1 if this build has the named feature: "sweep_early_exit", "replan_pairs", "multi_gpu", "row_tol", "certificates",
  * "replan_pairs_assign", "replan_pairs_window", "replan_pairs_exact", "replan_pairs_decomp", "replan_pairs_hr",
- * "replan_pairs_map", "replan_pairs_plan", "map_paths". */
+ * "replan_pairs_map", "replan_pairs_plan", "map_paths", "replan_pairs_queue". */
 int fq_has_feature(const char* name);
 
 /* Threading: a context is used from one thread at a time, like a SolverGurobi instance in the reference (one replan
@@ -303,7 +303,8 @@ int fq_replan_pairs_assign_dev(fq_ctx* ctx, const fq_pair_args* args, const fq_p
  *   next_*[j]    the window of the next replan: if both sweeps won, max(f*_w - gamma_whole, 1.0) and f*_w + gammap_whole
  *                (and likewise for safe); otherwise the input window unchanged, since replan() returns before its update
  *                (faster.cpp:420-424, :529-533).  appendToPlan's early return (:548) depends on the planner's plan_ deque
- *                and is not modelled; the states appendToPlan pushes are (fq_replan_pairs_plan below).
+ *                and is not modelled; the states appendToPlan pushes are (fq_replan_pairs_plan below), and with the deque
+ *                on the device the early return is too (fq_replan_pairs_queue below).
  * fq_pair_args is used as for fq_replan_pairs_assign except that factors_* must be NULL and n_fac_* 0 (FQ_E_ARG otherwise);
  * `assign` is required.  Feature "replan_pairs_window". */
 typedef struct fq_pair_window
@@ -717,6 +718,99 @@ int fq_replan_pairs_plan_async(fq_ctx* ctx, const fq_pair_args* args, const fq_p
 int fq_replan_pairs_plan_dev(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
                              const fq_pair_exact* exact, const fq_pair_decomp* decomp, const fq_pair_hr* hr, const fq_pair_map* map,
                              const fq_pair_plan* plan, fq_pair_result* results_all, void* stream);
+
+/* ---- each planner's committed plan, kept on the device ----------------------------------------------------------------
+ *
+ * Faster keeps its committed plan in a deque (plan_, faster.hpp:70) from one replan to the next: replan() takes A from it,
+ * appendToPlan replaces its tail with the new piece, and getNextGoal publishes its front on its own timer.  The entries
+ * below keep that deque for every planner in caller-owned ring arrays, so a batch planner's loop needs only A back on the
+ * host (for JPS).  Feature "replan_pairs_queue".
+ *
+ * Ring: n_rows rows of cap states (12 doubles each, fq_fill_x's layout: pos vel accel jerk).  Row r holds size[r] states,
+ * and its i-th state (0 = front) is states[(r * cap + (head[r] + i) % cap) * 12 ..].  A row is valid when 0 <= head < cap
+ * and 0 <= size <= cap.  Corridor (planner) j of a call works on row rows[j], or row j when rows is NULL, so a caller can
+ * submit only its active planners.  GOAL_REACHED / YAWING gating, yaw and the G projection stay with the caller.
+ *
+ * The host entries take HOST pointers and refuse (FQ_E_ARG, text in fq_last_error(NULL)): q or a required array NULL,
+ * n < 0, n_rows < 1, cap < 1, delta_t < 1, a row outside 0 .. n_rows-1 or named twice, and an invalid row named.  They are
+ * pure host code.  The _dev entries take DEVICE arrays (the struct lives on the host), are stream-ordered on `stream` of
+ * the current device (NULL: the legacy default stream) and never synchronise.  They refuse what the struct alone shows;
+ * a corridor whose row is out of range, named twice or invalid is skipped: select gives it k_end = -1 and a NaN x0, pop
+ * gives it NaN goals, reset leaves the row as it was.  Except: select only reads the rings, so fq_queue_select and
+ * fq_queue_select_dev accept a row named by several corridors and give each of them the row's A and k_end (an invalid or
+ * out-of-range row is still refused on the host and skipped on the device); reset does not read head and size, so it
+ * accepts an invalid row and makes it a ring. */
+typedef struct fq_queue
+{
+  double* states;   /* n_rows x cap x 12                                                                              */
+  int* head;        /* n_rows: slot of the front state                                                                */
+  int* size;        /* n_rows: states held                                                                            */
+  int n_rows;
+  int cap;          /* states per row, >= 1                                                                           */
+  int delta_t;      /* deltaT_ (faster.hpp:131: 10), >= 1                                                             */
+} fq_queue;
+
+/* updateState's first push (faster.cpp:253-266): row rows[j] := [the state with pos = pos[j] (n x 3), the rest 0]. */
+int fq_queue_reset(const fq_queue* q, int n, const int* rows, const double* pos);
+int fq_queue_reset_dev(const fq_queue* q, int n, const int* rows, const double* pos, void* stream);
+/* Choosing A (faster.cpp:350-352): k_end[j] = max(size - delta_t, 0) and x0[j] (n x 9) = pos, vel, accel of the row's
+ * state size - 1 - k_end[j].  An empty row gives k_end = -1 and a NaN x0, so that corridor's sweeps have no winner.  x0
+ * is fq_pair_args.x0 of the next replan, and the one array a caller reads back (for host JPS from A.pos). */
+int fq_queue_select(const fq_queue* q, int n, const int* rows, double* x0, int* k_end);
+int fq_queue_select_dev(const fq_queue* q, int n, const int* rows, double* x0, int* k_end, void* stream);
+/* getNextGoal (faster.cpp:699-723) called ticks[j] times (clamped to 0 .. max_ticks): goal t of corridor j, goals[(j *
+ * max_ticks + t) * 12 ..], is the row's front, which is then popped while the row holds more than one state.  Slots past
+ * ticks[j] are not written.  Yaw is not computed. */
+int fq_queue_pop(const fq_queue* q, int n, const int* rows, const int* ticks, int max_ticks, double* goals);
+int fq_queue_pop_dev(const fq_queue* q, int n, const int* rows, const int* ticks, int max_ticks, double* goals, void* stream);
+
+/* The chained replan that appends each corridor's piece to its row, as appendToPlan does (faster.cpp:548-551, :606-648).
+ * The chain is chosen by the structs given, with the rules of fq_replan_pairs_plan, and every output it returns is byte
+ * for byte what fq_replan_pairs_plan returns for the same arguments (args->x0 is fq_queue_select's x0).  Then, per
+ * corridor j on row r = rows[j], with the piece of fq_replan_pairs_plan (k_safe + 1 + n_s states, or none):
+ *   status FQ_QUEUE_NONE: the replan appends nothing (FQ_PLAN_NONE), or k_end[j] < 0 (no select since the last append);
+ *   FQ_QUEUE_PUBLISHED: size[r] - 1 - k_end[j] < 0, with size[r] read when the chain appends, so pops enqueued between the
+ *     select and this call count (delta_t or more of them): "Already published the point A";
+ *   FQ_QUEUE_CAPACITY: size[r] - k_end[j] - 1 + the piece's states > cap, decided for this row alone;
+ *   FQ_QUEUE_ROWS (_dev only): the row is out of range, named by another corridor, or invalid;
+ *   FQ_QUEUE_OK: the last k_end[j] + 1 states are erased and the piece pushed; size[r] changes, head[r] does not.
+ * Only an OK corridor's row changes.  k_end[j] becomes -1 for every corridor (consumed), so a second call without a new
+ * select appends nothing.  goal_seen[j] (if given, with G_term) = 1 when OK and |G_term[j] - the row's last pos| <
+ * goal_radius (faster.cpp:563-572), else 0.
+ * With a window, factor_*, trials_* and last_factor_safe are written as fq_replan_pairs_plan writes them (they are set
+ * inside genNewTraj, before the append), but next_* only for OK corridors: replan() returns before its window update when
+ * the append fails (faster.cpp:548-551), so every other corridor keeps its input window, also when next_* aliases it.
+ * Refused (FQ_E_ARG) besides the family's refusals: q NULL, a NULL ring array, k_end or status NULL, n_rows < 1, cap < 1,
+ * delta_t < 1, multi-GPU contexts, and on the host entries the row checks above. */
+#define FQ_QUEUE_OK 0
+#define FQ_QUEUE_NONE 1        /* nothing appended: no plan piece, or no select                                       */
+#define FQ_QUEUE_PUBLISHED 2   /* the state A was already published                                                    */
+#define FQ_QUEUE_CAPACITY 3    /* the row would exceed cap                                                             */
+#define FQ_QUEUE_ROWS 4        /* the row is out of range, shared with another corridor or invalid (_dev)              */
+typedef struct fq_pair_queue
+{
+  fq_queue ring;            /* in/out                                                                               */
+  const int* rows;          /* n_prob, or NULL: corridor j is row j                                                 */
+  int* k_end;               /* in/out n_prob: fq_queue_select's                                                     */
+  const double* G_term;     /* n_prob x 3, or NULL: no goal_seen                                                    */
+  double goal_radius;       /* par_.goal_radius                                                                     */
+  int* status;              /* out n_prob: FQ_QUEUE_*                                                               */
+  uint8_t* goal_seen;       /* out n_prob, or NULL                                                                  */
+} fq_pair_queue;
+
+/* HOST pointers everywhere; blocks until every output is in the caller's arrays (the whole ring is copied back). */
+int fq_replan_pairs_queue(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
+                          const fq_pair_exact* exact, const fq_pair_decomp* decomp, const fq_pair_hr* hr, const fq_pair_map* map,
+                          const fq_pair_queue* q);
+/* The same, returning once everything is enqueued; outputs are valid after fq_wait(ctx).  Arrays must stay alive. */
+int fq_replan_pairs_queue_async(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
+                                const fq_pair_exact* exact, const fq_pair_decomp* decomp, const fq_pair_hr* hr, const fq_pair_map* map,
+                                const fq_pair_queue* q);
+/* DEVICE pointers everywhere (the structs live on the host), with the hint rules of the selected family's _dev entry.
+ * Never synchronises, so a CUDA graph can capture select, this call and pop together. */
+int fq_replan_pairs_queue_dev(fq_ctx* ctx, const fq_pair_args* args, const fq_pair_assign* assign, const fq_pair_window* window,
+                              const fq_pair_exact* exact, const fq_pair_decomp* decomp, const fq_pair_hr* hr, const fq_pair_map* map,
+                              const fq_pair_queue* q, fq_pair_result* results_all, void* stream);
 
 /* ---- several GPUs behind the boundary (SURVEY.md 8b/8e) ---------------------------------------------------------
  *
