@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libfaster_b200.so")
-SOURCES = ["fq_kernels.cu", "fq_capi.cu", "fq_pair_capi.cu", "fq_map.cu", "fq_paths.cu", "fq_multi.cu", "fq_host.cpp", "fq_decomp.cpp", "fq_jps.cpp"]
+SOURCES = ["fq_kernels.cu", "fq_capi.cu", "fq_pair_capi.cu", "fq_map.cu", "fq_paths.cu", "fq_multi.cu", "fq_host.cpp", "fq_decomp.cpp", "fq_jps.cpp", "fq_jps.cu"]
 PUBLIC_HEADER = os.path.join(HERE, "..", "include", "faster_b200.h")
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC,-O3,-Wall"]

@@ -23,7 +23,8 @@ EXPORTS = ["fq_abi_version", "fq_create", "fq_destroy", "fq_last_error", "fq_set
            "fq_replan_pairs_map", "fq_replan_pairs_map_async", "fq_replan_pairs_map_dev", "fq_replan_pairs_plan",
            "fq_replan_pairs_plan_async", "fq_replan_pairs_plan_dev", "fq_map_paths", "fq_map_paths_dev", "fq_paths_cloud",
            "fq_jps_in", "fq_queue_reset", "fq_queue_reset_dev", "fq_queue_select", "fq_queue_select_dev", "fq_queue_pop",
-           "fq_queue_pop_dev", "fq_replan_pairs_queue", "fq_replan_pairs_queue_async", "fq_replan_pairs_queue_dev"]
+           "fq_queue_pop_dev", "fq_replan_pairs_queue", "fq_replan_pairs_queue_async", "fq_replan_pairs_queue_dev", "fq_jps_batch",
+           "fq_jps_batch_dev", "fq_jps3d_nodes"]
 
 
 class FqError(RuntimeError):
@@ -140,6 +141,23 @@ QUEUE_DELTA_T = 10                                                      # deltaT
 GOAL_RADIUS = 0.3                                                       # faster.yaml:6
 
 
+class JpsGrids(C.Structure):
+    """fq_jps_grids of include/faster_b200.h: every grid the batch JPS plans on; pointers as integers."""
+    _fields_ = [("cells", C.c_void_p), ("cell_ofs", C.c_void_p), ("dims", C.c_void_p), ("origin", C.c_void_p), ("res", C.c_void_p),
+                ("n_grids", C.c_int)]
+
+
+class JpsBatchArgs(C.Structure):
+    """fq_jps_batch_args of include/faster_b200.h; pointers as integers (host or device addresses)."""
+    _fields_ = [("n_prob", C.c_int), ("grids", JpsGrids), ("grid_index", C.c_void_p), ("x0", C.c_void_p), ("goal", C.c_void_p),
+                ("pos", C.c_void_p), ("Ra", C.c_double), ("dist_max", C.c_double), ("use_jps", C.c_int), ("max_nodes", C.c_int),
+                ("max_in", C.c_int), ("in_ofs", C.c_void_p), ("in", C.c_void_p), ("status", C.c_void_p), ("k_end", C.c_void_p)]
+
+
+JPS_OK, JPS_NO_PATH, JPS_NODES, JPS_LONG, JPS_INPUT = 0, 1, 2, 3, 4     # FQ_JPS_*
+JPS_MAX_NODES = 1 << 16                                                 # default per-planner node cap of the bindings
+
+
 HR_OUT_KEYS = ["last_factor_safe", "index_H", "need_safe"]
 HR_DEFAULTS = dict(drone_radius=0.42, delta_a=0.5, delta_H=1.0)         # faster.yaml:7,35,36
 
@@ -241,6 +259,8 @@ def lib():
         L.fq_map_paths.argtypes = [C.POINTER(MapPathsArgs)]
         L.fq_map_paths_dev.argtypes = [C.POINTER(MapPathsArgs), C.c_void_p]
         L.fq_paths_cloud.argtypes = [C.POINTER(MapPathsArgs), C.c_void_p, C.c_void_p]
+        L.fq_jps_batch.argtypes = [C.POINTER(JpsBatchArgs)]
+        L.fq_jps_batch_dev.argtypes = [C.POINTER(JpsBatchArgs), C.c_void_p]
         L.fq_jps_in.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_void_p, C.c_int]
         L.fq_create_multi.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_void_p]
         L.fq_comm_unique_id.argtypes = [C.c_void_p]
@@ -555,6 +575,62 @@ def jps_in(jps, start, goal, ra, dist_max=1.5):
     return out
 
 
+def jps_grids(grids):
+    """Packs a list of (grid int8 [zd, yd, xd], origin (3), res) into the host arrays of fq_jps_grids: dict(cells, cell_ofs,
+    dims, origin, res).  Move them to the device (same keys) for jps_batch_args' device use."""
+    gs = [np.ascontiguousarray(g, np.int8) for g, _, _ in grids]
+    ofs = np.concatenate([[0], np.cumsum([g.size for g in gs])[:-1]]).astype(np.int64)
+    return dict(cells=np.concatenate([g.reshape(-1) for g in gs]), cell_ofs=ofs,
+                dims=np.ascontiguousarray([g.shape[::-1] for g in gs], np.int32),
+                origin=np.ascontiguousarray([_f64(o, 3) for _, o, _ in grids], np.float64),
+                res=np.ascontiguousarray([float(r) for _, _, r in grids], np.float64))
+
+
+def jps_batch_args(n, grids, x0, goal, out, grid_index=None, pos=None, Ra=4.0, dist_max=1.5, use_jps=True,
+                   max_nodes=JPS_MAX_NODES, max_in=512, k_end=None):
+    """JpsBatchArgs over numpy arrays (fq_jps_batch) or device tensors (fq_jps_batch_dev): grids a jps_grids dict, out a dict of
+    in_ofs (n + 1, int32), in (n * max_in x 3, float64) and status (n, int32).  Every array is checked for element type,
+    contiguity and shape (ValueError), since it is read or written in place by address."""
+    ng = len(grids["res"])
+    g = JpsGrids(_addr(grids["cells"], "int8", (None,), "grid cells"), _addr(grids["cell_ofs"], "int64", (ng,), "grid cell_ofs"),
+                 _addr(grids["dims"], "int32", (ng, 3), "grid dims"), _addr(grids["origin"], "float64", (ng, 3), "grid origin"),
+                 _addr(grids["res"], "float64", (ng,), "grid res"), ng)
+    return JpsBatchArgs(int(n), g, _addr(grid_index, "int32", (n,), "grid_index"), _addr(x0, "float64", (n, 9), "x0"),
+                        _addr(goal, "float64", (n, 3), "goal"), _addr(pos, "float64", (n, 3), "pos"), float(Ra), float(dist_max),
+                        int(bool(use_jps)), int(max_nodes), int(max_in), _addr(out["in_ofs"], "int32", (n + 1,), "in_ofs"),
+                        _addr(out["in"], "float64", (n * max_in, 3), "in"), _addr(out["status"], "int32", (n,), "status"),
+                        _addr(k_end, "int32", (n,), "k_end"))
+
+
+def jps_batch(grids, x0, goal, grid_index=None, pos=None, Ra=4.0, dist_max=1.5, use_jps=True, max_nodes=JPS_MAX_NODES, max_in=512,
+              k_end=None):
+    """fq_jps_batch on host arrays: grids a list of (grid [zd, yd, xd], origin, res); x0 (n x 9, or n x 3: A), goal (n x 3).
+    -> dict(in_ofs, in (the rows written), status, k_end (a copy with -1 where status != JPS_OK, or None))."""
+    goal = np.ascontiguousarray(goal, np.float64).reshape(-1, 3)
+    n = len(goal)
+    x0 = np.asarray(x0, np.float64).reshape(n, -1)
+    x0 = np.ascontiguousarray(np.hstack([x0, np.zeros((n, 9 - x0.shape[1]))]) if x0.shape[1] < 9 else x0)
+    gd = jps_grids(grids)
+    gi = None if grid_index is None else np.ascontiguousarray(grid_index, np.int32)
+    pos = None if pos is None else np.ascontiguousarray(pos, np.float64).reshape(n, 3)
+    ke = None if k_end is None else np.array(k_end, np.int32)
+    out = dict(in_ofs=np.zeros(n + 1, np.int32), status=np.full(n, -1, np.int32), **{"in": np.zeros((n * max_in, 3))})
+    a = jps_batch_args(n, gd, x0, goal, out, gi, pos, Ra, dist_max, use_jps, max_nodes, max_in, ke)
+    rc = lib().fq_jps_batch(C.byref(a))
+    if rc != 0:
+        raise FqError("fq_jps_batch failed (%d): %s" % (rc, lib().fq_last_error(None).decode()))
+    out["in"] = out["in"][:out["in_ofs"][-1]].copy()
+    out["k_end"] = ke
+    return out
+
+
+def jps_batch_dev(args, stream=0):
+    """fq_jps_batch_dev: `args` (JpsBatchArgs, jps_batch_args over device tensors)."""
+    rc = lib().fq_jps_batch_dev(C.byref(args), stream or None)
+    if rc != 0:
+        raise FqError("fq_jps_batch_dev failed (%d): %s" % (rc, lib().fq_last_error(None).decode()))
+
+
 def map_paths_args(n_prob, in_ofs, in_, out_ptrs, drone_radius=HR_DEFAULTS["drone_radius"], max_poly_whole=3, max_poly_safe=4,
                    maps=(), map_index=None, max_in=0):
     """MapPathsArgs; in_ofs / in_ / map_index: addresses (map_index None: NULL), out_ptrs: addresses of PATHS_OUT_KEYS
@@ -694,6 +770,20 @@ def jps3d_plan_world(grid, origin, res, start, goal, use_jps=True, cap=4096):
     if n < 0:
         raise FqError("fq_jps3d_plan_world failed (%d)" % n)
     return out[:n].copy(), rc.value
+
+
+def jps3d_nodes(grid, start, goal, use_jps=True):
+    """The number of nodes fq_jps3d_plan's search creates from cell start to cell goal (grid int8 [zd, yd, xd])."""
+    g = np.ascontiguousarray(grid, np.int8)
+    zd, yd, xd = g.shape
+    s, t = np.asarray(start, np.int32).copy(), np.asarray(goal, np.int32).copy()
+    L = lib()
+    L.fq_jps3d_nodes.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int]
+    L.fq_jps3d_nodes.restype = C.c_longlong
+    n = L.fq_jps3d_nodes(g.ctypes.data, xd, yd, zd, s.ctypes.data, t.ctypes.data, int(use_jps))
+    if n < 0:
+        raise FqError("fq_jps3d_nodes failed (%d)" % n)
+    return int(n)
 
 
 def jps3d_rules():

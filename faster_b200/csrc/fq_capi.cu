@@ -146,7 +146,7 @@ extern "C" int fq_has_feature(const char* name)
   if (n == "sweep_early_exit" || n == "replan_pairs" || n == "multi_gpu" || n == "row_tol" || n == "certificates" ||
       n == "replan_pairs_assign" || n == "replan_pairs_window" || n == "replan_pairs_exact" ||
       n == "replan_pairs_decomp" || n == "replan_pairs_hr" || n == "replan_pairs_map" || n == "replan_pairs_plan" || n == "map_paths" ||
-      n == "replan_pairs_queue")
+      n == "replan_pairs_queue" || n == "jps_batch")
     return 1;
   return 0;
 }

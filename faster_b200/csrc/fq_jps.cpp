@@ -1,22 +1,9 @@
 // Host-side path search on a voxel grid: the first input generator of Faster::replan() (jps_manager_.solveJPS3D,
-// faster/src/faster.cpp:361 -> jps_manager.cpp:141 -> thirdparty/jps3d JPSPlanner<3>::plan, jps_planner.cpp:196-295 over
-// GraphSearch, graph_search.cpp:123-219 A* loop, :272-470 jump-point successors).  Written from scratch: jump point
-// search in 3D (26-connected, Euclidean step costs, Euclidean heuristic) plus plain A*, and the reference's path
-// post-processing (removeLinePts / removeCornerPts with ray-traced line-of-sight, jps_planner.cpp:36-105,
-// map_util.h:334-383).  Stays on the host (BASELINE north_star).
-//
-// Cell values follow the reference's map (map_util.h): 0 free, > 0 occupied, < 0 unknown.  Only free cells can be
-// entered; only OCCUPIED cells create forced neighbours (graph_search.cpp:58-66, :420-470).
-//
-// Pruning rules (what the reference tabulates in JPS3DNeib, graph_search.h:104-136; generated here from the geometric
-// rule, checked against the reference's tables in tests/test_jps_cpu.py).  For a move d = a + b + c (axis components):
-//   natural neighbours: every non-empty sub-sum of the components (1, 3 or 7 directions);
-//   forced pairs (blocker f1 -> successor f2):
-//     straight  d:      o -> o + d                       for the 8 offsets o perpendicular to d
-//     planar    a+b:    -b -> a-b,  -a -> b-a,  and for both normals n:  n -> d+n,  -b+n -> a-b+n,  -a+n -> b-a+n,
-//                       n -> a+n,  n -> b+n
-//     spatial   a+b+c:  -a -> d-2a (and cyclic),  -b-c -> a-b-c (and cyclic),  -a -> -a+c, -a -> -a+b (and cyclic)
+// faster/src/faster.cpp:361).  The search, its pruning rules and the path post-processing are fq_jps.h's, shared with the
+// batch kernel (fq_jps.cuh); this file gives them host storage.  Stays on the host (BASELINE north_star); the batch
+// entries fq_jps_batch / _dev run the same code on the GPU.
 #include "../../include/faster_b200.h"
+#include "fq_jps.h"
 
 #include <algorithm>
 #include <cmath>
@@ -26,283 +13,27 @@
 
 namespace
 {
-struct V3i
-{
-  int x, y, z;
-};
-inline V3i operator+(V3i a, V3i b) { return { a.x + b.x, a.y + b.y, a.z + b.z }; }
-inline V3i operator-(V3i a, V3i b) { return { a.x - b.x, a.y - b.y, a.z - b.z }; }
-inline V3i neg(V3i a) { return { -a.x, -a.y, -a.z }; }
-inline int dir_id(V3i d) { return (d.x + 1) + 3 * (d.y + 1) + 9 * (d.z + 1); }
+using fqjps::Grid;
+using fqjps::Node;
+using fqjps::V3i;
+using fqjps::World;
 
-struct Rules
+const fqjps::Rules& rules()
 {
-  // per direction id: natural neighbours, forced (blocker, successor) pairs, and the distinct blockers
-  std::vector<V3i> nat[27];
-  std::vector<std::pair<V3i, V3i>> forced[27];
-  std::vector<V3i> blockers[27];
-  Rules()
-  {
-    for (int dz = -1; dz <= 1; dz++)
-      for (int dy = -1; dy <= 1; dy++)
-        for (int dx = -1; dx <= 1; dx++)
-        {
-          const V3i d = { dx, dy, dz };
-          const int id = dir_id(d);
-          std::vector<V3i> comp;
-          if (dx) comp.push_back({ dx, 0, 0 });
-          if (dy) comp.push_back({ 0, dy, 0 });
-          if (dz) comp.push_back({ 0, 0, dz });
-          const int n = (int)comp.size();
-          if (n == 0)
-          { // start node: all 26 directions
-            for (int z = -1; z <= 1; z++)
-              for (int y = -1; y <= 1; y++)
-                for (int x = -1; x <= 1; x++)
-                  if (x || y || z) nat[id].push_back({ x, y, z });
-            continue;
-          }
-          // natural: single components, then pairs, then the full move (the move itself last: jump() recurses on the
-          // sub-moves first and then continues straight)
-          for (int k = 0; k < n; k++) nat[id].push_back(comp[k]);
-          if (n == 3)
-            for (int k = 0; k < 3; k++) nat[id].push_back(comp[k] + comp[(k + 1) % 3]);
-          if (n >= 2) nat[id].push_back(d);
-          auto add = [&](V3i f1, V3i f2) { forced[id].push_back({ f1, f2 }); };
-          if (n == 1)
-          {
-            for (int z = -1; z <= 1; z++)
-              for (int y = -1; y <= 1; y++)
-                for (int x = -1; x <= 1; x++)
-                {
-                  const V3i o = { x, y, z };
-                  if ((x || y || z) && o.x * d.x + o.y * d.y + o.z * d.z == 0) add(o, o + d);
-                }
-          }
-          else if (n == 2)
-          {
-            const V3i a = comp[0], b = comp[1];
-            const V3i e = { dx == 0 ? 1 : 0, dy == 0 ? 1 : 0, dz == 0 ? 1 : 0 };   // normal of the move's plane
-            add(neg(b), a - b);
-            add(neg(a), b - a);
-            for (int s = -1; s <= 1; s += 2)
-            {
-              const V3i nn = { e.x * s, e.y * s, e.z * s };
-              add(nn, d + nn);
-              add(nn - b, a - b + nn);
-              add(nn - a, b - a + nn);
-              add(nn, a + nn);
-              add(nn, b + nn);
-            }
-          }
-          else
-          {
-            const V3i c[3] = { comp[0], comp[1], comp[2] };
-            for (int k = 0; k < 3; k++) add(neg(c[k]), d - c[k] - c[k]);
-            for (int k = 0; k < 3; k++) add(neg(c[(k + 1) % 3]) - c[(k + 2) % 3], c[k] - c[(k + 1) % 3] - c[(k + 2) % 3]);
-            for (int k = 0; k < 3; k++)
-            {
-              add(neg(c[k]), c[(k + 1) % 3] - c[k]);
-              add(neg(c[k]), c[(k + 2) % 3] - c[k]);
-            }
-          }
-          for (const auto& pr : forced[id])
-          {
-            bool seen = false;
-            for (const V3i& bkr : blockers[id]) seen = seen || (bkr.x == pr.first.x && bkr.y == pr.first.y && bkr.z == pr.first.z);
-            if (!seen) blockers[id].push_back(pr.first);
-          }
-        }
-  }
-};
-const Rules& rules()
-{
-  static const Rules r;
+  static const fqjps::Rules r = [] { fqjps::Rules t; fqjps::rules_build(&t); return t; }();
   return r;
 }
 
-struct Grid
+// Host storage of one search: growing node pool and heap.  The cell -> node index map is as large as the grid (a few
+// hundred thousand cells) while a search touches a few hundred of them: it lives in a per-thread buffer whose entries
+// carry the number of the search that wrote them, so nothing is cleared between searches.
+struct HostStore
 {
-  const int8_t* m;
-  int xd, yd, zd;
-  bool inside(int x, int y, int z) const { return x >= 0 && x < xd && y >= 0 && y < yd && z >= 0 && z < zd; }
-  int id(int x, int y, int z) const { return x + y * xd + z * xd * yd; }
-  bool free_(int x, int y, int z) const { return inside(x, y, z) && m[id(x, y, z)] == 0; }
-  bool occupied(int x, int y, int z) const { return inside(x, y, z) && m[id(x, y, z)] > 0; }
-};
-
-struct Node
-{
-  int x, y, z;
-  V3i dir;
-  int parent;
-  double g, h;
-  int heap_pos;   // -1 not in heap; -2 closed
-};
-
-class Search
-{
-public:
-  // The cell -> node index map is as large as the grid (a few hundred thousand cells) while a search touches a few
-  // hundred of them: it lives in a per-thread buffer whose entries carry the number of the search that wrote them, so
-  // nothing is cleared between searches.
-  Search(const Grid& g, V3i goal) : g_(g), goal_(goal), cell_(scratch().cell), stamp_(scratch().stamp)
-  {
-    const size_t n = g.xd * (size_t)g.yd * g.zd;
-    Scratch& sc = scratch();
-    if (sc.cell.size() < n) { sc.cell.assign(n, -1); sc.stamp.assign(n, 0u); sc.epoch = 0; }
-    if (++sc.epoch == 0) { std::fill(sc.stamp.begin(), sc.stamp.end(), 0u); sc.epoch = 1; }
-    epoch_ = sc.epoch;
-  }
-
-  // priority: smaller f first; equal f (within 1e-6): larger g first (graph_search.h:19-27)
-  bool lower(int a, int b) const
-  {
-    const double fa = n_[a].g + n_[a].h, fb = n_[b].g + n_[b].h;
-    if (fa >= fb - 0.000001 && fa <= fb + 0.000001) return n_[a].g < n_[b].g;
-    return fa > fb;
-  }
-  void up(int i)
-  {
-    while (i > 0)
-    {
-      const int p = (i - 1) / 2;
-      if (!lower(heap_[p], heap_[i])) break;
-      std::swap(heap_[p], heap_[i]);
-      n_[heap_[p]].heap_pos = p; n_[heap_[i]].heap_pos = i;
-      i = p;
-    }
-  }
-  void down(int i)
-  {
-    const int n = (int)heap_.size();
-    for (;;)
-    {
-      int best = i;
-      const int l = 2 * i + 1, r = l + 1;
-      if (l < n && lower(heap_[best], heap_[l])) best = l;
-      if (r < n && lower(heap_[best], heap_[r])) best = r;
-      if (best == i) break;
-      std::swap(heap_[best], heap_[i]);
-      n_[heap_[best]].heap_pos = best; n_[heap_[i]].heap_pos = i;
-      i = best;
-    }
-  }
-  void push(int k) { n_[k].heap_pos = (int)heap_.size(); heap_.push_back(k); up(n_[k].heap_pos); }
-  int pop()
-  {
-    const int k = heap_[0];
-    heap_[0] = heap_.back();
-    n_[heap_[0]].heap_pos = 0;
-    heap_.pop_back();
-    if (!heap_.empty()) down(0);
-    n_[k].heap_pos = -2;
-    return k;
-  }
-  double heur(int x, int y, int z) const
-  {
-    return std::sqrt((double)((x - goal_.x) * (x - goal_.x) + (y - goal_.y) * (y - goal_.y) + (z - goal_.z) * (z - goal_.z)));
-  }
-  int node_at(int x, int y, int z, V3i dir)
-  {
-    const int cid = g_.id(x, y, z);
-    int& c = cell_[cid];
-    if (stamp_[cid] != epoch_)
-    {
-      stamp_[cid] = epoch_;
-      c = (int)n_.size();
-      n_.push_back({ x, y, z, dir, -1, INFINITY, heur(x, y, z), -1 });
-    }
-    return c;
-  }
-  bool has_forced(int x, int y, int z, V3i d) const
-  {
-    for (const V3i& b : rules().blockers[dir_id(d)])
-      if (g_.occupied(x + b.x, y + b.y, z + b.z)) return true;
-    return false;
-  }
-  // advance from (x,y,z) along d until a jump point (goal, forced neighbour, or a sub-move finds one); false if blocked
-  bool jump(int x, int y, int z, V3i d, V3i* out) const
-  {
-    for (;;)
-    {
-      x += d.x; y += d.y; z += d.z;
-      if (!g_.free_(x, y, z)) return false;
-      if ((x == goal_.x && y == goal_.y && z == goal_.z) || has_forced(x, y, z, d)) { *out = { x, y, z }; return true; }
-      const std::vector<V3i>& nat = rules().nat[dir_id(d)];
-      for (size_t k = 0; k + 1 < nat.size(); k++)
-      {
-        V3i tmp;
-        if (jump(x, y, z, nat[k], &tmp)) { *out = { x, y, z }; return true; }
-      }
-    }
-  }
-  void successors(int k, bool use_jps, std::vector<int>* ids, std::vector<double>* costs)
-  {
-    const Node cur = n_[k];
-    if (!use_jps)
-    {
-      for (const V3i& d : rules().nat[dir_id({ 0, 0, 0 })])
-      {
-        const int x = cur.x + d.x, y = cur.y + d.y, z = cur.z + d.z;
-        if (!g_.free_(x, y, z)) continue;
-        ids->push_back(node_at(x, y, z, d));
-        costs->push_back(std::sqrt((double)(d.x * d.x + d.y * d.y + d.z * d.z)));
-      }
-      return;
-    }
-    const int id = dir_id(cur.dir);
-    auto try_dir = [&](V3i d) {
-      V3i jp;
-      if (!jump(cur.x, cur.y, cur.z, d, &jp)) return;
-      ids->push_back(node_at(jp.x, jp.y, jp.z, d));
-      costs->push_back(std::sqrt((double)((jp.x - cur.x) * (jp.x - cur.x) + (jp.y - cur.y) * (jp.y - cur.y) + (jp.z - cur.z) * (jp.z - cur.z))));
-    };
-    for (const V3i& d : rules().nat[id]) try_dir(d);
-    for (const auto& pr : rules().forced[id])
-      if (g_.occupied(cur.x + pr.first.x, cur.y + pr.first.y, cur.z + pr.first.z)) try_dir(pr.second);
-  }
-  // returns the goal node index or -1
-  int run(V3i start, bool use_jps, int max_expand, int* expanded)
-  {
-    const int s = node_at(start.x, start.y, start.z, { 0, 0, 0 });
-    n_[s].g = 0;
-    push(s);
-    int it = 0;
-    std::vector<int> ids;
-    std::vector<double> costs;
-    while (!heap_.empty())
-    {
-      it++;
-      const int k = pop();
-      if (n_[k].x == goal_.x && n_[k].y == goal_.y && n_[k].z == goal_.z) { *expanded = it; return k; }
-      ids.clear(); costs.clear();
-      successors(k, use_jps, &ids, &costs);
-      for (size_t i = 0; i < ids.size(); i++)
-      {
-        Node& c = n_[ids[i]];
-        const double tg = n_[k].g + costs[i];
-        if (!(tg < c.g)) continue;
-        c.parent = k; c.g = tg;
-        if (c.heap_pos >= 0)
-        { // already open: better path, re-derive the arrival direction
-          V3i d = { c.x - n_[k].x, c.y - n_[k].y, c.z - n_[k].z };
-          d = { (d.x > 0) - (d.x < 0), (d.y > 0) - (d.y < 0), (d.z > 0) - (d.z < 0) };
-          c.dir = d;
-          up(c.heap_pos);
-        }
-        else if (c.heap_pos == -1) push(ids[i]);
-      }
-      if (max_expand > 0 && it >= max_expand) break;
-    }
-    *expanded = it;
-    return -1;
-  }
-  const Node& node(int k) const { return n_[k]; }
-
-private:
-  Grid g_;
-  V3i goal_;
+  std::vector<Node> n;
+  std::vector<int> h;
+  std::vector<int>& cell;
+  std::vector<unsigned>& stamp;
+  unsigned epoch;
   struct Scratch
   {
     std::vector<int> cell;
@@ -314,132 +45,96 @@ private:
     static thread_local Scratch s;
     return s;
   }
-  std::vector<int>& cell_;
-  std::vector<unsigned>& stamp_;
-  unsigned epoch_ = 0;
-  std::vector<Node> n_;
-  std::vector<int> heap_;
-};
-
-// ---- world-coordinate helpers (map_util.h:334-383) ------------------------------------------------------------------
-struct World
-{
-  Grid g;
-  double origin[3], res;
-  void to_int(const double* p, int* c) const
+  explicit HostStore(size_t cells) : cell(scratch().cell), stamp(scratch().stamp)
   {
-    for (int i = 0; i < 3; i++) c[i] = (int)std::round((p[i] - origin[i]) / res - 0.5);
+    Scratch& sc = scratch();
+    if (sc.cell.size() < cells) { sc.cell.assign(cells, -1); sc.stamp.assign(cells, 0u); sc.epoch = 0; }
+    if (++sc.epoch == 0) { std::fill(sc.stamp.begin(), sc.stamp.end(), 0u); sc.epoch = 1; }
+    epoch = sc.epoch;
   }
-  void to_float(const int* c, double* p) const
+  Node& node(int k) { return n[(size_t)k]; }
+  int& heap(int i)
   {
-    for (int i = 0; i < 3; i++) p[i] = (c[i] + 0.5) * res + origin[i];
+    if ((size_t)i >= h.size()) h.resize((size_t)i + 1);
+    return h[(size_t)i];
   }
-  // any ray-traced cell between p1 and p2 with value >= 100 (map_util.h:349-383)
-  bool blocked(const double* p1, const double* p2) const
+  int lookup(long long c) const { return stamp[(size_t)c] == epoch ? cell[(size_t)c] : -1; }
+  int add(long long c)
   {
-    double diff[3], mx = 0;
-    for (int i = 0; i < 3; i++) { diff[i] = p2[i] - p1[i]; mx = std::max(mx, std::fabs(diff[i] / res)); }
-    const int max_diff = (int)(mx / 0.8);
-    if (max_diff <= 0) return false;
-    const double s = 1.0 / max_diff;
-    int prev[3] = { -1, -1, -1 };
-    for (int n = 1; n < max_diff; n++)
-    {
-      double pt[3];
-      int c[3];
-      for (int i = 0; i < 3; i++) pt[i] = p1[i] + diff[i] * s * n;
-      to_int(pt, c);
-      if (!g.inside(c[0], c[1], c[2])) break;
-      if (c[0] != prev[0] || c[1] != prev[1] || c[2] != prev[2])
-        if (g.m[g.id(c[0], c[1], c[2])] >= 100) return true;
-      prev[0] = c[0]; prev[1] = c[1]; prev[2] = c[2];
-    }
-    return false;
+    stamp[(size_t)c] = epoch;
+    cell[(size_t)c] = (int)n.size();
+    n.push_back(Node{});
+    return cell[(size_t)c];
   }
 };
 
 typedef std::vector<double> Path;   // xyz triples
-inline double dist3(const double* a, const double* b)
-{
-  return std::sqrt((a[0] - b[0]) * (a[0] - b[0]) + (a[1] - b[1]) * (a[1] - b[1]) + (a[2] - b[2]) * (a[2] - b[2]));
-}
-
-Path remove_line_pts(const Path& p)
-{ // jps_planner.cpp:83-105
-  const size_t n = p.size() / 3;
-  if (n < 3) return p;
-  Path out(p.begin(), p.begin() + 3);
-  for (size_t i = 1; i + 1 < n; i++)
-  {
-    double s = 0;
-    for (int k = 0; k < 3; k++) s += std::fabs((p[3 * (i + 1) + k] - p[3 * i + k]) - (p[3 * i + k] - p[3 * (i - 1) + k]));
-    if (s > 1e-2) out.insert(out.end(), p.begin() + 3 * i, p.begin() + 3 * i + 3);
-  }
-  out.insert(out.end(), p.end() - 3, p.end());
-  return out;
-}
-
-Path remove_corner_pts(const World& w, const Path& p)
-{ // jps_planner.cpp:36-80
-  const size_t n = p.size() / 3;
-  if (n < 2) return p;
-  Path out(p.begin(), p.begin() + 3);
-  const double* prev = &p[0];
-  double cost1 = w.blocked(&p[0], &p[3]) ? INFINITY : dist3(&p[0], &p[3]);
-  for (size_t i = 1; i + 1 < n; i++)
-  {
-    const double* a = &p[3 * i];
-    const double* b = &p[3 * (i + 1)];
-    const double cost2 = w.blocked(a, b) ? INFINITY : dist3(a, b);
-    const double cost3 = w.blocked(prev, b) ? INFINITY : dist3(prev, b);
-    if (cost3 < cost1 + cost2) cost1 = cost3;
-    else
-    {
-      out.insert(out.end(), a, a + 3);
-      cost1 = dist3(a, b);
-      prev = a;
-    }
-  }
-  out.insert(out.end(), p.end() - 3, p.end());
-  return out;
-}
-Path reversed(const Path& p)
-{
-  Path r;
-  for (size_t i = p.size() / 3; i-- > 0;) r.insert(r.end(), p.begin() + 3 * i, p.begin() + 3 * i + 3);
-  return r;
-}
 }  // namespace
 
-extern "C" int fq_jps3d_plan(const int8_t* map, int xd, int yd, int zd, const int* start, const int* goal, int use_jps,
-                             int max_expand, int* path_out, int cap, double* cost, int* n_expanded)
+// fq_jps3d_plan with the number of nodes its search created (*n_nodes, may be NULL)
+static int plan(const int8_t* map, int xd, int yd, int zd, const int* start, const int* goal, int use_jps, int max_expand, int* path_out,
+                int cap, double* cost, int* n_expanded, long long* n_nodes)
 {
+  if (n_nodes) *n_nodes = 0;
   if (!map || xd <= 0 || yd <= 0 || zd <= 0 || !start || !goal) return FQ_E_ARG;
   if (cost) *cost = INFINITY;
   if (n_expanded) *n_expanded = 0;
   const Grid g = { map, xd, yd, zd };
   if (!g.free_(start[0], start[1], start[2]) || !g.free_(goal[0], goal[1], goal[2])) return 0;
-  Search s(g, { goal[0], goal[1], goal[2] });
-  int expanded = 0;
-  const int k = s.run({ start[0], start[1], start[2] }, use_jps != 0, max_expand, &expanded);
-  if (n_expanded) *n_expanded = expanded;
+  const fqjps::Rules& R = rules();
+  HostStore st(xd * (size_t)yd * zd);
+  fqjps::Search<HostStore> s(st, fqjps::v3(goal[0], goal[1], goal[2]));
+  s.start(g, fqjps::v3(start[0], start[1], start[2]));
+  int it = 0, k = -1;
+  while (s.heap_n > 0)
+  {
+    it++;
+    const int cur = s.pop();
+    if (s.is_goal(cur)) { k = cur; break; }
+    const Node c = st.node(cur);
+    for (int i = 0;; i++)
+    {
+      const int d = fqjps::candidate(R, g, c, use_jps != 0, i);
+      if (d < 0) break;
+      V3i jp;
+      double step;
+      if (!fqjps::successor(R, g, s.goal, c, use_jps != 0, d, &jp, &step)) continue;
+      s.relax(cur, s.node_at(g, jp.x, jp.y, jp.z, d), step);
+    }
+    if (max_expand > 0 && it >= max_expand) break;
+  }
+  if (n_expanded) *n_expanded = it;
+  if (n_nodes) *n_nodes = (long long)st.n.size();
   if (k < 0) return 0;
   std::vector<int> chain;
-  for (int i = k; i >= 0; i = s.node(i).parent) chain.push_back(i);
+  for (int i = k; i >= 0; i = st.node(i).parent) chain.push_back(i);
   const int n = (int)chain.size();
   double c = 0;
   for (int i = 0; i < n; i++)
   {
-    const Node& a = s.node(chain[n - 1 - i]);
+    const Node& a = st.node(chain[n - 1 - i]);
     if (path_out && i < cap) { path_out[3 * i] = a.x; path_out[3 * i + 1] = a.y; path_out[3 * i + 2] = a.z; }
     if (i > 0)
     {
-      const Node& b = s.node(chain[n - i]);
+      const Node& b = st.node(chain[n - i]);
       c += std::sqrt((double)((a.x - b.x) * (a.x - b.x) + (a.y - b.y) * (a.y - b.y) + (a.z - b.z) * (a.z - b.z)));
     }
   }
   if (cost) *cost = c;
   return n;
+}
+
+extern "C" int fq_jps3d_plan(const int8_t* map, int xd, int yd, int zd, const int* start, const int* goal, int use_jps,
+                             int max_expand, int* path_out, int cap, double* cost, int* n_expanded)
+{
+  return plan(map, xd, yd, zd, start, goal, use_jps, max_expand, path_out, cap, cost, n_expanded, nullptr);
+}
+
+extern "C" long long fq_jps3d_nodes(const int8_t* map, int xd, int yd, int zd, const int* start, const int* goal, int use_jps)
+{
+  long long n = 0;
+  const int rc = plan(map, xd, yd, zd, start, goal, use_jps, -1, nullptr, 0, nullptr, nullptr, &n);
+  return rc < 0 ? rc : n;
 }
 
 extern "C" int fq_jps3d_plan_world(const int8_t* map, int xd, int yd, int zd, const double* origin, double res,
@@ -448,7 +143,7 @@ extern "C" int fq_jps3d_plan_world(const int8_t* map, int xd, int yd, int zd, co
 {
   if (!map || !origin || !(res > 0) || !start || !goal || !path_out) return FQ_E_ARG;
   World w;
-  w.g = { map, xd, yd, zd };
+  w.g = Grid{ map, xd, yd, zd };
   w.res = res;
   for (int i = 0; i < 3; i++) w.origin[i] = origin[i];
   int s[3], g[3];
@@ -464,12 +159,17 @@ extern "C" int fq_jps3d_plan_world(const int8_t* map, int xd, int yd, int zd, co
     cells.assign((size_t)3 * n, 0);
     n = fq_jps3d_plan(map, xd, yd, zd, s, g, use_jps, -1, cells.data(), n, &c, nullptr);
   }
-  Path raw((size_t)3 * n);
+  Path raw((size_t)3 * n), a((size_t)3 * n), b((size_t)3 * n);
   for (int i = 0; i < n; i++) w.to_float(&cells[3 * i], &raw[3 * i]);
   // jps_planner.cpp:289-293: line points out, corner points out forwards and backwards
-  Path p = remove_corner_pts(w, remove_line_pts(raw));
-  p = reversed(remove_corner_pts(w, reversed(p)));
-  const int m = (int)(p.size() / 3);
+  auto blocked = [&](const double* p1, const double* p2) { return w.blocked(p1, p2); };
+  int m = fqjps::remove_line_pts(raw.data(), n, a.data());
+  m = fqjps::remove_corner_pts(blocked, a.data(), m, b.data(), true);
+  fqjps::reverse_into(b.data(), m, a.data());
+  m = fqjps::remove_corner_pts(blocked, a.data(), m, b.data(), true);
+  fqjps::reverse_into(b.data(), m, a.data());
+  a.resize((size_t)3 * m);
+  const Path& p = a;
   if (m > cap) return FQ_E_NOMEM;
   std::memcpy(path_out, p.data(), sizeof(double) * p.size());
   return m;
@@ -482,20 +182,21 @@ extern "C" void fq_jps3d_rules(int* ns, int* f1, int* f2, int* counts)
   std::memset(ns, 0, sizeof(int) * 27 * 3 * 26);
   std::memset(f1, 0, sizeof(int) * 27 * 3 * 12);
   std::memset(f2, 0, sizeof(int) * 27 * 3 * 12);
+  const fqjps::Rules& R = rules();
   for (int id = 0; id < 27; id++)
   {
-    const auto& nat = rules().nat[id];
-    const auto& fo = rules().forced[id];
-    counts[2 * id] = (int)nat.size();
-    counts[2 * id + 1] = (int)fo.size();
-    for (size_t k = 0; k < nat.size(); k++)
+    counts[2 * id] = R.n_nat[id];
+    counts[2 * id + 1] = R.n_forced[id];
+    for (int k = 0; k < R.n_nat[id]; k++)
     {
-      ns[(id * 3 + 0) * 26 + k] = nat[k].x; ns[(id * 3 + 1) * 26 + k] = nat[k].y; ns[(id * 3 + 2) * 26 + k] = nat[k].z;
+      const V3i d = fqjps::dir_of(R.nat[id][k]);
+      ns[(id * 3 + 0) * 26 + k] = d.x; ns[(id * 3 + 1) * 26 + k] = d.y; ns[(id * 3 + 2) * 26 + k] = d.z;
     }
-    for (size_t k = 0; k < fo.size(); k++)
-    {
-      f1[(id * 3 + 0) * 12 + k] = fo[k].first.x; f1[(id * 3 + 1) * 12 + k] = fo[k].first.y; f1[(id * 3 + 2) * 12 + k] = fo[k].first.z;
-      f2[(id * 3 + 0) * 12 + k] = fo[k].second.x; f2[(id * 3 + 1) * 12 + k] = fo[k].second.y; f2[(id * 3 + 2) * 12 + k] = fo[k].second.z;
-    }
+    for (int k = 0; k < R.n_forced[id]; k++)
+      for (int i = 0; i < 3; i++)
+      {
+        f1[(id * 3 + i) * 12 + k] = R.f1[id][k][i];
+        f2[(id * 3 + i) * 12 + k] = R.f2[id][k][i];
+      }
   }
 }

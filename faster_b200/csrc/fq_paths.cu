@@ -393,64 +393,7 @@ extern "C" int fq_jps_in(const double* jps, int n, const double* start, const do
     if (!std::isfinite(start[k]) || !std::isfinite(goal[k])) return fq_fail(nullptr, FQ_E_ARG, "jps_in: non-finite start or goal");
   if (!std::isfinite(ra)) return fq_fail(nullptr, FQ_E_ARG, "jps_in: ra must be finite");
   if (!std::isfinite(dist_max) || !(dist_max > 0)) return fq_fail(nullptr, FQ_E_ARG, "jps_in: dist_max must be finite and > 0");
-  // solveJPS3D (jps_manager.cpp:143-144, :172-186): start and goal with z = std::max(z, 0.0), forced at the ends
-  const double s[3] = { start[0], start[1], start[2] < 0.0 ? 0.0 : start[2] };
-  const double g[3] = { goal[0], goal[1], goal[2] < 0.0 ? 0.0 : goal[2] };
-  std::vector<double> path(jps, jps + 3 * (size_t)n);
-  if (n == 1) path.resize(6);
-  const size_t last = path.size() / 3 - 1;
-  for (int k = 0; k < 3; k++) { path[k] = s[k]; path[3 * last + k] = g[k]; }
-  // faster.cpp:373-382: getFirstIntersectionWithSphere(JPSk, ra, JPSk[0], &li1, &noPointsOutsideS)
-  const int size = (int)(last + 1);
-  const double c[3] = { path[0], path[1], path[2] };
-  int index = -1;
-  for (int i = 0; i < size && index < 0; i++)
-    if (fqpath::dist3(&path[3 * (size_t)i], c) > ra) index = i;
-  std::vector<double> jin;
-  if (index < 0)
-    jin = path;
-  else
-  {
-    const int li = index == 0 ? 1 : index - 1;
-    double E[3] = { c[0], c[1], c[2] };
-    if (index > 0) fqpath::sphere_point(&path[3 * (size_t)(index - 1)], &path[3 * (size_t)index], ra, c, E);
-    jin.assign(path.begin(), path.begin() + 3 * (li + 1));
-    jin.insert(jin.end(), E, E + 3);
-  }
-  // createMoreVertexes(JPS_in, dist_max) (faster.cpp:80-97): floor(dist / d) vertices on every segment longer than d, each
-  // d past the one before it
-  const int m = (int)(jin.size() / 3);
-  double count = m;
-  for (int j = 0; j + 1 < m; j++)
-  {
-    const double dist = fqpath::dist3(&jin[3 * (size_t)j + 3], &jin[3 * (size_t)j]);
-    if (dist > dist_max) count += std::floor(dist / dist_max);
-  }
-  if (count > (double)(1 << 30)) return fq_fail(nullptr, FQ_E_ARG, "jps_in: more than 2^30 vertices (dist_max too small)");
-  int w = 0;
-  auto emit = [&](const double* v) {
-    if (w < cap) for (int k = 0; k < 3; k++) out[3 * (size_t)w + k] = v[k];
-    w++;
-  };
-  for (int j = 0; j < m; j++)
-  {
-    const double* a = &jin[3 * (size_t)j];
-    emit(a);
-    if (j + 1 == m) break;
-    const double* b = a + 3;
-    double v[3];
-    for (int k = 0; k < 3; k++) v[k] = FQ_SUB(b[k], a[k]);
-    const double sq = FQ_ADD(FQ_ADD(FQ_MUL(v[0], v[0]), FQ_MUL(v[1], v[1])), FQ_MUL(v[2], v[2]));
-    const double dist = std::sqrt(sq);
-    if (!(dist > dist_max)) continue;
-    const int add = (int)std::floor(dist / dist_max);
-    for (int k = 0; k < 3; k++) v[k] = FQ_DIV(v[k], dist);                // (path[j + 1] - path[j]).normalized()
-    double p[3] = { a[0], a[1], a[2] };
-    for (int i = 0; i < add; i++)
-    {
-      for (int k = 0; k < 3; k++) p[k] = FQ_ADD(p[k], FQ_MUL(v[k], dist_max));
-      emit(p);
-    }
-  }
-  return w;
+  const fqpath::JpsIn j(jps, n, start, goal, ra);
+  if (j.count(dist_max) > (double)(1 << 30)) return fq_fail(nullptr, FQ_E_ARG, "jps_in: more than 2^30 vertices (dist_max too small)");
+  return j.write(dist_max, out, cap);
 }

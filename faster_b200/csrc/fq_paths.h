@@ -184,6 +184,79 @@ struct March
   }
 };
 
+// JPS_in from a path of n >= 1 vertices (faster.cpp:361-384), for fq_jps_in and the batch JPS kernel.  Vertex 0 := start
+// and the last vertex := goal, both with z = std::max(z, 0.0) as solveJPS3D forces them (jps_manager.cpp:143-144,
+// :172-186; a one-vertex path becomes [start, goal]); the path up to where it first leaves the sphere of radius ra around
+// vertex 0 (getFirstIntersectionWithSphere, :373-382); then createMoreVertexes(dist_max) (:80-97): floor(dist / d)
+// vertices on every segment longer than d, each d past the one before it.
+struct JpsIn
+{
+  const double* jps;
+  int n, m, li;            // the clipped path is path[0 .. li] ++ [E] (li >= 0), or the whole path (li < 0), m vertices
+  double s[3], g[3], E[3];
+  FQ_HD const double* path(int i) const { return i == 0 ? s : (i == (n < 2 ? 1 : n - 1) ? g : jps + 3 * i); }
+  FQ_HD const double* jin(int i) const { return li >= 0 && i == li + 1 ? E : path(i); }
+
+  FQ_HD JpsIn(const double* p, int count, const double* start, const double* goal, double ra) : jps(p), n(count)
+  {
+    for (int k = 0; k < 3; k++) { s[k] = start[k]; g[k] = goal[k]; }
+    s[2] = start[2] < 0.0 ? 0.0 : start[2];
+    g[2] = goal[2] < 0.0 ? 0.0 : goal[2];
+    const int size = n < 2 ? 2 : n;
+    int index = -1;
+    for (int i = 0; i < size && index < 0; i++)
+      if (dist3(path(i), s) > ra) index = i;
+    li = -1; m = size;
+    if (index >= 0)
+    {
+      li = index == 0 ? 1 : index - 1;
+      for (int k = 0; k < 3; k++) E[k] = s[k];
+      if (index > 0) sphere_point(path(index - 1), path(index), ra, s, E);
+      m = li + 2;
+    }
+  }
+  // the vertex count of createMoreVertexes's output, in double as the host counts it
+  FQ_HD double count(double dist_max) const
+  {
+    double c = m;
+    for (int j = 0; j + 1 < m; j++)
+    {
+      const double d = dist3(jin(j + 1), jin(j));
+      if (d > dist_max) c = FQ_ADD(c, floor(FQ_DIV(d, dist_max)));
+    }
+    return c;
+  }
+  // writes the first min(count, cap) vertices to out; returns the count
+  FQ_HD int write(double dist_max, double* out, int cap) const
+  {
+    int w = 0;
+    auto emit = [&](const double* v) {
+      if (w < cap) for (int k = 0; k < 3; k++) out[3 * (size_t)w + k] = v[k];
+      w++;
+    };
+    for (int j = 0; j < m; j++)
+    {
+      const double* a = jin(j);
+      emit(a);
+      if (j + 1 == m) break;
+      const double* b = jin(j + 1);
+      double v[3];
+      for (int k = 0; k < 3; k++) v[k] = FQ_SUB(b[k], a[k]);
+      const double dist = FQ_SQRT(FQ_ADD(FQ_ADD(FQ_MUL(v[0], v[0]), FQ_MUL(v[1], v[1])), FQ_MUL(v[2], v[2])));
+      if (!(dist > dist_max)) continue;
+      const int add = (int)floor(FQ_DIV(dist, dist_max));
+      for (int k = 0; k < 3; k++) v[k] = FQ_DIV(v[k], dist);             // (path[j + 1] - path[j]).normalized()
+      double p[3] = { a[0], a[1], a[2] };
+      for (int i = 0; i < add; i++)
+      {
+        for (int k = 0; k < 3; k++) p[k] = FQ_ADD(p[k], FQ_MUL(v[k], dist_max));
+        emit(p);
+      }
+    }
+    return w;
+  }
+};
+
 // vertex counts of the outputs: deleteVertexes(path, max_poly) keeps max_poly + 1 vertices (utils.cpp:1117-1124); a
 // corridor without paths (status != 0) gets one vertex of NaN
 FQ_HD int whole_poly(const Crop& c, int n, int max_poly) { return c.status ? 0 : (n - 1 < max_poly ? n - 1 : max_poly); }

@@ -48,7 +48,7 @@ typedef struct fq_ctx fq_ctx;     /* opaque: device, stream, plan tables, scratc
 int fq_abi_version(void);
 /* 1 if this build has the named feature: "sweep_early_exit", "replan_pairs", "multi_gpu", "row_tol", "certificates",
  * "replan_pairs_assign", "replan_pairs_window", "replan_pairs_exact", "replan_pairs_decomp", "replan_pairs_hr",
- * "replan_pairs_map", "replan_pairs_plan", "map_paths", "replan_pairs_queue". */
+ * "replan_pairs_map", "replan_pairs_plan", "map_paths", "replan_pairs_queue", "jps_batch". */
 int fq_has_feature(const char* name);
 
 /* Threading: a context is used from one thread at a time, like a SolverGurobi instance in the reference (one replan
@@ -662,6 +662,64 @@ int fq_paths_cloud(const fq_map_paths_args* p, const int* unk_ofs, const double*
 int fq_jps_in(const double* jps, int n, const double* start, const double* goal, double ra, double dist_max, double* out,
               int cap);
 
+/* ---- every planner's JPS search and JPS_in on the device ----------------------------------------------------------------
+ *
+ * jps_manager_.solveJPS3D(A, G) followed by fq_jps_in (faster.cpp:361-384) for a batch of planners, with fq_jps3d_plan_world's
+ * search and post-processing run on the GPU (one warp per planner), so that a replan cycle -- fq_queue_select_dev, this,
+ * fq_map_paths_dev, fq_replan_pairs_queue_dev, fq_queue_pop_dev -- needs no host step and can be captured as one CUDA
+ * graph.  For planner j: A = x0[j][0..2] and G = goal[j], both with z raised to 0 for the search (jps_manager.cpp:143-144);
+ * ra = min(|G - P| - 0.001, Ra) with P = pos[j] (the drone's state, faster.cpp:327), or A when pos is NULL, the norm in
+ * Eigen's order sqrt((dx^2 + dy^2) + dz^2).  The search runs on grid grid_index[j] (fq_jps3d_plan's map) from cell
+ * to_int(A) to cell to_int(G); the grid is the caller's (no readMap voxelisation, no setFreeVoxelAndSurroundings).
+ * JPS_in is written in fq_map_paths_args' layout (in_ofs from 0, compact rows), so fq_map_paths_dev can read it as it is.
+ * Every output equals, byte for byte, fq_jps3d_plan_world + fq_jps_in on the host, with these statuses:
+ *   FQ_JPS_OK       path found: its JPS_in;                                                           k_end unchanged
+ *   FQ_JPS_NO_PATH  start or goal cell outside the grid or not free, or the search exhausted: fq_jps_in([A], A, G, ra,
+ *                   dist_max), Faster::replan's early return (no append, window kept);                k_end[j] := -1
+ *   FQ_JPS_NODES    the search needed more than max_nodes nodes: one NaN vertex;                      k_end[j] := -1
+ *   FQ_JPS_LONG     JPS_in longer than max_in vertices: one NaN vertex;                               k_end[j] := -1
+ *   FQ_JPS_INPUT    (_dev only) grid_index out of range, a grid with a dimension <= 0, more than 2^31 cells, a res not
+ *                   finite or <= 0 or a non-finite origin, or a non-finite A, G or pos: one NaN vertex; k_end[j] := -1
+ * A single NaN vertex makes fq_map_paths_dev report FQ_PATHS_SHORT, so the chain gives that corridor no winner.
+ * Device scratch per planner: at most 116 max_nodes + 24 max_in + 112 bytes (node pool, heap, a hash of 2 max_nodes cells, two
+ * path buffers, the JPS_in slot), stream-ordered.  Feature "jps_batch". */
+#define FQ_JPS_OK 0
+#define FQ_JPS_NO_PATH 1
+#define FQ_JPS_NODES 2
+#define FQ_JPS_LONG 3
+#define FQ_JPS_INPUT 4
+typedef struct fq_jps_grids {       /* caller-owned, DEVICE arrays for _dev, HOST for fq_jps_batch                           */
+  const int8_t* cells;              /* every grid's cells, x fastest; 0 free, > 0 occupied, < 0 unknown (fq_jps3d_plan's map) */
+  const long long* cell_ofs;        /* n_grids: first cell of grid g                                                        */
+  const int* dims;                  /* n_grids x 3: xd, yd, zd                                                              */
+  const double* origin;             /* n_grids x 3                                                                          */
+  const double* res;                /* n_grids                                                                              */
+  int n_grids;
+} fq_jps_grids;
+typedef struct fq_jps_batch_args {
+  int n_prob;
+  fq_jps_grids grids;
+  const int* grid_index;            /* n_prob, or NULL: every planner plans on grid 0                                       */
+  const double* x0;                 /* n_prob x 9, as fq_queue_select writes it: A = x0[j][0..2]                            */
+  const double* goal;               /* n_prob x 3: G                                                                        */
+  const double* pos;                /* n_prob x 3 or NULL (= A): the state dist_to_goal is measured from                    */
+  double Ra, dist_max;              /* par_.Ra, par_.dist_max_vertexes                                                      */
+  int use_jps;                      /* != 0 JPS (the reference's call), 0 plain A*                                          */
+  int max_nodes, max_in;            /* per-planner caps: 1 .. 2^26 nodes; max_in 2 .. FQ_PATHS_MAX_IN                       */
+  int* in_ofs;                      /* out n_prob + 1: fq_map_paths_args.in_ofs                                             */
+  double* in;                       /* out: fq_map_paths_args.in, room for n_prob x max_in rows                             */
+  int* status;                      /* out n_prob: FQ_JPS_*                                                                 */
+  int* k_end;                       /* in/out n_prob or NULL: set to -1 where status != FQ_JPS_OK                           */
+} fq_jps_batch_args;
+/* HOST pointers; runs on the current device and blocks.  FQ_E_ARG (text in fq_last_error(NULL)): a NULL, n_prob outside
+ * 1..2^24, a NULL required array, n_grids < 1, a dimension <= 0, more than 2^31 cells in a grid, a negative cell_ofs, res
+ * not finite or <= 0, a non-finite origin, Ra not finite, dist_max not finite or <= 0, max_nodes outside 1..2^26, max_in
+ * outside 2..FQ_PATHS_MAX_IN; and, since it can read them, grid_index out of range and a non-finite A, G or pos. */
+int fq_jps_batch(const fq_jps_batch_args* a);
+/* DEVICE pointers; stream-ordered, never synchronises (a CUDA graph can capture it).  The refusals of fq_jps_batch that
+ * read no array; the grids and the per-planner inputs are checked per planner instead (FQ_JPS_INPUT). */
+int fq_jps_batch_dev(const fq_jps_batch_args* a, void* stream);
+
 /* ---- chained replan that returns each corridor's committed plan --------------------------------------------------------
  *
  * What a replan commits is not its coefficients but the states appendToPlan pushes onto the plan (faster.cpp:548,
@@ -898,6 +956,10 @@ int fq_jps3d_plan(const int8_t* map, int xd, int yd, int zd, const int* start, c
  * path_out: up to cap (x,y,z) points.  Returns the number of points, 0 if no path, <0 on error (FQ_E_NOMEM: cap). */
 int fq_jps3d_plan_world(const int8_t* map, int xd, int yd, int zd, const double* origin, double res, const double* start,
                         const double* goal, int use_jps, double* path_out, int cap, double* raw_cost);
+
+/* Introspection (tests): the number of nodes fq_jps3d_plan's search creates for this query (0 when start or goal is not
+ * free), which is what fq_jps_batch's max_nodes bounds; < 0 on error.  Pure host code. */
+long long fq_jps3d_nodes(const int8_t* map, int xd, int yd, int zd, const int* start, const int* goal, int use_jps);
 
 /* Introspection (tests): the pruning rules in the layout of the reference's JPS3DNeib (graph_search.h:104-136):
  * ns[27][3][26], f1[27][3][12], f2[27][3][12], counts[27][2] = (natural, forced) entries per direction id. */
